@@ -2,14 +2,18 @@
 //
 // Operands are int8 digit planes pre-packed in the no-swizzle K-major core-matrix layout (8 rows x 16 bytes per core matrix,
 // K-adjacent core matrices LBO apart, 8-row groups SBO apart), so one pipeline stage is a handful of contiguous 1-D bulk-TMA
-// copies and the wgmma shared-memory descriptors are two 32-bit adds each.  For a row-block of 128 rows of the left factor
-// and a column chunk of CN candidates, level r = p + q (2 <= r <= S + 1) accumulates every digit product d_p(A) d_q(B)
-// exactly in int32:
+// copies and the wgmma shared-memory descriptors of the right operand are 32-bit adds.  For a row-block of 128 rows of the
+// left factor and a column chunk of CN candidates, level r = p + q (2 <= r <= S + 1) accumulates every digit product
+// d_p(A) d_q(B) exactly in int32:
 //        A[n,t] = rowscale[n]·out_scale · Σ_{r=2..S+1} 2^(-8r) T_r[n,t]  +  half_var·rowsum[n]
 // (rowsum = nullptr: no centring term).  The accumulators live in registers: two consumer warpgroups take rows [0, 64) and
-// [64, 128) of the row-block, S levels x CN / 2 int32 registers per thread, which is what bounds CN (48 for S = 5, 32 for
-// S = 6, 64 below); a candidate tile of NTB columns is worked on as NTB / CN chunks.  One producer warp streams the stages
-// through a STAGES-deep mbarrier ring.  The grid is persistent: work item = (candidate tile, chunk, row-block group g),
+// [64, 128) of the row-block, S levels x CN / 2 int32 registers per thread, which is what bounds CN (32 for S = 6, 64 below;
+// the producer warpgroup hands its registers to the consumers with setmaxnreg); a candidate tile of NTB columns is worked
+// on as NTB / CN chunks.  The left operand is register-sourced: per digit plane each warp loads its 16 rows with ldmatrix
+// once and issues that plane's S + 1 - p MMAs against the shared-memory descriptors of the K* planes, so a plane is read
+// from shared memory once instead of once per pair.  Each plane's MMAs are one wgmma group; one group stays in flight while
+// the next plane is loaded, and a stage is released when the last group that reads it has retired.  One lane of the
+// producer warpgroup streams the stages through a STAGES-deep mbarrier ring.  The grid is persistent: work item = (candidate tile, chunk, row-block group g),
 // item = (tile·NCH + chunk)·G + g, CTA c takes items c, c + gridDim.x, ... (co-running CTAs share few candidate tiles, so the
 // K* digits stay in L2; the serpentine row-block assignment gives every group the same cost).
 //   EPI_SUMSQ: partial[g][t] = Σ_{rows n of group g} A[n,t]^2  (variance path)
@@ -52,10 +56,13 @@ using oz::SBO;
 
 constexpr int STAGES = 3;
 constexpr int CONSUMER_WARPS = 8;                     // two warpgroups
-constexpr int THREADS = CONSUMER_WARPS * 32 + 32;     // + the producer warp
+constexpr int THREADS = CONSUMER_WARPS * 32 + 128;    // + the producer warpgroup (setmaxnreg acts on whole warpgroups)
+// per-thread registers after setmaxnreg: 128 · 40 + 256 · 232 = 64512 of the 64K register file, which is also what the
+// launch allocates (168 per thread at __launch_bounds__(384, 1))
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 enum { EPI_SUMSQ = 0, EPI_STORE = 1 };
 
-template <int S> __host__ __device__ constexpr int chunk_cols() { return S >= 6 ? 32 : S == 5 ? 48 : 64; }
+template <int S> __host__ __device__ constexpr int chunk_cols() { return S >= 6 ? 32 : 64; }
 template <int S> __host__ __device__ constexpr int stage_bytes() { return S * (ATILE + chunk_cols<S>() * KST); }
 template <int S> __host__ __device__ constexpr size_t smem_bytes() {  // stages + barriers + per-warp column sums
   return (size_t)STAGES * stage_bytes<S>() + 256 + (size_t)CONSUMER_WARPS * chunk_cols<S>() * sizeof(double);
@@ -68,34 +75,41 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr) {
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D(64 x N, s32) += A(64 x 32, s8) B(N x 32, s8)^T, both operands K-major in shared memory
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// The A fragment of one k32 step of an 8-bit wgmma: the warp's 16 rows x 32 bytes as four 8 x 16-byte core matrices
+// (register j: rows +8 if j is odd, bytes +16 if j >= 2), each 128 contiguous bytes of the no-swizzle layout.
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&a)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3])
+               : "r"(saddr)
+               : "memory");
+}
+
+// D(64 x N, s32) += A(64 x 32, s8) B(N x 32, s8)^T, A from registers, B K-major in shared memory
 #define TB_R4(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3])
-__device__ __forceinline__ void wgmma_s8(uint32_t (&d)[16], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void wgmma_s8(uint32_t (&d)[16], const uint32_t (&a)[4], uint64_t db) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n}\n"
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p;\n}\n"
       : TB_R4(0), TB_R4(4), TB_R4(8), TB_R4(12)
-      : "l"(da), "l"(db), "r"(1));
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
 }
-__device__ __forceinline__ void wgmma_s8(uint32_t (&d)[24], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void wgmma_s8(uint32_t (&d)[32], const uint32_t (&a)[4], uint64_t db) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n48k32.s32.s8.s8 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p;\n}\n"
-      : TB_R4(0), TB_R4(4), TB_R4(8), TB_R4(12), TB_R4(16), TB_R4(20)
-      : "l"(da), "l"(db), "r"(1));
-}
-__device__ __forceinline__ void wgmma_s8(uint32_t (&d)[32], uint64_t da, uint64_t db) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
       "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
-      "%32, %33, p;\n}\n"
+      "{%32,%33,%34,%35}, %36, p;\n}\n"
       : TB_R4(0), TB_R4(4), TB_R4(8), TB_R4(12), TB_R4(16), TB_R4(20), TB_R4(24), TB_R4(28)
-      : "l"(da), "l"(db), "r"(1));
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
 }
 #undef TB_R4
 
@@ -138,9 +152,10 @@ digit_gemm_kernel(const int8_t* __restrict__ AS, const int8_t* __restrict__ BS, 
   for (int i = threadIdx.x; i < CONSUMER_WARPS * CN; i += blockDim.x) colbuf[i / CN][i % CN] = 0.0;
   __syncthreads();
 
-  if (warp == CONSUMER_WARPS) {
+  if (warp >= CONSUMER_WARPS) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == CONSUMER_WARPS && lane == 0) {
       int st = 0;
       uint32_t ph = 0;
       for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
@@ -168,7 +183,10 @@ digit_gemm_kernel(const int8_t* __restrict__ AS, const int8_t* __restrict__ BS, 
   }
 
   // ===================== consumer warpgroups: MMA + epilogue =====================
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2, wq = warp & 3;
+  // ldmatrix row address of this lane: row lane % 8 of core matrix lane / 8 of the warp's 16 rows x 32 bytes (ldmatrix_x4)
+  const uint32_t a_lane = (uint32_t)((wg * 8 + wq * 2 + ((lane >> 3) & 1)) * (int)SBO + (lane >> 4) * (int)LBO + (lane & 7) * 16);
   uint32_t acc[S][NR];
   int st = 0;
   uint32_t ph = 0;
@@ -182,27 +200,38 @@ digit_gemm_kernel(const int8_t* __restrict__ AS, const int8_t* __restrict__ BS, 
       for (int l = 0; l < S; ++l)
 #pragma unroll
         for (int j = 0; j < NR; ++j) acc[l][j] = 0u;
+      fence_acc(acc);
+      int held = -1;  // the previous stage: its last MMA group may still be running
       for (int kc = 0; kc < nk; ++kc) {
         mbar_wait(&full[st], ph);
         const uint32_t base = smem_u32(smem + (size_t)st * STAGE);
-        const uint64_t a0 = smem_desc(base + (uint32_t)wg * 8u * SBO), b0 = smem_desc(base + (uint32_t)(S * ATILE));
-        fence_acc(acc);
-        wgmma_fence();
+        const uint64_t b0 = smem_desc(base + (uint32_t)(S * ATILE));
 #pragma unroll
-        for (int p = 1; p <= S; ++p)
+        for (int p = 1; p <= S; ++p) {
+          uint32_t a[KST / 32][4];
+#pragma unroll
+          for (int kk = 0; kk < KST / 32; ++kk) ldmatrix_x4(a[kk], base + a_lane + (uint32_t)((p - 1) * ATILE + kk * 2 * (int)LBO));
+          // all groups but the last one have retired: the registers of the group before it can be reused, and at the
+          // second plane the previous stage's last group is done, so this warp's reads of that stage are over
+          wgmma_wait<1>();
+          if (p == 2 && held >= 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[held]);
+          }
+          wgmma_fence();
 #pragma unroll
           for (int q = 1; q <= S + 1 - p; ++q)
 #pragma unroll
-            for (int kk = 0; kk < KST / 32; ++kk)
-              wgmma_s8(acc[p + q - 2], a0 + (uint64_t)(((p - 1) * ATILE + kk * 2 * (int)LBO) >> 4),
-                       b0 + (uint64_t)(((q - 1) * BCH + kk * 2 * (int)LBO) >> 4));
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_acc(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[st]);  // this warp's reads of the stage are done
+            for (int kk = 0; kk < KST / 32; ++kk) wgmma_s8(acc[p + q - 2], a[kk], b0 + (uint64_t)(((q - 1) * BCH + kk * 2 * (int)LBO) >> 4));
+          wgmma_commit();
+        }
+        held = st;
         if (++st == STAGES) { st = 0; ph ^= 1; }
       }
+      wgmma_wait<0>();
+      fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[held]);
       // epilogue of the row-block.  Fragment of m64nN: register 4j + e holds row 16 wq + lane/4 (+8 for e >= 2) of the
       // warpgroup's 64, column 8j + 2 (lane % 4) + (e & 1) of the chunk
       const int64_t r0 = (int64_t)I * 128 + wg * 64 + wq * 16 + (lane >> 2), r1 = r0 + 8;

@@ -9,8 +9,8 @@
 //     and falls back to the 6-digit / 21-product kernel otherwise);
 //   * all S levels r = 2..S+1 are accumulated at once: ONE pass per row-block and column chunk, one epilogue;
 //   * fp32 models use S = 3 (6 products): ~5e-6·σ_f² against the 1e-4·σ_f² fp32 bar.
-// The K* digit tiles are NT candidates wide (96 for S = 5, 128 otherwise); the GEMM (digit_gemm.cuh) works on them in
-// column chunks of 48 / 64 candidates, whose S levels of int32 accumulators fit the registers of two consumer warpgroups.
+// The K* digit tiles are NT candidates wide (192 for S = 5, 128 otherwise); the GEMM (digit_gemm.cuh) works on them in
+// column chunks of 64 candidates, whose S levels of int32 accumulators fit the registers of two consumer warpgroups.
 #pragma once
 #include "digit_gemm.cuh"
 #include "kernel_fn.cuh"
@@ -25,7 +25,7 @@ using oz::SBO;
 constexpr double FILL = 0.4975;   // |x̂| bound: the largest 5-digit balanced value is 0.49804
 
 template <int S> struct Geo;
-template <> struct Geo<5> { static constexpr int NT = 96; };
+template <> struct Geo<5> { static constexpr int NT = 192; };
 template <> struct Geo<4> { static constexpr int NT = 128; };
 template <> struct Geo<3> { static constexpr int NT = 128; };
 
