@@ -56,6 +56,14 @@ enum tb_acq {
   TB_ACQ_MES = 6      /* min_value_entropy_search.__call__, entropy.py:193-213: mean over the min-value samples set by
                          tb_acq_set_min_value_samples of −γ·φ(γ)/(2Φ(−γ)) − log Φ(−γ), γ = (y* − mean)/sd; param unused */
 };
+/* OR-ed into `acq` of tb_acq_eval / tb_acq_argmax / tb_acq_maximize: the value (and gradient) is multiplied by the local
+ * penalty set by tb_acq_set_penalization (PenalizedAcquisition, acquisition/function/greedy_batch.py:250-269). */
+#define TB_ACQ_PENALIZED 0x100
+/* local penalisers (greedy_batch.py:315-388) */
+enum tb_penalizer {
+  TB_PEN_SOFT = 1, /* soft_local_penalizer: prod_j Φ((‖x − x_j‖ − radius_j)/scale_j) */
+  TB_PEN_HARD = 2  /* hard_local_penalizer: prod_j ((‖x − x_j‖/(radius_j + scale_j))^−5 + 1)^(−1/5) */
+};
 
 /* ---- errors / build info ------------------------------------------------------------------ */
 const char* tb_last_error(void);
@@ -113,6 +121,16 @@ int tb_acq_argmax(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, v
  * tf.Variable assigned in place; here they are a device array owned by the handle.  samples [S] (the reference holds them
  * as [S,1]), always double, S ≥ 1.  Required before any TB_ACQ_MES evaluation. */
 int tb_acq_set_min_value_samples(tb_gp* gp, const double* samples, int S);
+
+/* local_penalizer.__init__ / update (greedy_batch.py:272-312): the pending points and their exclusion radius
+ * (μ(x_j) − η)/L and scale sqrt(var(x_j))/L, held by the handle for calls with TB_ACQ_PENALIZED.  kind: tb_penalizer;
+ * pending [P,D], radius [P], scale [P]; always double, host or device pointers, P ≥ 1. */
+int tb_acq_set_penalization(tb_gp* gp, int kind, const double* pending, int P, const double* radius, const double* scale);
+
+/* the posterior mean and its gradient, what LocalPenalization's Lipschitz estimate differentiates
+ * (greedy_batch.py:207-217): Xc [M,D] → mean [M] = k(x, X) α + m and grad [M,D] = its derivative in x.  No variance: one
+ * kernel launch per 65,536 points, no GEMM.  Handle dtype, host or device pointers. */
+int tb_gp_mean_gradient(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* grad);
 
 /* _perform_parallel_continuous_optimization (acquisition/optimizer.py:566-697) with one ScipyOptimizerGreenlet per start
  * (:700-745, L-BFGS-B): here P independent projected L-BFGS runs advance together ON THE DEVICE — one batched fused

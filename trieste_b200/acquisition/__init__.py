@@ -19,7 +19,14 @@ from .function import (  # noqa: F401
     lower_confidence_bound,
     probability_below_threshold,
 )
-from .greedy_batch import Fantasizer  # noqa: F401
+from .greedy_batch import (  # noqa: F401
+    Fantasizer,
+    LocalPenalization,
+    PenalizedAcquisition,
+    hard_local_penalizer,
+    local_penalizer,
+    soft_local_penalizer,
+)
 from .interface import (  # noqa: F401
     AcquisitionFunctionBuilder,
     GreedyAcquisitionFunctionBuilder,

@@ -116,6 +116,9 @@ struct tb_gp {
   tb::DevBuf dXspare, dyspare, dLspare, dLinvSpare;  // ping-pong partners of dX / dy / dL / dLinv (tb_gp_append_data)
   tb::DevBuf dMes;              // min-value samples of TB_ACQ_MES (tb_acq_set_min_value_samples)
   int mesS = 0;
+  tb::DevBuf dPen;              // local penalisation (tb_acq_set_penalization): pending [P][D], radius [P], scale [P]
+  int penP = 0, penKind = 0, penD = 0;
+  tb::DevBuf sXc2;              // second candidate staging slot of the pipelined driver (the penalised tail reads candidates)
 
   // profiling of the dominant kernel
   bool profile = false;

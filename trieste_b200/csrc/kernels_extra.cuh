@@ -397,6 +397,55 @@ grad_kernel(const double* __restrict__ Xs, const double* __restrict__ alpha, con
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// K1h: posterior mean and its gradient, no variance.  mean[t] = sum_k k(x_t, x_k) alpha[k] + m,
+//   grad[t][d] = sum_k dk/dr2(k,t) * 2 (x~_t,d - x~_k,d) / l_d * alpha[k].  One warp per point walks all N training rows
+//   (the single pass over Xs and alpha of grad_kernel<..., 1>, without V).
+// ------------------------------------------------------------------------------------------------
+template <int KIND, int DP>
+__global__ void __launch_bounds__(256, 1)  // minimum of one CTA per SM: lets ptxas keep every DP in registers
+mean_grad_kernel(const double* __restrict__ Xs, const double* __restrict__ alpha, const double* __restrict__ Xc,
+                 const double* __restrict__ inv_ls, int N, int D, int64_t M, double variance, double mean_const,
+                 double* __restrict__ mean, double* __restrict__ grad) {
+  const int lane = threadIdx.x & 31;
+  const int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (t >= M) return;
+  double xc[DP], g[DP];
+#pragma unroll
+  for (int d = 0; d < DP; ++d) {
+    xc[d] = (d < D) ? Xc[t * D + d] * inv_ls[d] : 0.0;
+    g[d] = 0.0;
+  }
+  double macc = 0.0;
+  for (int k = lane; k < N; k += 32) {
+    const double* xr = Xs + (int64_t)k * DP;
+    double diff[DP], r2 = 0.0;
+#pragma unroll
+    for (int d = 0; d < DP; d += 2) {
+      double2 xv = __ldg(reinterpret_cast<const double2*>(xr + d));
+      diff[d] = xc[d] - xv.x;
+      diff[d + 1] = xc[d + 1] - xv.y;
+      r2 = fma(diff[d], diff[d], r2);
+      r2 = fma(diff[d + 1], diff[d + 1], r2);
+    }
+    const double a = __ldg(alpha + k);
+    macc = fma(kernel_from_r2<KIND>(r2, variance), a, macc);
+    const double w = 2.0 * kernel_dr2<KIND>(r2, variance) * a;
+#pragma unroll
+    for (int d = 0; d < DP; ++d) g[d] = fma(w, diff[d], g[d]);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) macc += __shfl_xor_sync(0xffffffffu, macc, o);
+  if (lane == 0) mean[t] = macc + mean_const;
+#pragma unroll
+  for (int d = 0; d < DP; ++d) {
+    double s = g[d];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0 && d < D) grad[t * D + d] = s * inv_ls[d];
+  }
+}
+
 // per-candidate partial derivatives of the acquisition w.r.t. (mean, var) from the tail inputs
 __global__ void __launch_bounds__(256)
 acq_partials_kernel(const double* __restrict__ partial, int G, int64_t McPad, const double* __restrict__ mean,

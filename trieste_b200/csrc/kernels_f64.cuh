@@ -411,15 +411,51 @@ __device__ __forceinline__ void mes_partials(const double* __restrict__ samp, in
   dvar = clipped ? 0.0 : -av / (2.0 * var * (double)ns);
 }
 
-// one thread per candidate of the chunk; block-level first-max argmax
+// ---- local penalisation (greedy_batch.py:315-388): the base value times prod_j pen_j(||x - x_j||) over the pending points
+//   soft (:315-354): pen_j = Phi((dist - radius_j) / scale_j)
+//   hard (:357-388): pen_j = ((dist / (radius_j + scale_j))^-5 + 1)^(-1/5)
+// f = pen_j and w = (d log pen_j / d dist) / dist, so that grad log pen_j = w (x - x_j).  At dist = 0 the gradient of the norm is
+// undefined and w is taken as 0.  The soft ratio phi/Phi goes through erfcx for z < -1 (mes_terms).
+__device__ __forceinline__ void penalty_factor(int kind, double dist, double radius, double scale, double& f, double& w) {
+  if (kind == TB_PEN_SOFT) {
+    const double z = (dist - radius) / scale;
+    f = ndtr_tfp(z);
+    double lc, ratio;
+    mes_terms(-z, lc, ratio);  // ratio = phi(z) / Phi(z)
+    w = dist > 0.0 ? ratio / (scale * dist) : 0.0;
+  } else {
+    const double u = dist / (radius + scale);
+    f = pow(pow(u, -5.0) + 1.0, -0.2);
+    // d log f / d dist = 1 / (dist (1 + u^5))
+    const double u5 = u * u * u * u * u;
+    w = dist > 0.0 ? (1.0 / dist) / (dist * (1.0 + u5)) : 0.0;
+  }
+}
+
+constexpr int PEN_TILE = 32;  // pending points per shared-memory tile of the penalised tail
+constexpr int PEN_DMAX = 32;  // largest input dimension (pick_dp)
+
+struct TailPenalty {
+  const double* xc = nullptr;      // [Mc][D] candidates of the chunk (device)
+  const double* pend = nullptr;    // [P][D] pending points
+  const double* radius = nullptr;  // [P]
+  const double* scale = nullptr;   // [P]
+  double* grad = nullptr;          // [Mc][D] gradient of the base acquisition, turned into the penalised one in place (nullable)
+  int P = 0, D = 0, kind = 0;
+};
+
+// one thread per candidate of the chunk; block-level first-max argmax.  PEN: the value (and the gradient, when
+// pen.grad is set) is multiplied by the local penalty before the argmax.
+template <bool PEN>
 __global__ void __launch_bounds__(256)
 tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const double* __restrict__ mean,
             int64_t Mc, int64_t idx0, double variance, int acq, double param, double aux,
             const double* __restrict__ samp, int nsamp, double* __restrict__ out_vals, double* __restrict__ out_mean, double* __restrict__ out_var,
-            double* __restrict__ blk_best, int64_t* __restrict__ blk_idx) {
+            double* __restrict__ blk_best, int64_t* __restrict__ blk_idx, const TailPenalty pen) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   double bv = -INFINITY;
   int64_t bi = INT64_MAX;
+  double vb = 0.0;  // PEN: the base value of this candidate
   if (t < Mc) {
     double ss = 0.0;
     for (int g = 0; g < G; ++g) ss += partial[(int64_t)g * McPad + t];
@@ -429,6 +465,63 @@ tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const doub
     if (out_var) out_var[t] = var;
     if (acq >= 0) {
       double v = (acq == TB_ACQ_MES) ? mes_value(samp, nsamp, mu, var) : acq_value(acq, param, aux, mu, var);
+      if (PEN) {
+        vb = v;
+      } else {
+        if (out_vals) out_vals[t] = v;
+        if (v == v) { bv = v; bi = idx0 + t; }
+      }
+    }
+  }
+  if (PEN) {
+    __shared__ double sp[PEN_TILE * PEN_DMAX], sr[PEN_TILE], sc[PEN_TILE];
+    const bool live = t < Mc && acq >= 0;
+    const int D = pen.D;
+    double x[PEN_DMAX], g[PEN_DMAX];
+#pragma unroll
+    for (int d = 0; d < PEN_DMAX; ++d) {
+      x[d] = (live && d < D) ? pen.xc[t * D + d] : 0.0;
+      g[d] = 0.0;
+    }
+    double prod = 1.0;
+    for (int j0 = 0; j0 < pen.P; j0 += PEN_TILE) {  // every thread of the block walks the tiles (barriers)
+      const int nj = min(PEN_TILE, pen.P - j0);
+      __syncthreads();
+      for (int i = threadIdx.x; i < nj * D; i += blockDim.x) sp[i] = pen.pend[(int64_t)j0 * D + i];
+      if (threadIdx.x < nj) {
+        sr[threadIdx.x] = pen.radius[j0 + threadIdx.x];
+        sc[threadIdx.x] = pen.scale[j0 + threadIdx.x];
+      }
+      __syncthreads();
+      if (!live) continue;
+      for (int j = 0; j < nj; ++j) {
+        double r2 = 0.0;
+#pragma unroll
+        for (int d = 0; d < PEN_DMAX; ++d)
+          if (d < D) {
+            const double df = x[d] - sp[j * D + d];
+            r2 = fma(df, df, r2);
+          }
+        double f, w;
+        penalty_factor(pen.kind, sqrt(r2), sr[j], sc[j], f, w);
+        prod *= f;
+        if (pen.grad) {
+#pragma unroll
+          for (int d = 0; d < PEN_DMAX; ++d)
+            if (d < D) g[d] = fma(w, x[d] - sp[j * D + d], g[d]);
+        }
+      }
+    }
+    if (live) {
+      // exp(log base + log pen) of the reference (greedy_batch.py:265-268): NaN for a negative base value
+      const double v = vb < 0.0 ? NAN : vb * prod;
+      if (pen.grad) {
+        // product rule pen grad(base) + base pen grad(log pen); where pen = 0 its gradient is taken as 0 (finite limit)
+        double* gr = pen.grad + t * D;
+#pragma unroll
+        for (int d = 0; d < PEN_DMAX; ++d)
+          if (d < D) gr[d] = fma(prod, gr[d], prod == 0.0 ? 0.0 : vb * (prod * g[d]));
+      }
       if (out_vals) out_vals[t] = v;
       if (v == v) { bv = v; bi = idx0 + t; }
     }

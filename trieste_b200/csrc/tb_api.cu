@@ -291,7 +291,7 @@ int tb_gp_destroy(tb_gp* gp) {
                         &gp->sVals, &gp->sVar, &gp->sXc, &gp->sBlkBest, &gp->sBlkIdx, &gp->sRun,
                         &gp->sA, &gp->sV, &gp->sGrad, &gp->sMisc, &gp->dMes, &gp->dXspare, &gp->dyspare, &gp->dLspare, &gp->dLinvSpare,
                         &gp->dAS5, &gp->dRowScale5, &gp->dRowSum5, &gp->dX2, &gp->dKinvS5, &gp->dKinvScale5, &gp->dKinvSum5,
-                        &gp->dKinvSpare, &gp->sMeanPart})
+                        &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->sXc2})
     b->release();
   for (auto& ev : gp->prof_events) {
     cudaEventDestroy(ev.first);
@@ -662,6 +662,7 @@ struct EvalRequest {
   double* out_var = nullptr;
   double* out_grad = nullptr;  // [M, D] (nullable)
   bool want_argmax = false;
+  bool pen = false;  // TB_ACQ_PENALIZED: multiply by the handle's local penalty (tb_acq_set_penalization)
   double best_value = 0.0;
   int64_t best_index = -1;
 };
@@ -781,10 +782,38 @@ static void launch_grad_dp(tb_gp* gp, const double* xc, int64_t mc, double* grad
 #undef TB_GRAD
 }
 
+// The acquisition tail of one chunk.  A penalised request (rq.pen) multiplies the value, and the gradient in gd (device,
+// [mc][D], nullable) in place, by the handle's local penalty at the candidates xc (device, [mc][D]); so the tail must run
+// after the gradient assembly and before the gradient leaves the device.  Unpenalised requests run the plain tail.
+static void launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const double* partial, int G, int64_t McPad,
+                        const double* mean, int64_t mc, int64_t c0, double* d_vals, double* d_mean, double* d_var,
+                        const double* xc, double* gd) {
+  const int blocks = (int)((mc + 255) / 256);
+  double* bb = rq.want_argmax ? gp->sBlkBest.as<double>() : nullptr;
+  int64_t* bi = rq.want_argmax ? gp->sBlkIdx.as<int64_t>() : nullptr;
+  TailPenalty pen;
+  if (rq.pen) {
+    pen.xc = xc;
+    pen.pend = gp->dPen.as<double>();
+    pen.radius = pen.pend + (int64_t)gp->penP * gp->D;
+    pen.scale = pen.radius + gp->penP;
+    pen.grad = gd;
+    pen.P = gp->penP;
+    pen.D = gp->D;
+    pen.kind = gp->penKind;
+    tail_kernel<true><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, gp->noise,
+                                              gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, pen);
+  } else {
+    tail_kernel<false><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, gp->noise,
+                                               gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, pen);
+  }
+  TB_LAUNCHED();
+}
+
 // after the lower GEMM (A stored as packed panels in sA, sum-of-squares in sPartial):
 // V = Linv^T A, then the gradient assembly
 static int gradient_chunk(tb_gp* gp, int acq, double param, const double* xc, int64_t mc, int tiles, int G,
-                          int64_t McPad, double* out_grad) {
+                          int64_t McPad, double* gd) {  // gd: device [mc][D]
   cudaStream_t st = gp->stream;
   double* cmu = gp->sMisc.as<double>();
   acq_partials_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, st>>>(gp->sPartial.as<double>(), G, McPad,
@@ -796,8 +825,6 @@ static int gradient_chunk(tb_gp* gp, int acq, double param, const double* xc, in
       gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB, nkB, G, McPad, nullptr, nullptr, gp->sV.as<double>(),
       (int64_t)gp->NB * BM);
   TB_LAUNCHED();
-  const bool gdev = is_device_ptr(out_grad);
-  double* gd = gdev ? out_grad : gp->sGrad.as<double>();
   switch (gp->kernel) {
     case TB_RBF: launch_grad_dp<TB_RBF>(gp, xc, mc, gd); break;
     case TB_MATERN12: launch_grad_dp<TB_MATERN12>(gp, xc, mc, gd); break;
@@ -806,7 +833,6 @@ static int gradient_chunk(tb_gp* gp, int acq, double param, const double* xc, in
   }
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
-  if (!gdev) TB_CUDA(cudaMemcpyAsync(out_grad, gd, sizeof(double) * mc * gp->D, cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
@@ -891,7 +917,7 @@ static int ensure_kinv_digits(tb_gp* gp) {
 
 // int8 engine, gradient path: sum-of-squares is already in sPartial (variance GEMM); V = K^-1 k* on the tensor cores
 static int gradient_chunk_oz(tb_gp* gp, int acq, double param, const double* xc, int64_t mc, int tiles, int G, int64_t McPad,
-                             double* out_grad) {
+                             double* gd) {  // gd: device [mc][D]
   cudaStream_t st = gp->stream;
   double* cmu = gp->sMisc.as<double>();
   acq_partials_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, st>>>(gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc,
@@ -902,8 +928,6 @@ static int gradient_chunk_oz(tb_gp* gp, int acq, double param, const double* xc,
                                           gp->nst, Gv, McPad, gp->oz_out_scale, oz_npass(gp), 1, nullptr, gp->sV.as<double>(),
                                           (int64_t)gp->NB * BM));
   TB_LAUNCHED();
-  const bool gdev = is_device_ptr(out_grad);
-  double* gd = gdev ? out_grad : gp->sGrad.as<double>();
   switch (gp->kernel) {
     case TB_RBF: launch_grad_dp<TB_RBF>(gp, xc, mc, gd); break;
     case TB_MATERN12: launch_grad_dp<TB_MATERN12>(gp, xc, mc, gd); break;
@@ -912,7 +936,6 @@ static int gradient_chunk_oz(tb_gp* gp, int acq, double param, const double* xc,
   }
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
-  if (!gdev) TB_CUDA(cudaMemcpyAsync(out_grad, gd, sizeof(double) * mc * gp->D, cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
@@ -1016,7 +1039,10 @@ static int run_eval_oz(tb_gp* gp, EvalRequest& rq) {
     TB_TRY(mean[i]->reserve(sizeof(double) * chunk_cap));
     TB_TRY(part[i]->reserve(sizeof(double) * (size_t)G * chunk_cap));
   }
-  if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * chunk_cap * D));
+  // host candidates are staged per slot: the tail of chunk c (stream A) may read them while stream B stages chunk c + 1
+  tb::DevBuf* xs[2] = {&gp->sXc, &gp->sXc2};
+  if (!xc_dev)
+    for (int i = 0; i < nslots; ++i) TB_TRY(xs[i]->reserve(sizeof(double) * chunk_cap * D));
   if (rq.out_vals && !vals_dev) TB_TRY(gp->sVals.reserve(sizeof(double) * chunk_cap));
   if (rq.out_var && !var_dev) TB_TRY(gp->sVar.reserve(sizeof(double) * chunk_cap));
   const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
@@ -1037,8 +1063,8 @@ static int run_eval_oz(tb_gp* gp, EvalRequest& rq) {
     if (xc_dev) {
       xc_chunk = rq.Xc + c0 * D;
     } else {
-      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, rq.Xc + c0 * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, sb));
-      xc_chunk = gp->sXc.as<double>();
+      TB_CUDA(cudaMemcpyAsync(xs[slot]->p, rq.Xc + c0 * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, sb));
+      xc_chunk = xs[slot]->as<double>();
     }
     if (fast) {
       TB_TRY(oz5_launch_kstar(gp, sb, xc_chunk, mc, tiles, ks[slot]->as<int8_t>(), mean[slot]->as<double>()));
@@ -1074,11 +1100,8 @@ static int run_eval_oz(tb_gp* gp, EvalRequest& rq) {
     double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;
     double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
     const int tb_blocks = (int)((mc + 255) / 256);
-    tail_kernel<<<tb_blocks, 256, 0, sa>>>(part[slot]->as<double>(), G, McPad, mean[slot]->as<double>(), mc, c0, gp->variance,
-                                           rq.acq, rq.param, gp->noise, gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var,
-                                           rq.want_argmax ? gp->sBlkBest.as<double>() : nullptr,
-                                           rq.want_argmax ? gp->sBlkIdx.as<int64_t>() : nullptr);
-    TB_LAUNCHED();
+    launch_tail(gp, sa, rq, part[slot]->as<double>(), G, McPad, mean[slot]->as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk,
+                nullptr);
     if (rq.want_argmax) {
       argmax_fold_kernel<<<1, 256, 0, sa>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks,
                                             gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
@@ -1091,8 +1114,6 @@ static int run_eval_oz(tb_gp* gp, EvalRequest& rq) {
     if (rq.out_var && !var_dev)
       TB_CUDA(cudaMemcpyAsync(rq.out_var + c0, gp->sVar.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, sa));
     TB_CUDA(cudaEventRecord(gp->evDone[slot], sa));
-    // the host staging of the candidates is single-buffered: the next H2D (stream B) must not overtake this chunk's kstar,
-    // which stream order on B already guarantees
   }
   if (rq.want_argmax) {
     TB_CUDA(cudaMemcpyAsync(&rq.best_value, gp->sRun.p, 8, cudaMemcpyDeviceToHost, sa));
@@ -1207,16 +1228,12 @@ static int run_eval_grad_oz5(tb_gp* gp, EvalRequest& rq) {
     }
     TB_LAUNCHED();
     TB_CUDA(cudaGetLastError());
-    if (!gdev) TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
     double* d_vals = rq.out_vals ? (vals_dev ? rq.out_vals + c0 : gp->sVals.as<double>()) : nullptr;
     double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;
     double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
     const int tb_blocks = (int)((mc + 255) / 256);
-    tail_kernel<<<tb_blocks, 256, 0, st>>>(gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, gp->variance, rq.acq,
-                                           rq.param, gp->noise, gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var,
-                                           rq.want_argmax ? gp->sBlkBest.as<double>() : nullptr,
-                                           rq.want_argmax ? gp->sBlkIdx.as<int64_t>() : nullptr);
-    TB_LAUNCHED();
+    launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd);
+    if (!gdev) TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
     if (rq.want_argmax) {
       argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks, gp->sRun.as<double>(),
                                             reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
@@ -1345,22 +1362,21 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
     }
     TB_CUDA(cudaGetLastError());
 
+    const bool gdev = rq.out_grad && is_device_ptr(rq.out_grad);
+    double* gd = rq.out_grad ? (gdev ? rq.out_grad + c0 * D : gp->sGrad.as<double>()) : nullptr;
     if (rq.out_grad) {
       if (use_oz)
-        TB_TRY(gradient_chunk_oz(gp, rq.acq, rq.param, xc_chunk, mc, tiles, G, McPad, rq.out_grad + c0 * D));
+        TB_TRY(gradient_chunk_oz(gp, rq.acq, rq.param, xc_chunk, mc, tiles, G, McPad, gd));
       else
-        TB_TRY(gradient_chunk(gp, rq.acq, rq.param, xc_chunk, mc, tiles, G, McPad, rq.out_grad + c0 * D));
+        TB_TRY(gradient_chunk(gp, rq.acq, rq.param, xc_chunk, mc, tiles, G, McPad, gd));
     }
 
     double* d_vals = rq.out_vals ? (vals_dev ? rq.out_vals + c0 : gp->sVals.as<double>()) : nullptr;
     double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;  // sMean already holds it
     double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
     const int tb_blocks = (int)((mc + 255) / 256);
-    tail_kernel<<<tb_blocks, 256, 0, st>>>(gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0,
-                                           gp->variance, rq.acq, rq.param, gp->noise, gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var,
-                                           rq.want_argmax ? gp->sBlkBest.as<double>() : nullptr,
-                                           rq.want_argmax ? gp->sBlkIdx.as<int64_t>() : nullptr);
-    TB_LAUNCHED();
+    launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd);
+    if (rq.out_grad && !gdev) TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
     if (rq.want_argmax) {
       argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks,
                                             gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
@@ -1399,6 +1415,67 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
   return 0;
 }
 
+// posterior mean and its gradient (no variance, no GEMM, no K^-1): one mean_grad_kernel launch per 65,536 points
+static int run_mean_grad(tb_gp* gp, const double* Xc, int64_t M, double* mean, double* grad) {
+  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_CHECK(M >= 0, "negative point count");
+  if (M == 0) return 0;
+  TB_CUDA(cudaSetDevice(gp->device));
+  cudaStream_t st = gp->stream;
+  const int D = gp->D;
+  constexpr int64_t CHUNK = 65536;
+  const int64_t cap = std::min(M, CHUNK);
+  const bool xc_dev = is_device_ptr(Xc), mean_dev = is_device_ptr(mean), grad_dev = is_device_ptr(grad);
+  if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * cap * D));
+  if (!mean_dev) TB_TRY(gp->sMean.reserve(sizeof(double) * cap));
+  if (!grad_dev) TB_TRY(gp->sGrad.reserve(sizeof(double) * cap * D));
+  const double* Xs = gp->dXs.as<double>();
+  const double* al = gp->dAlpha.as<double>();
+  const double* il = gp->dInvLs.as<double>();
+  for (int64_t c0 = 0; c0 < M; c0 += CHUNK) {
+    const int64_t mc = std::min(CHUNK, M - c0);
+    const double* xc = Xc + c0 * D;
+    if (!xc_dev) {
+      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, xc, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
+      xc = gp->sXc.as<double>();
+    }
+    double* md = mean_dev ? mean + c0 : gp->sMean.as<double>();
+    double* gd = grad_dev ? grad + c0 * D : gp->sGrad.as<double>();
+    const unsigned blocks = (unsigned)((mc + 7) / 8);
+#define TB_MG(KIND, DPV) \
+  mean_grad_kernel<KIND, DPV><<<blocks, 256, 0, st>>>(Xs, al, xc, il, (int)gp->N, D, mc, gp->variance, gp->mean_const, md, gd)
+#define TB_MG_DP(KIND)        \
+  switch (gp->DP) {           \
+    case 2: TB_MG(KIND, 2); break;   \
+    case 4: TB_MG(KIND, 4); break;   \
+    case 6: TB_MG(KIND, 6); break;   \
+    case 8: TB_MG(KIND, 8); break;   \
+    case 10: TB_MG(KIND, 10); break; \
+    case 12: TB_MG(KIND, 12); break; \
+    case 16: TB_MG(KIND, 16); break; \
+    case 20: TB_MG(KIND, 20); break; \
+    case 24: TB_MG(KIND, 24); break; \
+    default: TB_MG(KIND, 32); break; \
+  }
+    switch (gp->kernel) {
+      case TB_RBF: TB_MG_DP(TB_RBF); break;
+      case TB_MATERN12: TB_MG_DP(TB_MATERN12); break;
+      case TB_MATERN32: TB_MG_DP(TB_MATERN32); break;
+      default: TB_MG_DP(TB_MATERN52); break;
+    }
+#undef TB_MG_DP
+#undef TB_MG
+    TB_LAUNCHED();
+    TB_CUDA(cudaGetLastError());
+    if (!mean_dev) TB_CUDA(cudaMemcpyAsync(mean + c0, md, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+    if (!grad_dev) TB_CUDA(cudaMemcpyAsync(grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
+    if (!xc_dev || !mean_dev || !grad_dev) TB_CUDA(cudaStreamSynchronize(st));  // scratch is reused by the next chunk
+  }
+  TB_CUDA(cudaStreamSynchronize(st));
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace tb
 
 extern "C" {
@@ -1413,14 +1490,27 @@ static int tb_gp_predict_f64(tb_gp* gp, const void* Xc, int64_t M, void* mean, v
   return tb::run_eval(gp, rq);
 }
 
+// TB_ACQ_PENALIZED is stripped from acq here: every kernel and check below sees the plain kind
+static int split_penalized(const tb_gp* gp, int& acq, bool& pen, const char* who) {
+  pen = (acq & TB_ACQ_PENALIZED) != 0;
+  acq &= ~TB_ACQ_PENALIZED;
+  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_MES, std::string(who) + ": unknown acquisition kind");
+  if (pen)
+    TB_CHECK(gp->penP > 0 && gp->penD == gp->D,
+             std::string(who) + ": a penalised acquisition needs the local penalty first (tb_acq_set_penalization)");
+  return 0;
+}
+
 static int tb_acq_eval_f64(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad) {
   TB_CHECK(gp && (M == 0 || (Xc && out)), "tb_acq_eval: null argument");
-  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_MES, "tb_acq_eval: unknown acquisition kind");
+  bool pen = false;
+  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_eval"));
   if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
     TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
   if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
   tb::EvalRequest rq;
   rq.acq = acq;
+  rq.pen = pen;
   rq.param = param;
   rq.Xc = (const double*)Xc;
   rq.M = M;
@@ -1432,12 +1522,14 @@ static int tb_acq_eval_f64(tb_gp* gp, int acq, double param, const void* Xc, int
 static int tb_acq_argmax_f64(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* best_value,
                   int64_t* best_index) {
   TB_CHECK(gp && Xc && best_value && best_index, "tb_acq_argmax: null argument");
-  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_MES, "tb_acq_argmax: unknown acquisition kind");
+  bool pen = false;
+  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_argmax"));
   if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
     TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
   if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
   tb::EvalRequest rq;
   rq.acq = acq;
+  rq.pen = pen;
   rq.param = param;
   rq.Xc = (const double*)Xc;
   rq.M = M;
@@ -1461,6 +1553,25 @@ int tb_acq_set_min_value_samples(tb_gp* gp, const double* samples, int S) {
   TB_CUDA(cudaMemcpyAsync(gp->dMes.p, samples, sizeof(double) * (size_t)S, cudaMemcpyDefault, gp->stream));
   TB_CUDA(cudaStreamSynchronize(gp->stream));
   gp->mesS = S;
+  return 0;
+}
+
+int tb_acq_set_penalization(tb_gp* gp, int kind, const double* pending, int P, const double* radius, const double* scale) {
+  TB_CHECK(gp && pending && radius && scale, "tb_acq_set_penalization: null argument");
+  TB_CHECK(kind == TB_PEN_SOFT || kind == TB_PEN_HARD, "tb_acq_set_penalization: kind must be 1 (soft) or 2 (hard)");
+  TB_CHECK(P > 0, "tb_acq_set_penalization: need at least one pending point");
+  TB_CHECK(gp->have_data, "tb_acq_set_penalization: the model has no data (input dimension unknown)");
+  TB_CUDA(cudaSetDevice(gp->device));
+  const size_t PD = (size_t)P * gp->D;
+  TB_TRY(gp->dPen.reserve(sizeof(double) * (PD + 2 * (size_t)P)));
+  double* d = gp->dPen.as<double>();
+  TB_CUDA(cudaMemcpyAsync(d, pending, sizeof(double) * PD, cudaMemcpyDefault, gp->stream));
+  TB_CUDA(cudaMemcpyAsync(d + PD, radius, sizeof(double) * (size_t)P, cudaMemcpyDefault, gp->stream));
+  TB_CUDA(cudaMemcpyAsync(d + PD + P, scale, sizeof(double) * (size_t)P, cudaMemcpyDefault, gp->stream));
+  TB_CUDA(cudaStreamSynchronize(gp->stream));
+  gp->penP = P;
+  gp->penKind = kind;
+  gp->penD = gp->D;
   return 0;
 }
 
@@ -2618,6 +2729,21 @@ int tb_gp_predict(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* var) {
   return br.finish();
 }
 
+int tb_gp_mean_gradient(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* grad) {
+  TB_CHECK(gp && (M == 0 || (Xc && mean && grad)), "tb_gp_mean_gradient: null argument");
+  if (gp->dtype == TB_F64) return tb::run_mean_grad(gp, (const double*)Xc, M, (double*)mean, (double*)grad);
+  if (M == 0) return 0;
+  TB_CUDA(cudaSetDevice(gp->device));
+  tb::F32Bridge br(gp);
+  const double* xd;
+  double *md, *gd;
+  TB_TRY(br.in(Xc, M * gp->D, &xd));
+  TB_TRY(br.out(mean, M, &md));
+  TB_TRY(br.out(grad, M * gp->D, &gd));
+  TB_TRY(tb::run_mean_grad(gp, xd, M, md, gd));
+  return br.finish();
+}
+
 int tb_acq_eval(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad) {
   TB_CHECK(gp && (M == 0 || (Xc && out)), "tb_acq_eval: null argument");
   if (gp->dtype == TB_F64) return tb_acq_eval_f64(gp, acq, param, Xc, M, out, grad);
@@ -2665,7 +2791,8 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   TB_CHECK(gp && lower && upper, "tb_acq_maximize: null argument");
   TB_CHECK(P >= 0 && P < ((int64_t)1 << 31), "tb_acq_maximize: number of starts out of range");
   TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_acq_maximize: null argument");
-  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_MES, "tb_acq_maximize: unknown acquisition kind");
+  bool pen = false;
+  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_maximize"));
   if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
     TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
   if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
@@ -2731,6 +2858,7 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
     const int n_round = n_active;
     tb::EvalRequest rq;
     rq.acq = acq;
+    rq.pen = pen;
     rq.param = param;
     rq.Xc = bxt.as<double>();
     rq.M = n_active;

@@ -195,6 +195,19 @@ class GaussianProcessRegression:
         _lib.check(_lib.lib().tb_gp_predict(self._h, _ptr(flat), M, pm, pv))
         return mean.reshape(lead + (1,)), var.reshape(lead + (1,))
 
+    def mean_gradient(self, query_points) -> Tuple[np.ndarray, np.ndarray]:
+        """[..., D] -> (mean [..., 1], d mean / d x [..., D]): the posterior mean and the gradient the reference takes of it
+        with a GradientTape for the Lipschitz estimate of local penalisation (greedy_batch.py:207-217).  No variance is
+        formed: one pass over the training rows per point."""
+        x, _ = _lib.as_contiguous(query_points, self._dtype)
+        self._check_dim(x)
+        flat, lead = _flatten_leading(x, 1)
+        M, D = flat.shape
+        mean, pm = _lib.empty_like_kind(flat, (M, 1), self._dtype)
+        grad, pg = _lib.empty_like_kind(flat, (M, D), self._dtype)
+        _lib.check(_lib.lib().tb_gp_mean_gradient(self._h, _ptr(flat), M, pm, pg))
+        return mean.reshape(lead + (1,)), grad.reshape(lead + (D,))
+
     def predict_joint(self, query_points) -> Tuple[np.ndarray, np.ndarray]:
         """[..., B, D] -> (mean [..., B, 1], cov [..., 1, B, B]) (interfaces.py:133-140;
         interface.py:126-133)."""
