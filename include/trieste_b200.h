@@ -53,8 +53,14 @@ enum tb_acq {
                          ProbabilityOfFeasibility :421-478): Normal(mean, sqrt(var)).cdf(param) */
   TB_ACQ_AEI = 5,     /* augmented_expected_improvement.__call__, function.py:311-325: EI(param = eta) times
                          1 − sqrt(noise)/sqrt(noise + var), noise = the handle's likelihood variance */
-  TB_ACQ_MES = 6      /* min_value_entropy_search.__call__, entropy.py:193-213: mean over the min-value samples set by
+  TB_ACQ_MES = 6,     /* min_value_entropy_search.__call__, entropy.py:193-213: mean over the min-value samples set by
                          tb_acq_set_min_value_samples of −γ·φ(γ)/(2Φ(−γ)) − log Φ(−γ), γ = (y* − mean)/sd; param unused */
+  TB_ACQ_GIBBON_QUALITY = 7,   /* gibbon_quality_term.__call__, entropy.py:479-500: −½ mean_s log(1 + ρ² r_s (γ_s − r_s)),
+                                  ρ² = var/(var + σ²), r = φ(γ)/Φ(−γ), over the tb_acq_set_min_value_samples samples */
+  TB_ACQ_GIBBON_REPULSION = 8, /* gibbon_repulsion_term.__call__, entropy.py:580-618: w·½(log(yvar − ‖L_B⁻¹c(x)‖²) − log yvar)
+                                  over the pending points set by tb_acq_set_gibbon_repulsion; yvar = var + σ²;
+                                  needs no min-value samples */
+  TB_ACQ_GIBBON = 9            /* GibbonAcquisition.__call__, entropy.py:435-436: repulsion + quality */
 };
 /* OR-ed into `acq` of tb_acq_eval / tb_acq_argmax / tb_acq_maximize: the value (and gradient) is multiplied by the local
  * penalty set by tb_acq_set_penalization (PenalizedAcquisition, acquisition/function/greedy_batch.py:250-269). */
@@ -126,6 +132,14 @@ int tb_acq_set_min_value_samples(tb_gp* gp, const double* samples, int S);
  * (μ(x_j) − η)/L and scale sqrt(var(x_j))/L, held by the handle for calls with TB_ACQ_PENALIZED.  kind: tb_penalizer;
  * pending [P,D], radius [P], scale [P]; always double, host or device pointers, P ≥ 1. */
 int tb_acq_set_penalization(tb_gp* gp, int kind, const double* pending, int P, const double* radius, const double* scale);
+
+/* gibbon_repulsion_term.__init__ / update (entropy.py:580-618): the m pending points P and the repulsion weight w
+ * ((1/m)² with rescaled_repulsion, else 1), held by the handle for TB_ACQ_GIBBON_REPULSION and TB_ACQ_GIBBON.  From them the
+ * handle derives W = K⁻¹k(X, P) and L_B⁻¹, L_B = chol(B + σ²I), B = predict_joint(P) with its diagonal clipped at ≥ 1e-12.
+ * They follow the posterior: after tb_gp_update_posterior_cache or tb_gp_append_data they are rebuilt before the next
+ * GIBBON launch, and not otherwise.  pending [m,D], always double, host or device pointer, m ≥ 1, needs a valid cache;
+ * TB_ERR_NUMERIC if B + σ²I is not positive definite. */
+int tb_acq_set_gibbon_repulsion(tb_gp* gp, const double* pending, int m, double weight);
 
 /* the posterior mean and its gradient, what LocalPenalization's Lipschitz estimate differentiates
  * (greedy_batch.py:207-217): Xc [M,D] → mean [M] = k(x, X) α + m and grad [M,D] = its derivative in x.  No variance: one

@@ -15,7 +15,8 @@ import numpy as np
 from .. import _lib
 from ..data import Dataset
 from ..models import GaussianProcessRegression, _flatten_leading, _ptr
-from .interface import AcquisitionFunctionClass, SingleModelAcquisitionBuilder, SingleModelVectorizedAcquisitionBuilder
+from .interface import (AcquisitionFunctionClass, SingleModelAcquisitionBuilder, SingleModelGreedyAcquisitionBuilder,
+                        SingleModelVectorizedAcquisitionBuilder)
 
 JITTER = 1e-6  # trieste/utils/misc.py:183
 
@@ -179,11 +180,13 @@ class min_value_entropy_search(_FusedSingleQuery):
         return self._samples[:, None]
 
     def _before_call(self) -> None:
-        _lib.check(
-            _lib.lib().tb_acq_set_min_value_samples(
-                self._model.handle, self._samples.ctypes.data_as(C.POINTER(C.c_double)), int(self._samples.size)
-            )
-        )
+        _push_min_value_samples(self._model, self._samples)
+
+
+def _push_min_value_samples(model: GaussianProcessRegression, samples: np.ndarray) -> None:
+    _lib.check(
+        _lib.lib().tb_acq_set_min_value_samples(model.handle, samples.ctypes.data_as(C.POINTER(C.c_double)), int(samples.size))
+    )
 
 
 class _lcb(_FusedSingleQuery):
@@ -352,6 +355,166 @@ class MinValueEntropySearch(SingleModelAcquisitionBuilder):
             raise ValueError(f"expected a min_value_entropy_search function, got {function!r}")
         function.update(self._draw(model, dataset))
         return function
+
+
+class gibbon_quality_term(_FusedSingleQuery):
+    """entropy.py:439-500: the information each single point gives about the objective minimum y*,
+    ``-1/2 mean_s log(1 + rho^2 r_s (gamma_s - r_s))`` with ``rho^2 = var / (var + noise)`` and gamma, r as for MES.  The
+    samples (rank two, non-empty) are pushed to the native handle before every launch."""
+
+    _acq = _lib.ACQ_GIBBON_QUALITY
+
+    def __init__(self, model, samples):
+        super().__init__(model, 0.0)
+        self.update(samples)
+
+    def update(self, samples) -> None:
+        s = np.asarray(_to_host(samples), dtype=np.float64)
+        if s.ndim != 2:
+            raise ValueError(f"samples must have rank two, got shape {s.shape}")
+        if s.shape[0] == 0:
+            raise ValueError("samples must not be empty")
+        self._samples = np.ascontiguousarray(s.reshape(-1))
+
+    @property
+    def samples(self) -> np.ndarray:
+        return self._samples[:, None]
+
+    def _before_call(self) -> None:
+        _push_min_value_samples(self._model, self._samples)
+
+
+class gibbon_repulsion_term(_FusedSingleQuery):
+    """entropy.py:503-618: ``w/2 (log V_det - log yvar)``, the log-determinant gain of adding x to the m pending points,
+    ``V_det = yvar - c(x)^T (B + noise I)^-1 c(x)`` with c the posterior covariance between x and the pending points and B
+    theirs; ``w = (1/m)^2`` with ``rescaled_repulsion``, else 1.  The device derives K^-1 k(X, P) and the Cholesky factor of
+    B + noise I once per pending set and posterior; the pending points are pushed before every launch."""
+
+    _acq = _lib.ACQ_GIBBON_REPULSION
+
+    def __init__(self, model, pending_points, rescaled_repulsion: bool = True):
+        super().__init__(model, 0.0)
+        self._rescaled_repulsion = bool(rescaled_repulsion)
+        self.update(pending_points)
+
+    def update(self, pending_points, lipschitz_constant=None, eta=None) -> None:
+        """entropy.py:594-601: only the pending points change; the other arguments are those of the penalisation protocol."""
+        p = np.asarray(_to_host(pending_points), dtype=np.float64)
+        if p.ndim != 2:
+            raise ValueError(f"pending_points must have rank 2, got shape {p.shape}")
+        if p.shape[0] == 0:
+            raise ValueError("pending_points must not be empty")
+        self._model._check_dim(p)
+        self._pending = np.ascontiguousarray(p)
+
+    @property
+    def pending_points(self) -> np.ndarray:
+        return self._pending
+
+    @property
+    def weight(self) -> float:
+        return (1.0 / self._pending.shape[0]) ** 2 if self._rescaled_repulsion else 1.0
+
+    def _before_call(self) -> None:
+        _lib.check(
+            _lib.lib().tb_acq_set_gibbon_repulsion(
+                self._model.handle, self._pending.ctypes.data, int(self._pending.shape[0]), float(self.weight)
+            )
+        )
+
+
+class GibbonAcquisition(_FusedSingleQuery):
+    """entropy.py:422-436: ``diversity_term(x) + quality_term(x)``, both evaluated in the same fused launch."""
+
+    _acq = _lib.ACQ_GIBBON
+
+    def __init__(self, quality_term: gibbon_quality_term, diversity_term: gibbon_repulsion_term):
+        if not isinstance(quality_term, gibbon_quality_term) or not isinstance(diversity_term, gibbon_repulsion_term):
+            raise ValueError("GibbonAcquisition needs a gibbon_quality_term and a gibbon_repulsion_term")
+        if quality_term._model is not diversity_term._model:
+            raise ValueError("the quality and repulsion terms of GibbonAcquisition must share one model")
+        super().__init__(quality_term._model, 0.0)
+        self._quality_term = quality_term
+        self._diversity_term = diversity_term
+
+    def _before_call(self) -> None:
+        self._quality_term._before_call()
+        self._diversity_term._before_call()
+
+
+class GIBBON(SingleModelGreedyAcquisitionBuilder):
+    """entropy.py:236-419: greedy batches by GIBBON (Moss et al. 2021), modified for minimisation.  The min-value samples
+    are drawn as :class:`MinValueEntropySearch` draws them (its ``_draw``: exact Thompson sampling over the data and
+    ``grid_size`` search-space points by default, Gumbel above the exact sampler's point limit); ``seed`` makes the draws
+    reproducible.  Without pending points the builder returns the quality term, otherwise one :class:`GibbonAcquisition`
+    object that is updated in place at every later greedy step."""
+
+    def __init__(self, search_space, num_samples: int = 5, grid_size: int = 1000, min_value_sampler=None,
+                 rescaled_repulsion: bool = True, seed=None):
+        if min_value_sampler is not None and not min_value_sampler.sample_min_value:
+            raise ValueError(
+                "GIBBON requires a min_value_sampler that samples minimum values, however the passed sampler has "
+                "sample_min_value=False."
+            )
+        # validates num_samples and grid_size, and owns the draws
+        self._min_value_draws = MinValueEntropySearch(search_space, num_samples, grid_size, min_value_sampler, seed=seed)
+        self._search_space = search_space
+        self._num_samples = num_samples
+        self._grid_size = grid_size
+        self._min_value_sampler = min_value_sampler
+        self._rescaled_repulsion = bool(rescaled_repulsion)
+        self._min_value_samples: Optional[np.ndarray] = None
+        self._quality_term: Optional[gibbon_quality_term] = None
+        self._diversity_term: Optional[gibbon_repulsion_term] = None
+        self._gibbon_acquisition: Optional[GibbonAcquisition] = None
+
+    def __repr__(self) -> str:
+        return (f"GIBBON({self._search_space!r}, {self._num_samples!r}, {self._grid_size!r}, {self._min_value_sampler!r}, "
+                f"{self._rescaled_repulsion!r})")
+
+    def prepare_acquisition_function(self, model, dataset: Optional[Dataset] = None, pending_points=None):
+        """entropy.py:315-341."""
+        _require_native(model)
+        dataset = _check_populated(dataset)
+        acq = self._update_quality_term(dataset, model)
+        if pending_points is not None and len(pending_points) != 0:
+            acq = self._update_repulsion_term(acq, dataset, model, pending_points)
+        return acq
+
+    def update_acquisition_function(self, function, model, dataset: Optional[Dataset] = None, pending_points=None,
+                                    new_optimization_step: bool = True):
+        """entropy.py:343-374: new samples at a new optimisation step; the quality term alone without pending points."""
+        dataset = _check_populated(dataset)
+        if self._quality_term is None:
+            raise ValueError("GIBBON: prepare_acquisition_function must be called before update_acquisition_function")
+        if new_optimization_step:
+            self._update_quality_term(dataset, model)
+        if pending_points is None:
+            return self._quality_term
+        return self._update_repulsion_term(function, dataset, model, pending_points)
+
+    def _update_repulsion_term(self, function, dataset: Dataset, model, pending_points):
+        """entropy.py:376-401: the same GibbonAcquisition object once it exists."""
+        pts = np.asarray(_to_host(pending_points))
+        if pts.ndim != 2:
+            raise ValueError(f"pending_points must have rank 2, got shape {pts.shape}")
+        if self._gibbon_acquisition is not None and isinstance(self._diversity_term, gibbon_repulsion_term):
+            self._diversity_term.update(pts)
+            return self._gibbon_acquisition
+        self._diversity_term = gibbon_repulsion_term(model, pts, rescaled_repulsion=self._rescaled_repulsion)
+        self._gibbon_acquisition = GibbonAcquisition(self._quality_term, self._diversity_term)
+        return self._gibbon_acquisition
+
+    def _update_quality_term(self, dataset: Dataset, model):
+        """entropy.py:403-419."""
+        _require_native(model)
+        dataset = _check_populated(dataset)
+        self._min_value_samples = self._min_value_draws._draw(model, dataset)
+        if self._quality_term is not None:
+            self._quality_term.update(self._min_value_samples)
+        else:
+            self._quality_term = gibbon_quality_term(model, self._min_value_samples)
+        return self._quality_term
 
 
 class AugmentedExpectedImprovement(ExpectedImprovement):

@@ -119,6 +119,15 @@ struct tb_gp {
   tb::DevBuf dPen;              // local penalisation (tb_acq_set_penalization): pending [P][D], radius [P], scale [P]
   int penP = 0, penKind = 0, penD = 0;
   tb::DevBuf sXc2;              // second candidate staging slot of the pipelined driver (the penalised tail reads candidates)
+  // GIBBON repulsion (tb_acq_set_gibbon_repulsion): raw pending points [m][D] and weight, and what is derived from them and
+  // the posterior cache: scaled pending points [m][DP], L_B^-1 [mp][m] (zero rows past m), What = K^-1 k(X,P) L_B^-T [N][mp]
+  std::vector<double> gibP;
+  int gibM = 0, gibMp = 0, gibD = 0;
+  double gibW = 0.0;
+  uint64_t cache_gen = 0;               // bumped whenever the posterior cache is (re)built
+  uint64_t gib_gen = ~(uint64_t)0;      // cache_gen the derived GIBBON state was built for
+  tb::DevBuf dGibPs, dGibLinv, dGibWhat;
+  tb::DevBuf sGib;                      // per chunk: |u|^2 [mc], -w / V_det [mc], u [mp][mc] (gradient path)
 
   // profiling of the dominant kernel
   bool profile = false;

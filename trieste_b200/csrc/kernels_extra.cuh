@@ -446,12 +446,203 @@ mean_grad_kernel(const double* __restrict__ Xs, const double* __restrict__ alpha
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// K1i: GIBBON's cross term (entropy.py:580-618).  For the m pending points P (scaled coordinates Ps [m][DP]):
+//   c_j(x) = k(x, p_j) - sum_n k(x, x_n) W_nj,  W = K^-1 k(X, P)          (covariance_between_points, unclipped)
+//   u = L_B^-1 c(x),  |u|^2,  L_B = chol(B + noise I)
+// computed as u_i = sum_{j<=i} Linv_B[i][j] k(x, p_j) - sum_n k(x, x_n) What[n][i], What = W L_B^-T (built once per pending
+// set and posterior cache).  One thread per candidate; the pending set is walked in register tiles of GIB_TILE rows of u, each
+// one pass over the training rows (warp-uniform loads of Xs and What rows: broadcast through L1), so m has no upper bound.
+// U (nullable, [mp][Mc]): u itself, for the gradient.
+// ------------------------------------------------------------------------------------------------
+constexpr int GIB_TILE = 16;
+
+template <int KIND, int DP>
+__global__ void __launch_bounds__(128, 4)  // up to 128 registers: every DP keeps xc and the tile of u in registers
+gibbon_cross_kernel(const double* __restrict__ Xs, const double* __restrict__ What, const double* __restrict__ Ps,
+                    const double* __restrict__ LBinv, const double* __restrict__ Xc, const double* __restrict__ inv_ls, int N,
+                    int D, int m, int mp, int64_t Mc, double variance, const __grid_constant__ fm::Consts fc,
+                    double* __restrict__ uu_out, double* __restrict__ U) {
+  __shared__ double exp_tab[64];  // 2^(j/64) for the branch-free exp of fastmath.cuh (as the K* generation kernels)
+  if (threadIdx.x < 64) exp_tab[threadIdx.x] = fm::EXP2_TABLE_DEV[threadIdx.x];
+  __syncthreads();
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= Mc) return;
+  double xc[DP];
+#pragma unroll
+  for (int d = 0; d < DP; ++d) xc[d] = (d < D) ? Xc[t * D + d] * inv_ls[d] : 0.0;
+  double uu = 0.0;
+  for (int i0 = 0; i0 < mp; i0 += GIB_TILE) {
+    double acc[GIB_TILE];
+#pragma unroll
+    for (int i = 0; i < GIB_TILE; ++i) acc[i] = 0.0;
+    const int jend = min(m, i0 + GIB_TILE);  // Linv_B is lower triangular
+    for (int j = 0; j < jend; ++j) {
+      const double* pr = Ps + (int64_t)j * DP;
+      double r2 = 0.0;
+#pragma unroll
+      for (int d = 0; d < DP; d += 2) {
+        const double2 pv = __ldg(reinterpret_cast<const double2*>(pr + d));
+        const double a = xc[d] - pv.x, b = xc[d + 1] - pv.y;
+        r2 = fma(a, a, r2);
+        r2 = fma(b, b, r2);
+      }
+      const double kj = kernel_from_r2_fast<KIND>(r2, variance, exp_tab, fc);
+      const double* lr = LBinv + (int64_t)i0 * m + j;
+#pragma unroll
+      for (int i = 0; i < GIB_TILE; ++i) acc[i] = fma(__ldg(lr + (int64_t)i * m), kj, acc[i]);
+    }
+    for (int n = 0; n < N; ++n) {
+      const double* xr = Xs + (int64_t)n * DP;
+      double r2 = 0.0;
+#pragma unroll
+      for (int d = 0; d < DP; d += 2) {
+        const double2 xv = __ldg(reinterpret_cast<const double2*>(xr + d));
+        const double a = xc[d] - xv.x, b = xc[d + 1] - xv.y;
+        r2 = fma(a, a, r2);
+        r2 = fma(b, b, r2);
+      }
+      const double kn = -kernel_from_r2_fast<KIND>(r2, variance, exp_tab, fc);
+      const double* wr = What + (int64_t)n * mp + i0;
+#pragma unroll
+      for (int i = 0; i < GIB_TILE; i += 2) {
+        const double2 w = __ldg(reinterpret_cast<const double2*>(wr + i));
+        acc[i] = fma(kn, w.x, acc[i]);
+        acc[i + 1] = fma(kn, w.y, acc[i + 1]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < GIB_TILE; ++i) {
+      uu = fma(acc[i], acc[i], uu);
+      if (U) U[(int64_t)(i0 + i) * Mc + t] = acc[i];
+    }
+  }
+  uu_out[t] = uu;
+}
+
+// grad[t] += coef[t] (sum_j s_j dk(x, p_j)/dx - sum_n (What u)_n dk(x, x_n)/dx),  s = L_B^-T u,  coef = -w / V_det:
+// the |u|^2 part of the repulsion gradient, d|u|^2/dx = 2 u^T du/dx.  One warp per candidate, one pass over the training rows.
+template <int KIND, int DP>
+__global__ void __launch_bounds__(256, 1)
+gibbon_grad_kernel(const double* __restrict__ Xs, const double* __restrict__ What, const double* __restrict__ Ps,
+                   const double* __restrict__ LBinv, const double* __restrict__ Xc, const double* __restrict__ inv_ls, int N,
+                   int D, int m, int mp, int64_t Mc, double variance, const double* __restrict__ U,
+                   const double* __restrict__ coef, double* __restrict__ grad) {
+  const int lane = threadIdx.x & 31;
+  const int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (t >= Mc) return;
+  double xc[DP], g[DP];
+#pragma unroll
+  for (int d = 0; d < DP; ++d) {
+    xc[d] = (d < D) ? Xc[t * D + d] * inv_ls[d] : 0.0;
+    g[d] = 0.0;
+  }
+  const double* u = U + t;  // u_i = u[i * Mc]
+  for (int k = lane; k < N; k += 32) {
+    const double* xr = Xs + (int64_t)k * DP;
+    double diff[DP], r2 = 0.0;
+#pragma unroll
+    for (int d = 0; d < DP; d += 2) {
+      const double2 xv = __ldg(reinterpret_cast<const double2*>(xr + d));
+      diff[d] = xc[d] - xv.x;
+      diff[d + 1] = xc[d + 1] - xv.y;
+      r2 = fma(diff[d], diff[d], r2);
+      r2 = fma(diff[d + 1], diff[d + 1], r2);
+    }
+    const double* wr = What + (int64_t)k * mp;
+    double wu = 0.0;
+    for (int i = 0; i < m; ++i) wu = fma(__ldg(wr + i), u[(int64_t)i * Mc], wu);
+    const double w = -2.0 * kernel_dr2<KIND>(r2, variance) * wu;
+#pragma unroll
+    for (int d = 0; d < DP; ++d) g[d] = fma(w, diff[d], g[d]);
+  }
+  for (int j = lane; j < m; j += 32) {
+    double s = 0.0;
+    for (int i = j; i < m; ++i) s = fma(__ldg(LBinv + (int64_t)i * m + j), u[(int64_t)i * Mc], s);
+    const double* pr = Ps + (int64_t)j * DP;
+    double diff[DP], r2 = 0.0;
+#pragma unroll
+    for (int d = 0; d < DP; ++d) {
+      diff[d] = xc[d] - __ldg(pr + d);
+      r2 = fma(diff[d], diff[d], r2);
+    }
+    const double w = 2.0 * kernel_dr2<KIND>(r2, variance) * s;
+#pragma unroll
+    for (int d = 0; d < DP; ++d) g[d] = fma(w, diff[d], g[d]);
+  }
+  const double c = coef[t];
+#pragma unroll
+  for (int d = 0; d < DP; ++d) {
+    double s = g[d];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0 && d < D) grad[t * D + d] = fma(c, s * inv_ls[d], grad[t * D + d]);
+  }
+}
+
+// k(X, P) as m columns of length N (Kxp[j * N + n])
+template <int KIND>
+__global__ void __launch_bounds__(128)
+gibbon_kxp_kernel(const double* __restrict__ Xs, const double* __restrict__ Ps, int N, int DP, double variance,
+                  double* __restrict__ Kxp) {
+  const int n = blockIdx.x * 128 + threadIdx.x;
+  const int j = blockIdx.y;
+  if (n >= N) return;
+  double r2 = 0.0;
+  for (int d = 0; d < DP; ++d) {
+    const double df = Xs[(int64_t)n * DP + d] - Ps[(int64_t)j * DP + d];
+    r2 = fma(df, df, r2);
+  }
+  Kxp[(int64_t)j * N + n] = kernel_from_r2<KIND>(r2, variance);
+}
+
+// B = k(P, P) - Y^T Y, Y = Linv k(X, P) (columns of length N): the posterior covariance of the pending points; one block per entry
+template <int KIND>
+__global__ void __launch_bounds__(256)
+gibbon_pcov_kernel(const double* __restrict__ Ps, const double* __restrict__ Y, int N, int DP, int m, double variance,
+                   double* __restrict__ B) {
+  const int i = blockIdx.x, j = blockIdx.y;
+  const double* yi = Y + (int64_t)i * N;
+  const double* yj = Y + (int64_t)j * N;
+  double acc = 0.0;
+  for (int n = threadIdx.x; n < N; n += blockDim.x) acc = fma(yi[n], yj[n], acc);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  __shared__ double red[8];
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += red[w];
+    double r2 = 0.0;
+    for (int d = 0; d < DP; ++d) {
+      const double df = Ps[(int64_t)i * DP + d] - Ps[(int64_t)j * DP + d];
+      r2 = fma(df, df, r2);
+    }
+    B[(int64_t)i * m + j] = kernel_from_r2<KIND>(r2, variance) - s;
+  }
+}
+
+// What[n][i] = sum_{j<=i} W[j][n] Linv_B[i][j] for i < m, 0 for m <= i < mp  (W columns of length N)
+__global__ void __launch_bounds__(128)
+gibbon_what_kernel(const double* __restrict__ W, const double* __restrict__ LBinv, int N, int m, int mp,
+                   double* __restrict__ What) {
+  const int n = blockIdx.x * 128 + threadIdx.x;
+  const int i = blockIdx.y;
+  if (n >= N) return;
+  double acc = 0.0;
+  if (i < m)
+    for (int j = 0; j <= i; ++j) acc = fma(W[(int64_t)j * N + n], LBinv[(int64_t)i * m + j], acc);
+  What[(int64_t)n * mp + i] = acc;
+}
+
 // per-candidate partial derivatives of the acquisition w.r.t. (mean, var) from the tail inputs
 __global__ void __launch_bounds__(256)
 acq_partials_kernel(const double* __restrict__ partial, int G, int64_t McPad, const double* __restrict__ mean,
                     int64_t Mc, double variance, int acq, double param, double aux, const double* __restrict__ samp, int nsamp,
                     double* __restrict__ cmu,
-                    double* __restrict__ cvar) {
+                    double* __restrict__ cvar, const double* __restrict__ gib_uu = nullptr, double gib_w = 0.0,
+                    double* __restrict__ gib_coef = nullptr) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= Mc) return;
   double ss = 0.0;
@@ -459,8 +650,23 @@ acq_partials_kernel(const double* __restrict__ partial, int G, int64_t McPad, co
   const double raw = variance - ss;
   const bool clipped = raw < 1e-12;
   double dm, dv;
-  if (acq == TB_ACQ_MES) mes_partials(samp, nsamp, mean[t], fmax(raw, 1e-12), clipped, dm, dv);
-  else acq_partials(acq, param, aux, mean[t], fmax(raw, 1e-12), clipped, dm, dv);
+  if (acq == TB_ACQ_MES) {
+    mes_partials(samp, nsamp, mean[t], fmax(raw, 1e-12), clipped, dm, dv);
+  } else if (acq >= TB_ACQ_GIBBON_QUALITY) {
+    const double var = fmax(raw, 1e-12);
+    dm = 0.0;
+    dv = 0.0;
+    if (acq != TB_ACQ_GIBBON_REPULSION) gibbon_quality_partials(samp, nsamp, mean[t], var, aux, clipped, dm, dv);
+    if (acq != TB_ACQ_GIBBON_QUALITY) {
+      // repulsion w/2 (log V_det - log yvar), V_det = yvar - |u|^2: its var part enters through cvar; the |u|^2 part is
+      // -w / V_det times d|u|^2/dx / 2, added by gibbon_grad_kernel
+      const double yvar = var + aux, vdet = yvar - gib_uu[t];
+      if (!clipped) dv += gib_w * 0.5 * (1.0 / vdet - 1.0 / yvar);
+      gib_coef[t] = -gib_w / vdet;
+    }
+  } else {
+    acq_partials(acq, param, aux, mean[t], fmax(raw, 1e-12), clipped, dm, dv);
+  }
   cmu[t] = dm;
   cvar[t] = dv;
 }

@@ -411,6 +411,61 @@ __device__ __forceinline__ void mes_partials(const double* __restrict__ samp, in
   dvar = clipped ? 0.0 : -av / (2.0 * var * (double)ns);
 }
 
+// ---- GIBBON (entropy.py:479-500, 580-618)
+//   quality   = -1/2 mean_s log(1 + rho2 r_s (gamma_s - r_s)),  rho2 = var / (var + noise), gamma and r as for MES
+//   repulsion = w/2 (log(yvar - |u|^2) - log yvar),  yvar = var + noise,  |u|^2 = c(x)^T (B + noise I)^-1 c(x) (cross kernel)
+// The quality term is evaluated as the reference writes it: for large gamma r (gamma - r) -> -1 cancels there too.
+__device__ __forceinline__ double gibbon_quality_value(const double* __restrict__ samp, int ns, double mean, double var,
+                                                       double noise) {
+  const double rho2 = var / (var + noise);
+  const double sd = fmax(sqrt(var), MES_CLAMP_LB);
+  double acc = 0.0;
+  for (int s = 0; s < ns; ++s) {
+    const double gamma = (samp[s] - mean) / sd;
+    double lc, r;
+    mes_terms(gamma, lc, r);
+    acc += log(1.0 + rho2 * r * (gamma - r));
+  }
+  return -0.5 * (acc / (double)ns);
+}
+// d/dmean and d/dvar of the above.  With h = r (gamma - r), r' = r (r - gamma), h' = r' (gamma - r) + r (1 - r'),
+// I = 1 + rho2 h:  dq/dgamma = -rho2 h' / (2 I),  dq/drho2 = -h / (2 I),  dgamma/dmean = -1/sd,  dgamma/dvar = -gamma/(2 var),
+// drho2/dvar = noise / yvar^2; the variance partial is zero where the variance is clipped
+__device__ __forceinline__ void gibbon_quality_partials(const double* __restrict__ samp, int ns, double mean, double var,
+                                                        double noise, bool clipped, double& dmu, double& dvar) {
+  const double yvar = var + noise;
+  const double rho2 = var / yvar;
+  const double sd = fmax(sqrt(var), MES_CLAMP_LB);
+  double am = 0.0, av = 0.0, ar = 0.0;
+  for (int s = 0; s < ns; ++s) {
+    const double gamma = (samp[s] - mean) / sd;
+    double lc, r;
+    mes_terms(gamma, lc, r);
+    const double h = r * (gamma - r);
+    const double dr = r * (r - gamma);
+    const double dh = dr * (gamma - r) + r * (1.0 - dr);
+    const double inv = 1.0 / (1.0 + rho2 * h);
+    const double dg = -0.5 * rho2 * dh * inv;
+    am += dg;
+    av += dg * gamma;
+    ar += -0.5 * h * inv;
+  }
+  dmu = -am / (sd * (double)ns);
+  dvar = clipped ? 0.0 : (-av / (2.0 * var) + ar * noise / (yvar * yvar)) / (double)ns;
+}
+__device__ __forceinline__ double gibbon_repulsion_value(double var, double noise, double uu, double w) {
+  const double yvar = var + noise;
+  return w * (0.5 * (log(yvar - uu) - log(yvar)));
+}
+// kinds TB_ACQ_GIBBON_QUALITY / _REPULSION / TB_ACQ_GIBBON (repulsion + quality, entropy.py:435-436)
+__device__ __forceinline__ double gibbon_value(int acq, const double* __restrict__ samp, int ns, double mean, double var,
+                                               double noise, double uu, double w) {
+  if (acq == TB_ACQ_GIBBON_QUALITY) return gibbon_quality_value(samp, ns, mean, var, noise);
+  const double rep = gibbon_repulsion_value(var, noise, uu, w);
+  if (acq == TB_ACQ_GIBBON_REPULSION) return rep;
+  return rep + gibbon_quality_value(samp, ns, mean, var, noise);
+}
+
 // ---- local penalisation (greedy_batch.py:315-388): the base value times prod_j pen_j(||x - x_j||) over the pending points
 //   soft (:315-354): pen_j = Phi((dist - radius_j) / scale_j)
 //   hard (:357-388): pen_j = ((dist / (radius_j + scale_j))^-5 + 1)^(-1/5)
@@ -442,6 +497,8 @@ struct TailPenalty {
   const double* scale = nullptr;   // [P]
   double* grad = nullptr;          // [Mc][D] gradient of the base acquisition, turned into the penalised one in place (nullable)
   int P = 0, D = 0, kind = 0;
+  const double* gib_uu = nullptr;  // GIBBON repulsion kinds: |u|^2 [Mc] of the cross kernel, and the repulsion weight
+  double gib_w = 0.0;
 };
 
 // one thread per candidate of the chunk; block-level first-max argmax.  PEN: the value (and the gradient, when
@@ -464,7 +521,10 @@ tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const doub
     if (out_mean) out_mean[t] = mu;
     if (out_var) out_var[t] = var;
     if (acq >= 0) {
-      double v = (acq == TB_ACQ_MES) ? mes_value(samp, nsamp, mu, var) : acq_value(acq, param, aux, mu, var);
+      double v = (acq == TB_ACQ_MES) ? mes_value(samp, nsamp, mu, var)
+                 : (acq >= TB_ACQ_GIBBON_QUALITY)
+                     ? gibbon_value(acq, samp, nsamp, mu, var, aux, pen.gib_uu ? pen.gib_uu[t] : 0.0, pen.gib_w)
+                     : acq_value(acq, param, aux, mu, var);
       if (PEN) {
         vb = v;
       } else {

@@ -291,7 +291,8 @@ int tb_gp_destroy(tb_gp* gp) {
                         &gp->sVals, &gp->sVar, &gp->sXc, &gp->sBlkBest, &gp->sBlkIdx, &gp->sRun,
                         &gp->sA, &gp->sV, &gp->sGrad, &gp->sMisc, &gp->dMes, &gp->dXspare, &gp->dyspare, &gp->dLspare, &gp->dLinvSpare,
                         &gp->dAS5, &gp->dRowScale5, &gp->dRowSum5, &gp->dX2, &gp->dKinvS5, &gp->dKinvScale5, &gp->dKinvSum5,
-                        &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->sXc2})
+                        &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->sXc2, &gp->dGibPs, &gp->dGibLinv, &gp->dGibWhat,
+                        &gp->sGib})
     b->release();
   for (auto& ev : gp->prof_events) {
     cudaEventDestroy(ev.first);
@@ -417,6 +418,7 @@ static int finish_cache(tb_gp* gp, int64_t appended_from = 0) {
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
   gp->cache_valid = true;
+  ++gp->cache_gen;  // state derived from the posterior (GIBBON repulsion) is rebuilt before its next use
   gp->upper_valid = false;
   gp->oz_valid = false;
   gp->oz5_valid = false;
@@ -782,16 +784,97 @@ static void launch_grad_dp(tb_gp* gp, const double* xc, int64_t mc, double* grad
 #undef TB_GRAD
 }
 
+static inline bool gibbon_repulsion_kind(int acq) { return acq == TB_ACQ_GIBBON_REPULSION || acq == TB_ACQ_GIBBON; }
+
+#define TB_GIB_DP(LAUNCH, KIND) \
+  switch (gp->DP) {             \
+    case 2: LAUNCH(KIND, 2); break;   \
+    case 4: LAUNCH(KIND, 4); break;   \
+    case 6: LAUNCH(KIND, 6); break;   \
+    case 8: LAUNCH(KIND, 8); break;   \
+    case 10: LAUNCH(KIND, 10); break; \
+    case 12: LAUNCH(KIND, 12); break; \
+    case 16: LAUNCH(KIND, 16); break; \
+    case 20: LAUNCH(KIND, 20); break; \
+    case 24: LAUNCH(KIND, 24); break; \
+    default: LAUNCH(KIND, 32); break; \
+  }
+#define TB_GIB_KIND(LAUNCH)                           \
+  switch (gp->kernel) {                               \
+    case TB_RBF: TB_GIB_DP(LAUNCH, TB_RBF); break;           \
+    case TB_MATERN12: TB_GIB_DP(LAUNCH, TB_MATERN12); break; \
+    case TB_MATERN32: TB_GIB_DP(LAUNCH, TB_MATERN32); break; \
+    default: TB_GIB_DP(LAUNCH, TB_MATERN52); break;          \
+  }
+
+// GIBBON cross term of one chunk (ensure_gibbon has run): |u|^2 into sGib[0, mc); with keep_u also u into sGib[2 mc, ...) for
+// gibbon_grad_kernel.  One launch whatever m.
+static int launch_gibbon_cross(tb_gp* gp, cudaStream_t st, const double* xc, int64_t mc, bool keep_u) {
+  TB_TRY(gp->sGib.reserve(sizeof(double) * (size_t)mc * (2 + (keep_u ? gp->gibMp : 0))));
+  double* uu = gp->sGib.as<double>();
+  double* U = keep_u ? uu + 2 * mc : nullptr;
+  const unsigned blocks = (unsigned)((mc + 127) / 128);
+#define TB_GIB_CROSS(KIND, DPV)                                                                                                  \
+  gibbon_cross_kernel<KIND, DPV><<<blocks, 128, 0, st>>>(gp->dXs.as<double>(), gp->dGibWhat.as<double>(), gp->dGibPs.as<double>(), \
+                                                         gp->dGibLinv.as<double>(), xc, gp->dInvLs.as<double>(), (int)gp->N, gp->D,  \
+                                                         gp->gibM, gp->gibMp, mc, gp->variance, fm::Consts(), uu, U)
+  TB_GIB_KIND(TB_GIB_CROSS)
+#undef TB_GIB_CROSS
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// the |u|^2 part of the repulsion gradient, added in place to gd (device [mc][D]) after the gradient assembly
+static int launch_gibbon_grad(tb_gp* gp, cudaStream_t st, const double* xc, int64_t mc, double* gd) {
+  const double* uu = gp->sGib.as<double>();
+  const unsigned blocks = (unsigned)((mc + 7) / 8);
+#define TB_GIB_GRAD(KIND, DPV)                                                                                                  \
+  gibbon_grad_kernel<KIND, DPV><<<blocks, 256, 0, st>>>(gp->dXs.as<double>(), gp->dGibWhat.as<double>(), gp->dGibPs.as<double>(), \
+                                                        gp->dGibLinv.as<double>(), xc, gp->dInvLs.as<double>(), (int)gp->N, gp->D,  \
+                                                        gp->gibM, gp->gibMp, mc, gp->variance, uu + 2 * mc, uu + mc, gd)
+  TB_GIB_KIND(TB_GIB_GRAD)
+#undef TB_GIB_GRAD
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// d acq / d (mean, var) of one chunk into sMisc (cmu [mc], cvar [mc]); the GIBBON repulsion kinds first run the cross term
+// of the chunk, whose |u|^2 the partials and the tail read
+static int launch_partials(tb_gp* gp, cudaStream_t st, int acq, double param, const double* partial, int G, int64_t McPad,
+                           const double* mean, const double* xc, int64_t mc) {
+  double* cmu = gp->sMisc.as<double>();
+  const bool gib = gibbon_repulsion_kind(acq);
+  if (gib) TB_TRY(launch_gibbon_cross(gp, st, xc, mc, true));
+  double* g = gib ? gp->sGib.as<double>() : nullptr;
+  acq_partials_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, st>>>(partial, G, McPad, mean, mc, gp->variance, acq, param,
+                                                                    gp->noise, gp->dMes.as<double>(), gp->mesS, cmu, cmu + mc,
+                                                                    g, gp->gibW, g ? g + mc : nullptr);
+  TB_LAUNCHED();
+  return 0;
+}
+
 // The acquisition tail of one chunk.  A penalised request (rq.pen) multiplies the value, and the gradient in gd (device,
 // [mc][D], nullable) in place, by the handle's local penalty at the candidates xc (device, [mc][D]); so the tail must run
-// after the gradient assembly and before the gradient leaves the device.  Unpenalised requests run the plain tail.
-static void launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const double* partial, int G, int64_t McPad,
-                        const double* mean, int64_t mc, int64_t c0, double* d_vals, double* d_mean, double* d_var,
-                        const double* xc, double* gd) {
+// after the gradient assembly and before the gradient leaves the device.  Unpenalised requests run the plain tail.  The GIBBON
+// repulsion kinds add their term: without a gradient the cross kernel runs here; with one it ran before the partials
+// (launch_partials) and its |u|^2 gradient part is added to gd here.
+static int launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const double* partial, int G, int64_t McPad,
+                       const double* mean, int64_t mc, int64_t c0, double* d_vals, double* d_mean, double* d_var,
+                       const double* xc, double* gd) {
   const int blocks = (int)((mc + 255) / 256);
   double* bb = rq.want_argmax ? gp->sBlkBest.as<double>() : nullptr;
   int64_t* bi = rq.want_argmax ? gp->sBlkIdx.as<int64_t>() : nullptr;
   TailPenalty pen;
+  if (gibbon_repulsion_kind(rq.acq)) {
+    if (gd)
+      TB_TRY(launch_gibbon_grad(gp, st, xc, mc, gd));
+    else
+      TB_TRY(launch_gibbon_cross(gp, st, xc, mc, false));
+    pen.gib_uu = gp->sGib.as<double>();
+    pen.gib_w = gp->gibW;
+  }
   if (rq.pen) {
     pen.xc = xc;
     pen.pend = gp->dPen.as<double>();
@@ -808,6 +891,7 @@ static void launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const
                                                gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, pen);
   }
   TB_LAUNCHED();
+  return 0;
 }
 
 // after the lower GEMM (A stored as packed panels in sA, sum-of-squares in sPartial):
@@ -815,11 +899,7 @@ static void launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const
 static int gradient_chunk(tb_gp* gp, int acq, double param, const double* xc, int64_t mc, int tiles, int G,
                           int64_t McPad, double* gd) {  // gd: device [mc][D]
   cudaStream_t st = gp->stream;
-  double* cmu = gp->sMisc.as<double>();
-  acq_partials_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, st>>>(gp->sPartial.as<double>(), G, McPad,
-                                                                    gp->sMean.as<double>(), mc, gp->variance, acq,
-                                                                    param, gp->noise, gp->dMes.as<double>(), gp->mesS, cmu, cmu + mc);
-  TB_LAUNCHED();
+  TB_TRY(launch_partials(gp, st, acq, param, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), xc, mc));
   const int nkB = gp->NB * (BM / BK);
   trigemm_kernel<true, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
       gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB, nkB, G, McPad, nullptr, nullptr, gp->sV.as<double>(),
@@ -919,10 +999,7 @@ static int ensure_kinv_digits(tb_gp* gp) {
 static int gradient_chunk_oz(tb_gp* gp, int acq, double param, const double* xc, int64_t mc, int tiles, int G, int64_t McPad,
                              double* gd) {  // gd: device [mc][D]
   cudaStream_t st = gp->stream;
-  double* cmu = gp->sMisc.as<double>();
-  acq_partials_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, st>>>(gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc,
-                                                                    gp->variance, acq, param, gp->noise, gp->dMes.as<double>(), gp->mesS, cmu, cmu + mc);
-  TB_LAUNCHED();
+  TB_TRY(launch_partials(gp, st, acq, param, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), xc, mc));
   const int Gv = std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)));
   TB_TRY(oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dKinvS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dKinvScale.as<double>(), gp->NB,
                                           gp->nst, Gv, McPad, gp->oz_out_scale, oz_npass(gp), 1, nullptr, gp->sV.as<double>(),
@@ -1100,8 +1177,8 @@ static int run_eval_oz(tb_gp* gp, EvalRequest& rq) {
     double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;
     double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
     const int tb_blocks = (int)((mc + 255) / 256);
-    launch_tail(gp, sa, rq, part[slot]->as<double>(), G, McPad, mean[slot]->as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk,
-                nullptr);
+    TB_TRY(launch_tail(gp, sa, rq, part[slot]->as<double>(), G, McPad, mean[slot]->as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk,
+                       nullptr));
     if (rq.want_argmax) {
       argmax_fold_kernel<<<1, 256, 0, sa>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks,
                                             gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
@@ -1213,11 +1290,7 @@ static int run_eval_grad_oz5(tb_gp* gp, EvalRequest& rq) {
     }
     TB_TRY(oz5_launch_kstar(gp, st, xc_chunk, mc, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
     TB_TRY(oz5_launch_gemm(gp, st, gp->sKs.as<int8_t>(), tiles, G, McPad, gp->sPartial.as<double>()));
-    double* cmu = gp->sMisc.as<double>();
-    acq_partials_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, st>>>(gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc,
-                                                                      gp->variance, rq.acq, rq.param, gp->noise, gp->dMes.as<double>(), gp->mesS,
-                                                                      cmu, cmu + mc);
-    TB_LAUNCHED();
+    TB_TRY(launch_partials(gp, st, rq.acq, rq.param, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), xc_chunk, mc));
     TB_TRY(oz5_launch_gemm_store(gp, st, 1, gp->sKs.as<int8_t>(), tiles, G, gp->sV.as<double>(), ldv));
     double* gd = gdev ? rq.out_grad + c0 * D : gp->sGrad.as<double>();
     switch (gp->kernel) {
@@ -1232,7 +1305,7 @@ static int run_eval_grad_oz5(tb_gp* gp, EvalRequest& rq) {
     double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;
     double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
     const int tb_blocks = (int)((mc + 255) / 256);
-    launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd);
+    TB_TRY(launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd));
     if (!gdev) TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
     if (rq.want_argmax) {
       argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks, gp->sRun.as<double>(),
@@ -1375,7 +1448,7 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
     double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;  // sMean already holds it
     double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
     const int tb_blocks = (int)((mc + 255) / 256);
-    launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd);
+    TB_TRY(launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd));
     if (rq.out_grad && !gdev) TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
     if (rq.want_argmax) {
       argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks,
@@ -1476,6 +1549,98 @@ static int run_mean_grad(tb_gp* gp, const double* Xc, int64_t M, double* mean, d
   return 0;
 }
 
+// GIBBON repulsion state derived from the pending points and the current posterior cache (gibbon_cross_kernel):
+//   Kxp = k(X, P), Y = Linv Kxp, W = Linv^T Y = K^-1 k(X, P), B = k(P, P) - Y^T Y with its diagonal clipped at >= 1e-12
+//   (predict_joint, interface.py:126-133), L_B = chol(B + noise I) and L_B^-1 on the host (m x m), What = W L_B^-T.
+// Rebuilt only when the cache generation moved since the last build: O(N^2 m) once per pending set and posterior.
+static int ensure_gibbon(tb_gp* gp) {
+  TB_CHECK(gp->cache_valid, "GIBBON repulsion: posterior cache is not built: call tb_gp_update_posterior_cache first");
+  if (gp->gib_gen == gp->cache_gen) return 0;
+  TB_CUDA(cudaSetDevice(gp->device));
+  cudaStream_t st = gp->stream;
+  const int m = gp->gibM, D = gp->D, DP = gp->DP;
+  const int mp = ((m + GIB_TILE - 1) / GIB_TILE) * GIB_TILE;
+  const int N = (int)gp->N;
+  std::vector<double> ps((size_t)m * DP, 0.0);
+  for (int j = 0; j < m; ++j)
+    for (int d = 0; d < D; ++d) ps[(size_t)j * DP + d] = gp->gibP[(size_t)j * D + d] / gp->ls[d];
+  TB_TRY(gp->dGibPs.reserve(sizeof(double) * ps.size()));
+  TB_CUDA(cudaMemcpyAsync(gp->dGibPs.p, ps.data(), sizeof(double) * ps.size(), cudaMemcpyHostToDevice, st));
+  tb::DevBuf work;  // Kxp, Y, W [m][N] and B [m][m]
+  struct Release {
+    tb::DevBuf* b;
+    ~Release() { b->release(); }
+  } rel{&work};
+  TB_TRY(work.reserve(sizeof(double) * (3 * (size_t)m * N + (size_t)m * m)));
+  double* Kxp = work.as<double>();
+  double* Y = Kxp + (size_t)m * N;
+  double* W = Y + (size_t)m * N;
+  double* B = W + (size_t)m * N;
+  const double* Xs = gp->dXs.as<double>();
+  const double* Psd = gp->dGibPs.as<double>();
+  const double* Linv = gp->dLinv.as<double>();
+  const dim3 cols((unsigned)((N + 127) / 128), (unsigned)m);
+  switch (gp->kernel) {
+    case TB_RBF: gibbon_kxp_kernel<TB_RBF><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
+    case TB_MATERN12: gibbon_kxp_kernel<TB_MATERN12><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
+    case TB_MATERN32: gibbon_kxp_kernel<TB_MATERN32><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
+    default: gibbon_kxp_kernel<TB_MATERN52><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
+  }
+  TB_LAUNCHED();
+  trmv_lower_cols_kernel<<<cols, 128, 0, st>>>(Linv, N, N, Kxp, N, Y, N);
+  TB_LAUNCHED();
+  trmv_lower_t_cols_kernel<<<dim3((unsigned)((N + 7) / 8), (unsigned)m), 256, 0, st>>>(Linv, N, N, Y, N, W, N);
+  TB_LAUNCHED();
+  const dim3 pairs((unsigned)m, (unsigned)m);
+  switch (gp->kernel) {
+    case TB_RBF: gibbon_pcov_kernel<TB_RBF><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
+    case TB_MATERN12: gibbon_pcov_kernel<TB_MATERN12><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
+    case TB_MATERN32: gibbon_pcov_kernel<TB_MATERN32><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
+    default: gibbon_pcov_kernel<TB_MATERN52><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
+  }
+  TB_LAUNCHED();
+  std::vector<double> b((size_t)m * m);
+  TB_CUDA(cudaMemcpyAsync(b.data(), B, sizeof(double) * b.size(), cudaMemcpyDeviceToHost, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  TB_CUDA(cudaGetLastError());
+  // L_B = chol(B + noise I) (lower, in place) and its inverse, rows padded to mp with zeros
+  for (int i = 0; i < m; ++i) b[(size_t)i * m + i] = std::max(b[(size_t)i * m + i], 1e-12) + gp->noise;
+  for (int j = 0; j < m; ++j) {
+    double djj = b[(size_t)j * m + j];
+    for (int k = 0; k < j; ++k) djj -= b[(size_t)j * m + k] * b[(size_t)j * m + k];
+    TB_CHECK_CODE(djj > 0.0 && std::isfinite(djj),
+                  "GIBBON repulsion: Cholesky decomposition of the pending points' covariance plus noise was not successful "
+                  "(not positive definite at leading minor " + std::to_string(j + 1) + ")", tb::ERR_NUMERIC);
+    const double ljj = std::sqrt(djj);
+    b[(size_t)j * m + j] = ljj;
+    for (int i = j + 1; i < m; ++i) {
+      double v = b[(size_t)i * m + j];
+      for (int k = 0; k < j; ++k) v -= b[(size_t)i * m + k] * b[(size_t)j * m + k];
+      b[(size_t)i * m + j] = v / ljj;
+    }
+  }
+  std::vector<double> li((size_t)mp * m, 0.0);
+  for (int c = 0; c < m; ++c) {  // column c of L^-1 by forward substitution
+    li[(size_t)c * m + c] = 1.0 / b[(size_t)c * m + c];
+    for (int i = c + 1; i < m; ++i) {
+      double v = 0.0;
+      for (int k = c; k < i; ++k) v -= b[(size_t)i * m + k] * li[(size_t)k * m + c];
+      li[(size_t)i * m + c] = v / b[(size_t)i * m + i];
+    }
+  }
+  TB_TRY(gp->dGibLinv.reserve(sizeof(double) * li.size()));
+  TB_CUDA(cudaMemcpyAsync(gp->dGibLinv.p, li.data(), sizeof(double) * li.size(), cudaMemcpyHostToDevice, st));
+  TB_TRY(gp->dGibWhat.reserve(sizeof(double) * (size_t)N * mp));
+  gibbon_what_kernel<<<dim3((unsigned)((N + 127) / 128), (unsigned)mp), 128, 0, st>>>(W, gp->dGibLinv.as<double>(), N, m, mp,
+                                                                                    gp->dGibWhat.as<double>());
+  TB_LAUNCHED();
+  TB_CUDA(cudaStreamSynchronize(st));  // the host vectors and the work buffer go out of scope
+  TB_CUDA(cudaGetLastError());
+  gp->gibMp = mp;
+  gp->gib_gen = gp->cache_gen;
+  return 0;
+}
+
 }  // namespace tb
 
 extern "C" {
@@ -1494,10 +1659,26 @@ static int tb_gp_predict_f64(tb_gp* gp, const void* Xc, int64_t M, void* mean, v
 static int split_penalized(const tb_gp* gp, int& acq, bool& pen, const char* who) {
   pen = (acq & TB_ACQ_PENALIZED) != 0;
   acq &= ~TB_ACQ_PENALIZED;
-  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_MES, std::string(who) + ": unknown acquisition kind");
+  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_GIBBON, std::string(who) + ": unknown acquisition kind");
+  TB_CHECK(!(pen && acq >= TB_ACQ_GIBBON_QUALITY),
+           std::string(who) + ": the GIBBON kinds do not compose with TB_ACQ_PENALIZED (the repulsion term is their batch term)");
   if (pen)
     TB_CHECK(gp->penP > 0 && gp->penD == gp->D,
              std::string(who) + ": a penalised acquisition needs the local penalty first (tb_acq_set_penalization)");
+  return 0;
+}
+
+// the handle state a GIBBON kind reads: min-value samples for the quality term; pending points for the repulsion term, whose
+// derived state is brought up to date with the posterior cache here
+static int prepare_gibbon(tb_gp* gp, int acq, const char* who) {
+  if (acq < TB_ACQ_GIBBON_QUALITY) return 0;
+  if (acq != TB_ACQ_GIBBON_REPULSION)
+    TB_CHECK(gp->mesS > 0, std::string(who) + ": GIBBON's quality term needs the min-value samples first (tb_acq_set_min_value_samples)");
+  if (acq != TB_ACQ_GIBBON_QUALITY) {
+    TB_CHECK(gp->gibM > 0 && gp->gibD == gp->D,
+             std::string(who) + ": GIBBON's repulsion term needs the pending points first (tb_acq_set_gibbon_repulsion)");
+    TB_TRY(tb::ensure_gibbon(gp));
+  }
   return 0;
 }
 
@@ -1508,6 +1689,7 @@ static int tb_acq_eval_f64(tb_gp* gp, int acq, double param, const void* Xc, int
   if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
     TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
   if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
+  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_eval"));
   tb::EvalRequest rq;
   rq.acq = acq;
   rq.pen = pen;
@@ -1527,6 +1709,7 @@ static int tb_acq_argmax_f64(tb_gp* gp, int acq, double param, const void* Xc, i
   if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
     TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
   if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
+  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_argmax"));
   tb::EvalRequest rq;
   rq.acq = acq;
   rq.pen = pen;
@@ -1573,6 +1756,28 @@ int tb_acq_set_penalization(tb_gp* gp, int kind, const double* pending, int P, c
   gp->penKind = kind;
   gp->penD = gp->D;
   return 0;
+}
+
+int tb_acq_set_gibbon_repulsion(tb_gp* gp, const double* pending, int m, double weight) {
+  TB_CHECK(gp && pending, "tb_acq_set_gibbon_repulsion: null argument");
+  TB_CHECK(m > 0, "tb_acq_set_gibbon_repulsion: need at least one pending point");
+  TB_CHECK(std::isfinite(weight), "tb_acq_set_gibbon_repulsion: the repulsion weight must be finite");
+  TB_CHECK(gp->have_data, "tb_acq_set_gibbon_repulsion: the model has no data (input dimension unknown)");
+  TB_CHECK(gp->cache_valid, "tb_acq_set_gibbon_repulsion: posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_CUDA(cudaSetDevice(gp->device));
+  std::vector<double> p((size_t)m * gp->D);
+  TB_CUDA(cudaMemcpy(p.data(), pending, sizeof(double) * p.size(), cudaMemcpyDefault));
+  // the same pending set again (pushed before every launch): the derived state stays if the posterior did not move either
+  const bool same = gp->gibM == m && gp->gibD == gp->D && gp->gibP == p;
+  gp->gibW = weight;
+  if (same && gp->gib_gen == gp->cache_gen) return 0;
+  gp->gibP.swap(p);
+  gp->gibM = m;
+  gp->gibD = gp->D;
+  gp->gib_gen = ~(uint64_t)0;
+  const int rc = tb::ensure_gibbon(gp);
+  if (rc) gp->gibM = 0;  // a pending set that cannot be factorised is not kept
+  return rc;
 }
 
 int tb_gp_profile(tb_gp* gp, int enable) {
@@ -2800,6 +3005,7 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   TB_CHECK(maxiter >= 1 && maxls >= 1, "tb_acq_maximize: maxiter and maxls must be positive");
   TB_CHECK(gtol >= 0.0 && ftol >= 0.0, "tb_acq_maximize: tolerances must be non-negative");
   TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_maximize"));
   if (P == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
