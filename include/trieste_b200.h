@@ -170,6 +170,30 @@ int tb_acq_batch_mc_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const void* 
 int tb_acq_batch_mc_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double eta,
                             double jitter, void* out, void* grad);
 
+/* batch_expected_improvement.__call__ (function.py:1747-1805): the multi-point EI of Chevalier & Ginsbourger over the
+ * joint posterior of each q-batch, with q CDFs of dimension q and q² of dimension q−1 by Genz's QMC recursion
+ * (MultivariateNormalCDF, acquisition/function/utils.py:109-199).  Xc [B,q,D] (handle dtype) → out [B] (handle dtype);
+ * w [q−1,S] the Sobol points (double, host or device, column j contiguous as in eps: the same points serve both CDF
+ * dimensions, column j of a Sobol sequence being the same in every dimension).  eta is the minimisation threshold; the
+ * sign flip to the maximisation form (:1797-1803) and the hard-coded 1e-6 jitters (:1776-1783, utils.py:114) are
+ * applied inside.  2 ≤ q ≤ 32 (the reference's q = 1 fails inside MultivariateNormalCDF(dim=0)); TB_ERR_INVALID also for
+ * S < 1, a null pointer or no posterior cache; TB_ERR_NUMERIC if a matrix cannot be factorised. */
+int tb_acq_batch_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w, int S, double eta, void* out);
+
+/* The same value together with its gradient w.r.t. the query batches (what tfp.math.value_and_gradient returns under
+ * batchify_joint, optimizer.py:621-629, 897-936): the reverse pass of the Genz recursion, the small Cholesky
+ * factorisations and the Σ/c/R construction down to the adjoints of the joint mean and covariance, then the same
+ * gradient assembly as tb_acq_batch_mc_ei_grad.  out [B], grad [B,q,D]. */
+int tb_acq_batch_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w, int S, double eta, void* out,
+                         void* grad);
+
+/* MultivariateNormalCDF.__call__ (acquisition/function/utils.py:109-199): P(X ≤ x) for X ~ N(mean, cov + jitter I) by
+ * Genz's recursion over the S Sobol points w [Q−1,S] (column-contiguous; may be null for Q = 1).  x, mean [B,Q],
+ * cov [B,Q,Q] → out [B].  fp64 only; host or device pointers.  1 ≤ Q ≤ 32, S ≥ 1; TB_ERR_NUMERIC if cov + jitter I of a
+ * row is not positive definite. */
+int tb_mvn_cdf(int device, const double* x, const double* mean, const double* cov, int64_t B, int Q, const double* w,
+               int S, double jitter, double* out);
+
 /* BatchReparametrizationSampler.sample (sampler.py:208-287): → samples [B,S,q]. */
 int tb_gp_reparam_sample(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S,
                          double jitter, void* samples);

@@ -48,6 +48,9 @@ SIGNATURES = {
     "tb_acq_maximize": (_i32, [_vp, _i32, _f64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
     "tb_acq_batch_mc_ei": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _f64, _vp]),
     "tb_acq_batch_mc_ei_grad": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _f64, _vp, _vp]),
+    "tb_acq_batch_ei": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _vp]),
+    "tb_acq_batch_ei_grad": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _vp, _vp]),
+    "tb_mvn_cdf": (_i32, [_i32, _vp, _vp, _vp, _i64, _i32, _vp, _i32, _f64, _vp]),
     "tb_gp_covariance_between_points": (_i32, [_vp, _vp, _i64, _vp, _i64, _vp]),
     "tb_gp_sample_joint": (_i32, [_vp, _vp, _i64, _vp, _i32, _f64, _vp]),
     "tb_gp_reparam_sample": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _vp]),

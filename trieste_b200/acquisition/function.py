@@ -1,5 +1,5 @@
 """Analytic and Monte-Carlo single-objective acquisition functions of the hot path — mirrors
-trieste/acquisition/function/function.py (EI :96-223, LCB :328-418, batch MC-EI :1074-1186).
+trieste/acquisition/function/function.py (EI :96-223, LCB :328-418, batch MC-EI :1074-1186, batch EI :1189-1805).
 
 Each callable keeps the reference's shape contract (``x: [..., 1, D] -> [..., 1]``; batch
 functions ``[..., B, D] -> [..., 1]``) but evaluates predict + tail in ONE pass of fused GPU
@@ -758,4 +758,104 @@ class BatchMonteCarloExpectedImprovement(SingleModelAcquisitionBuilder):
             raise ValueError(f"expected a batch_monte_carlo_expected_improvement, got {function!r}")
         mean, _ = model.predict(np.asarray(dataset.query_points))
         function.update(np.min(mean, axis=0))
+        return function
+
+
+class batch_expected_improvement(AcquisitionFunctionClass):
+    """function.py:1281-1805: the multi-point EI of Chevalier & Ginsbourger, its multivariate-normal CDFs by Genz's QMC
+    recursion over ``sample_size`` Sobol points, evaluated on the device (``tb_acq_batch_ei``).  As in the reference, the
+    points and the batch size q are fixed by the first call: ``update`` draws a new skip but changes only ``eta``, and
+    a call with another q — or with q = 1, where the reference's dimension-(q-1) CDF cannot be built — raises."""
+
+    def __init__(self, sample_size: int, model, eta, jitter: float, seed: Optional[int] = None):
+        self._sample_size = int(sample_size)
+        self._jitter = jitter  # validated and kept, never used (the reference hard-codes 1e-6, :1776-1783)
+        self._model = _require_native(model)
+        self._eta = float(np.asarray(eta).reshape(-1)[0])
+        self._rng = np.random.default_rng(seed)
+        self._num_sobol_skip = self._draw_skip()
+        self._q: Optional[int] = None
+        self._w: Optional[np.ndarray] = None  # [q-1, S], drawn at the first call
+
+    def _draw_skip(self) -> int:
+        return int(np.floor(1e9 * self._rng.random(dtype=np.float32)))  # :1306, :1313
+
+    def update(self, eta) -> None:
+        self._eta = float(np.asarray(eta).reshape(-1)[0])
+        self._num_sobol_skip = self._draw_skip()
+
+    @property
+    def eta(self) -> float:
+        return self._eta
+
+    def _prepare(self, x):
+        x, _ = _lib.as_contiguous(x, self._model.dtype)
+        if x.ndim < 2:
+            raise ValueError(f"expected [..., B, D] query batches, got shape {tuple(x.shape)}")
+        self._model._check_dim(x)
+        flat, lead = _flatten_leading(x, 2)
+        q = flat.shape[1]
+        if self._q is None:
+            self._q = q
+        if q != self._q:
+            raise ValueError(f"batch_expected_improvement was first called with batch size {self._q}; got {q}")
+        if q < 2:
+            raise ValueError("batch_expected_improvement needs a batch size of at least 2 (its CDFs have dimension q - 1)")
+        if self._w is None:
+            from ..sampler import sobol_points
+
+            self._w = np.ascontiguousarray(sobol_points(self._sample_size, q - 1, self._num_sobol_skip).T)
+        return flat, lead
+
+    def __call__(self, x):
+        flat, lead = self._prepare(x)
+        nb, q = flat.shape[0], flat.shape[1]
+        out, po = _lib.empty_like_kind(flat, (nb, 1), self._model.dtype)
+        _lib.check(_lib.lib().tb_acq_batch_ei(self._model.handle, _ptr(flat), nb, q, self._w.ctypes.data,
+                                              self._sample_size, self._eta, po))
+        return out.reshape(lead + (1,))
+
+    def value_and_gradient(self, x):
+        """[..., B, D] -> (values [..., 1], d values / d x [..., B, D]), the reverse pass of ``__call__``."""
+        flat, lead = self._prepare(x)
+        nb, q, D = flat.shape
+        out, po = _lib.empty_like_kind(flat, (nb, 1), self._model.dtype)
+        grad, pg = _lib.empty_like_kind(flat, (nb, q, D), self._model.dtype)
+        _lib.check(_lib.lib().tb_acq_batch_ei_grad(self._model.handle, _ptr(flat), nb, q, self._w.ctypes.data,
+                                                   self._sample_size, self._eta, po, pg))
+        return out.reshape(lead + (1,)), grad.reshape(lead + (q, D))
+
+
+class BatchExpectedImprovement(SingleModelAcquisitionBuilder):
+    """function.py:1189-1278: eta = min over the data of the posterior mean.  ``seed`` makes the Sobol skip draws
+    reproducible."""
+
+    def __init__(self, sample_size: int, *, jitter: float = JITTER, seed: Optional[int] = None):
+        if sample_size <= 0:
+            raise ValueError(f"sample_size must be positive, got {sample_size}")
+        if jitter < 0:
+            raise ValueError(f"jitter must be non-negative, got {jitter}")
+        self._sample_size = sample_size
+        self._jitter = jitter
+        self._seed = seed
+
+    def __repr__(self) -> str:
+        return f"BatchExpectedImprovement({self._sample_size!r}, jitter={self._jitter!r})"
+
+    @staticmethod
+    def _eta(model, dataset: Optional[Dataset]) -> float:
+        dataset = _check_populated(dataset)
+        mean, _ = model.predict(np.asarray(dataset.query_points))
+        if mean.shape[-1] != 1:
+            raise ValueError("Expected model with event shape [1].")
+        return float(np.min(mean, axis=0)[0])
+
+    def prepare_acquisition_function(self, model, dataset: Optional[Dataset] = None):
+        return batch_expected_improvement(self._sample_size, model, self._eta(model, dataset), self._jitter, seed=self._seed)
+
+    def update_acquisition_function(self, function, model, dataset: Optional[Dataset] = None):
+        eta = self._eta(model, dataset)
+        if not isinstance(function, batch_expected_improvement):
+            raise ValueError(f"expected a batch_expected_improvement function, got {function!r}")
+        function.update(eta)
         return function

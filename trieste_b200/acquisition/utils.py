@@ -1,4 +1,5 @@
-"""``split_acquisition_function`` / ``split_acquisition_function_calls`` — mirrors trieste/acquisition/utils.py:31-109.
+"""``split_acquisition_function`` / ``split_acquisition_function_calls`` — mirrors trieste/acquisition/utils.py:31-109 —
+and ``MultivariateNormalCDF`` (acquisition/function/utils.py:29-199).
 
 In the reference these wrappers bound the memory of one TensorFlow evaluation by cutting the leading (candidate) axis into
 blocks.  Here the fused kernels already stream any batch through bounded scratch (``run_eval`` / ``run_eval_oz`` chunk at
@@ -56,3 +57,47 @@ def split_acquisition_function_calls(optimizer, split_size: int):
         return optimizer(search_space, (taf, n) if isinstance(f, tuple) else taf)
 
     return split_optimizer
+
+
+class MultivariateNormalCDF:
+    """acquisition/function/utils.py:29-199: the CDF of a multivariate Gaussian by Genz's QMC recursion over
+    ``sample_size`` Sobol points (``skip = num_sobol_skip``), evaluated on the device (``tb_mvn_cdf``, fp64; results are
+    returned in ``dtype``).  The points are drawn once, on construction."""
+
+    def __init__(self, sample_size: int, dim: int, dtype=np.float64, num_sobol_skip: int = 0):
+        if sample_size <= 0:
+            raise ValueError(f"sample_size must be positive, got {sample_size}")
+        if dim <= 0:
+            raise ValueError(f"dim must be positive, got {dim}")
+        from ..sampler import sobol_points
+
+        self._S = int(sample_size)
+        self._Q = int(dim)
+        self._dtype = np.dtype(dtype)
+        self._num_sobol_skip = int(num_sobol_skip)
+        # [Q-1, S] column-contiguous; column j of the Sobol sequence is the same in every dimension
+        self._w = np.ascontiguousarray(sobol_points(self._S, self._Q - 1, self._num_sobol_skip).T)
+
+    def __call__(self, x, mean, cov, jitter: float = 1e-6):
+        """x, mean [B, Q], cov [B, Q, Q] -> [B]."""
+        from .. import _lib
+
+        x, px = _lib.as_contiguous(x)
+        mean, pm = _lib.as_contiguous(mean)
+        cov, pc = _lib.as_contiguous(cov)
+        B = x.shape[0]
+        if B <= 0:
+            raise ValueError("MultivariateNormalCDF needs at least one row")
+        Q = self._Q
+        if tuple(x.shape) != (B, Q) or tuple(mean.shape) != (B, Q) or tuple(cov.shape) != (B, Q, Q):
+            raise ValueError(f"expected x, mean [B, {Q}] and cov [B, {Q}, {Q}], got {tuple(x.shape)}, "
+                             f"{tuple(mean.shape)}, {tuple(cov.shape)}")
+        device = (x.device.index or 0) if _lib.is_torch(x) and x.is_cuda else 0
+        out, po = _lib.empty_like_kind(x, (B,))
+        _lib.check(_lib.lib().tb_mvn_cdf(device, px, pm, pc, B, Q, self._w.ctypes.data if Q > 1 else None, self._S,
+                                         float(jitter), po))
+        if isinstance(out, np.ndarray):
+            return out.astype(self._dtype)
+        import torch
+
+        return out.to(torch.float32 if self._dtype == np.float32 else torch.float64)

@@ -161,6 +161,74 @@ joint_kernel(const double* __restrict__ Aplain, int64_t lda, int Nrows,  // [can
   }
 }
 
+// In-place Cholesky (lower) of the n x n row-major matrix A by one warp, as in joint_kernel: lane 0 takes the pivot, the
+// lanes split the column below it.  The strict upper triangle is left as it was and never read back.  False when a
+// pivot is not positive (the result is then meaningless).
+__device__ __forceinline__ bool warp_cholesky(double* A, int n, int lane) {
+  bool bad = false;
+  for (int j = 0; j < n; ++j) {
+    double djj = 0.0;
+    if (lane == 0) {
+      double sdiag = A[j * n + j];
+      for (int k = 0; k < j; ++k) sdiag = fma(-A[j * n + k], A[j * n + k], sdiag);
+      djj = sqrt(sdiag);
+      A[j * n + j] = djj;
+    }
+    djj = __shfl_sync(0xffffffffu, djj, 0);
+    if (!(djj > 0.0)) bad = true;
+    __syncwarp();
+    for (int i = j + 1 + lane; i < n; i += 32) {
+      double v = A[i * n + j];
+      for (int k = 0; k < j; ++k) v = fma(-A[i * n + k], A[j * n + k], v);
+      A[i * n + j] = v / djj;
+    }
+    __syncwarp();
+  }
+  return !bad;
+}
+
+// Cholesky reverse mode (Murray 2016, tf.linalg.cholesky's gradient) by one warp: C the lower factor, G the adjoint of
+// its lower triangle on entry and the symmetric adjoint of the factorised matrix, C^-T sym(Phi(C^T G)) C^-1, on exit
+// (Phi = lower triangle with the diagonal halved).  T is n x n scratch.
+__device__ __forceinline__ void warp_cholesky_backward(const double* C, double* G, double* T, int n, int lane) {
+  const int nn = n * n;
+  // P = Phi(C^T G) (lower, diagonal halved) -> T
+  for (int e = lane; e < nn; e += 32) {
+    const int a = e / n, c = e % n;
+    double v = 0.0;
+    if (a >= c) {
+      for (int i = a; i < n; ++i) v = fma(C[i * n + a], G[i * n + c], v);
+      if (a == c) v *= 0.5;
+    }
+    T[e] = v;
+  }
+  __syncwarp();
+  // M = (P + P^T) / 2 (symmetric) -> G
+  for (int e = lane; e < nn; e += 32) {
+    const int a = e / n, c = e % n;
+    G[e] = (a == c) ? T[e] : 0.5 * (a > c ? T[a * n + c] : T[c * n + a]);
+  }
+  __syncwarp();
+  // T1 = C^-T M: back substitution of C^T T1 = M, lane = column -> T
+  for (int c = lane; c < n; c += 32) {
+    for (int a = n - 1; a >= 0; --a) {
+      double v = G[a * n + c];
+      for (int i = a + 1; i < n; ++i) v = fma(-C[i * n + a], T[i * n + c], v);
+      T[a * n + c] = v / C[a * n + a];
+    }
+  }
+  __syncwarp();
+  // result = T1 C^-1: row r solves C^T x = T1[r][:]^T, lane = row -> G
+  for (int r = lane; r < n; r += 32) {
+    for (int a = n - 1; a >= 0; --a) {
+      double v = T[r * n + a];
+      for (int i = a + 1; i < n; ++i) v = fma(-C[i * n + a], G[r * n + i], v);
+      G[r * n + a] = v / C[a * n + a];
+    }
+  }
+  __syncwarp();
+}
+
 // ------------------------------------------------------------------------------------------------
 // K2g: reverse pass of the batch Monte-Carlo EI of one q-batch (function.py:1181-1186 through sampler.py:262-287), i.e.
 // what TensorFlow's autodiff produces for  mean_s max(eta - min_j (mu + C eps_s)_j, 0),  C = chol(cov + jitter I):
@@ -195,27 +263,7 @@ qei_backward_kernel(const double* __restrict__ mean_in, const double* __restrict
     gmu[e] = 0.0;
   }
   __syncwarp();
-  // in-place Cholesky (lower), as in joint_kernel
-  bool bad = false;
-  for (int j = 0; j < q; ++j) {
-    double djj = 0.0;
-    if (lane == 0) {
-      double sdiag = Cs[j * q + j];
-      for (int k = 0; k < j; ++k) sdiag = fma(-Cs[j * q + k], Cs[j * q + k], sdiag);
-      djj = sqrt(sdiag);
-      Cs[j * q + j] = djj;
-    }
-    djj = __shfl_sync(0xffffffffu, djj, 0);
-    if (!(djj > 0.0)) bad = true;
-    __syncwarp();
-    for (int i = j + 1 + lane; i < q; i += 32) {
-      double v = Cs[i * q + j];
-      for (int k = 0; k < j; ++k) v = fma(-Cs[i * q + k], Cs[j * q + k], v);
-      Cs[i * q + j] = v / djj;
-    }
-    __syncwarp();
-  }
-  if (bad) {
+  if (!warp_cholesky(Cs, q, lane)) {
     if (lane == 0) atomicExch(err_flag, 1);
     return;
   }
@@ -243,41 +291,7 @@ qei_backward_kernel(const double* __restrict__ mean_in, const double* __restrict
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   __syncwarp();
-  // P = Phi(C^T G) (lower, diagonal halved) -> Ts
-  for (int e = lane; e < qq; e += 32) {
-    const int a = e / q, c = e % q;
-    double v = 0.0;
-    if (a >= c) {
-      for (int i = a; i < q; ++i) v = fma(Cs[i * q + a], Gs[i * q + c], v);
-      if (a == c) v *= 0.5;
-    }
-    Ts[e] = v;
-  }
-  __syncwarp();
-  // M = (P + P^T) / 2 (symmetric) -> Gs
-  for (int e = lane; e < qq; e += 32) {
-    const int a = e / q, c = e % q;
-    Gs[e] = (a == c) ? Ts[e] : 0.5 * (a > c ? Ts[a * q + c] : Ts[c * q + a]);
-  }
-  __syncwarp();
-  // T1 = C^-T M: back substitution of C^T T1 = M, lane = column -> Ts
-  for (int c = lane; c < q; c += 32) {
-    for (int a = q - 1; a >= 0; --a) {
-      double v = Gs[a * q + c];
-      for (int i = a + 1; i < q; ++i) v = fma(-Cs[i * q + a], Ts[i * q + c], v);
-      Ts[a * q + c] = v / Cs[a * q + a];
-    }
-  }
-  __syncwarp();
-  // Sigma_bar = T1 C^-1: row r solves C^T x = T1[r][:]^T, lane = row -> Gs
-  for (int r = lane; r < q; r += 32) {
-    for (int a = q - 1; a >= 0; --a) {
-      double v = Ts[r * q + a];
-      for (int i = a + 1; i < q; ++i) v = fma(-Cs[i * q + a], Gs[r * q + i], v);
-      Gs[r * q + a] = v / Cs[a * q + a];
-    }
-  }
-  __syncwarp();
+  warp_cholesky_backward(Cs, Gs, Ts, q, lane);
   if (lane == 0) out_val[b] = acc * invS;
   for (int e = lane; e < q; e += 32) {
     cmu[t0 + e] = gmu[e];

@@ -2,6 +2,7 @@
 // runs in the kernels of kernels_f64.cuh / kernels_extra.cuh.
 #include "gp_handle.cuh"
 #include "kernels_extra.cuh"
+#include "batch_ei.cuh"
 #include "ozaki.cuh"
 #include "oz5_api.h"
 #include <chrono>
@@ -1856,11 +1857,11 @@ int tb_gp_profile_read(tb_gp* gp, double* trigemm_ms, int64_t* trigemm_launches,
 namespace tb {
 
 struct JointRequest {
-  int mode = JOINT_PREDICT;
+  int mode = JOINT_PREDICT;  // or JOINT_BEI: mean / cov into scratch, then bei_kernel into out_qei
   const double* Xc = nullptr;  // [B, q, D]
   int64_t B = 0;
   int q = 0;
-  const double* eps = nullptr;  // [q, S] host or device
+  const double* eps = nullptr;  // [q, S] host or device (JOINT_BEI: the Sobol points w [q-1, S])
   int S = 0;
   double eta = 0.0, jitter = 0.0;
   double* out_mean = nullptr;     // [B, q]
@@ -1926,15 +1927,34 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
   TB_TRY(gp->sMean.reserve(sizeof(double) * tiles_cap * nt));
   const bool xc_dev = is_device_ptr(rq.Xc);
   if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * cand_cap * D));
+  const bool bei = rq.mode == JOINT_BEI;
+  const int eps_rows = bei ? q - 1 : q;
   const double* eps_dev = nullptr;
   if (rq.mode != JOINT_PREDICT) {
     if (is_device_ptr(rq.eps)) {
       eps_dev = rq.eps;
     } else {
-      TB_TRY(gp->sMisc.reserve(sizeof(double) * (size_t)q * rq.S + 64));
-      TB_CUDA(cudaMemcpyAsync(gp->sMisc.p, rq.eps, sizeof(double) * (size_t)q * rq.S, cudaMemcpyHostToDevice, st));
+      TB_TRY(gp->sMisc.reserve(sizeof(double) * (size_t)eps_rows * rq.S + 64));
+      TB_CUDA(cudaMemcpyAsync(gp->sMisc.p, rq.eps, sizeof(double) * (size_t)eps_rows * rq.S, cudaMemcpyHostToDevice, st));
       eps_dev = gp->sMisc.as<double>();
     }
+  }
+  // JOINT_BEI: the chunk's joint posterior stays on the device for bei_kernel
+  tb::DevBuf bmu, bcov;
+  struct Release {
+    tb::DevBuf *a, *b;
+    ~Release() { a->release(); b->release(); }
+  } rel{&bmu, &bcov};
+  JointRequest jpredict = rq;
+  jpredict.mode = JOINT_PREDICT;
+  size_t smem_bei = 0;
+  int bei_warps = 0;
+  if (bei) {
+    TB_TRY(bmu.reserve(sizeof(double) * (size_t)cand_cap));
+    TB_TRY(bcov.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
+    bei_warps = std::min(BEI_MAX_WARPS, q + q * q);
+    smem_bei = (bei_cta_doubles(q) + (size_t)bei_warps * bei_warp_doubles(q)) * sizeof(double);
+    TB_CUDA(cudaFuncSetAttribute(bei_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bei));
   }
   TB_TRY(gp->sRun.reserve(16));
   int* err = reinterpret_cast<int*>(gp->sRun.p);
@@ -1990,11 +2010,20 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
     }
     const int blocks = (int)((nbc + JOINT_WARPS - 1) / JOINT_WARPS);
     const int Nrows = (int)lda;
+    const JointRequest& jr = bei ? jpredict : rq;
+    double* om = bei ? bmu.as<double>() : dptr[0];
+    double* oc = bei ? bcov.as<double>() : dptr[1];
+    double* oq = bei ? nullptr : dptr[3];
     switch (gp->kernel) {
-      case TB_RBF: TB_TRY(launch_joint<TB_RBF>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, rq, eps_dev, dptr[0], dptr[1], dptr[2], dptr[3], err)); break;
-      case TB_MATERN12: TB_TRY(launch_joint<TB_MATERN12>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, rq, eps_dev, dptr[0], dptr[1], dptr[2], dptr[3], err)); break;
-      case TB_MATERN32: TB_TRY(launch_joint<TB_MATERN32>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, rq, eps_dev, dptr[0], dptr[1], dptr[2], dptr[3], err)); break;
-      default: TB_TRY(launch_joint<TB_MATERN52>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, rq, eps_dev, dptr[0], dptr[1], dptr[2], dptr[3], err)); break;
+      case TB_RBF: TB_TRY(launch_joint<TB_RBF>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
+      case TB_MATERN12: TB_TRY(launch_joint<TB_MATERN12>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
+      case TB_MATERN32: TB_TRY(launch_joint<TB_MATERN32>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
+      default: TB_TRY(launch_joint<TB_MATERN52>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
+    }
+    if (bei) {
+      bei_kernel<<<(unsigned)nbc, bei_warps * 32, smem_bei, st>>>(om, oc, q, eps_dev, rq.S, rq.eta, dptr[3], err);
+      TB_LAUNCHED();
+      TB_CUDA(cudaGetLastError());
     }
     for (auto& o : outs)
       if (o.user && !is_device_ptr(o.user))
@@ -2249,20 +2278,26 @@ static int run_sample_joint(tb_gp* gp, const double* Xc, int64_t M, const double
   return 0;
 }
 
-// ---- value AND gradient of the batch Monte-Carlo EI (reverse pass of function.py:1181-1186) ----
-// chunk pipeline: K* digits -> A = Linv K* (stored) -> per-batch mean / cov (joint_kernel) -> qei_backward_kernel
+// ---- value AND gradient of a batch acquisition of the joint posterior ----
+// chunk pipeline: K* digits -> A = Linv K* (stored) -> per-batch mean / cov (joint_kernel) -> the tail's reverse kernel
 // (value, G_mu, Sigma_bar) -> V = K^-1 K* (dense digit GEMM over the same K* digits) -> per-batch mix V~ = Sigma_bar V
-// -> grad_kernel (the training-point sums) -> qei_cross_kernel (the K(x_b, x_b) term).
+// -> grad_kernel (the training-point sums) -> qei_cross_kernel (the K(x_b, x_b) term).  Tails:
+//   QEI_TAIL_MC   qei_backward_kernel: batch Monte-Carlo EI (function.py:1181-1186), eps [q, S] normal base samples
+//   QEI_TAIL_GENZ bei_backward_kernel: batch EI (function.py:1747-1805), eps = the Sobol points w [q-1, S]
 template <int KIND>
 static void launch_qei_cross(tb_gp* gp, const double* xc, int64_t npts, int q, const double* sbar, double* grad) {
   qei_cross_kernel<KIND><<<(unsigned)((npts + 127) / 128), 128, 0, gp->stream>>>(xc, gp->dInvLs.as<double>(), gp->D, npts, q, sbar,
                                                                                  gp->variance, grad);
 }
 
+enum { QEI_TAIL_MC = 0, QEI_TAIL_GENZ = 1 };
+
 static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const double* eps, int S, double eta, double jitter,
-                        double* out_val, double* out_grad) {
+                        double* out_val, double* out_grad, int tail = QEI_TAIL_MC) {
   TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
   TB_CHECK(q >= 1 && q <= 32, "batch size q must be in [1, 32]");
+  const bool genz = tail == QEI_TAIL_GENZ;
+  const int eps_rows = genz ? q - 1 : q;
   TB_CHECK(B >= 0, "negative batch count");
   TB_CHECK(S >= 1 && eps, "need S >= 1 base samples");
   TB_CHECK(jitter >= 0.0, "jitter must be non-negative");
@@ -2314,8 +2349,8 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
   } rel{{&beps, &bcov, &bmu, &bsbar, &bval}};
   const double* eps_dev = eps;
   if (!is_device_ptr(eps)) {
-    TB_TRY(beps.reserve(sizeof(double) * (size_t)q * S));
-    TB_CUDA(cudaMemcpyAsync(beps.p, eps, sizeof(double) * (size_t)q * S, cudaMemcpyHostToDevice, st));
+    TB_TRY(beps.reserve(sizeof(double) * (size_t)eps_rows * S));
+    TB_CUDA(cudaMemcpyAsync(beps.p, eps, sizeof(double) * (size_t)eps_rows * S, cudaMemcpyHostToDevice, st));
     eps_dev = beps.as<double>();
   }
   TB_TRY(bcov.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
@@ -2326,8 +2361,18 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
   int* err = reinterpret_cast<int*>(gp->sRun.p);
   TB_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
   const size_t smem_joint = (size_t)JOINT_WARPS * (QP * QP + QP * D + QP) * sizeof(double);
-  const size_t smem_back = (size_t)QEIG_WARPS * (3 * q * q + 2 * q) * sizeof(double);
-  TB_CUDA(cudaFuncSetAttribute(qei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_back));
+  size_t smem_back;
+  int bei_warps = 0;
+  if (genz) {
+    // as many warps (up to 4) as fit: one per unit CDF in flight, each with its per-sample state in shared memory
+    const size_t cta = bei_cta_doubles(q) * sizeof(double), per_warp = bei_back_warp_doubles(q) * sizeof(double);
+    bei_warps = (int)std::min<size_t>(std::min<size_t>(BEI_MAX_WARPS, q + q * q), (227 * 1024 - cta) / per_warp);
+    smem_back = cta + bei_warps * per_warp;
+    TB_CUDA(cudaFuncSetAttribute(bei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_back));
+  } else {
+    smem_back = (size_t)QEIG_WARPS * (3 * q * q + 2 * q) * sizeof(double);
+    TB_CUDA(cudaFuncSetAttribute(qei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_back));
+  }
   JointRequest jr;
   jr.mode = JOINT_PREDICT;
   jr.q = q;
@@ -2394,8 +2439,13 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
     }
     double* cmu = gp->sMisc.as<double>();
     double* dval = val_dev ? out_val + b0 : bval.as<double>();
-    qei_backward_kernel<<<(unsigned)((nbc + QEIG_WARPS - 1) / QEIG_WARPS), QEIG_WARPS * 32, smem_back, st>>>(
-        dmu, dcov, nbc, q, eps_dev, S, eta, jitter, dval, cmu, cmu + mc, bsbar.as<double>(), err);
+    if (genz) {
+      bei_backward_kernel<<<(unsigned)nbc, bei_warps * 32, smem_back, st>>>(dmu, dcov, q, eps_dev, S, eta, dval, cmu, cmu + mc,
+                                                                           bsbar.as<double>(), err);
+    } else {
+      qei_backward_kernel<<<(unsigned)((nbc + QEIG_WARPS - 1) / QEIG_WARPS), QEIG_WARPS * 32, smem_back, st>>>(
+          dmu, dcov, nbc, q, eps_dev, S, eta, jitter, dval, cmu, cmu + mc, bsbar.as<double>(), err);
+    }
     TB_LAUNCHED();
     qei_mix_kernel<<<dim3((unsigned)nbc, (unsigned)((gp->N + 255) / 256)), 256, 0, st>>>(gp->sV.as<double>(), lda, (int)gp->N, q,
                                                                                         bsbar.as<double>());
@@ -3178,6 +3228,109 @@ int tb_acq_batch_mc_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const v
   TB_TRY(br.out(grad, B * q * gp->D, &gd));
   TB_TRY(tb::run_qei_grad(gp, xd, B, q, ed, S, eta, jitter, od, gd));
   return br.finish();
+}
+
+// ---- batch expected improvement (Chevalier & Ginsbourger with Genz CDFs) ----
+static int bei_args(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w, int S, const void* out, const void* grad,
+                    bool want_grad, const char* fn) {
+  TB_CHECK(gp && w && (B == 0 || (Xc && out && (!want_grad || grad))), std::string(fn) + ": null argument");
+  TB_CHECK(q >= 2 && q <= 32, std::string(fn) + ": batch size q must be in [2, 32]");
+  TB_CHECK(S >= 1, std::string(fn) + ": need S >= 1 Sobol points");
+  TB_CHECK(B >= 0, std::string(fn) + ": negative batch count");
+  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  return 0;
+}
+
+int tb_acq_batch_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w, int S, double eta, void* out) {
+  TB_TRY(bei_args(gp, Xc, B, q, w, S, out, nullptr, false, "tb_acq_batch_ei"));
+  if (B == 0) return 0;
+  tb::JointRequest rq;
+  rq.mode = tb::JOINT_BEI;
+  rq.B = B;
+  rq.q = q;
+  rq.eps = w;
+  rq.S = S;
+  rq.eta = eta;
+  if (gp->dtype == TB_F64) {
+    rq.Xc = (const double*)Xc;
+    rq.out_qei = (double*)out;
+    return tb::run_joint(gp, rq);
+  }
+  TB_CUDA(cudaSetDevice(gp->device));
+  tb::F32Bridge br(gp);
+  TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
+  TB_TRY(br.out(out, B, &rq.out_qei));
+  TB_TRY(tb::run_joint(gp, rq));
+  return br.finish();
+}
+
+int tb_acq_batch_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w, int S, double eta, void* out,
+                         void* grad) {
+  TB_TRY(bei_args(gp, Xc, B, q, w, S, out, grad, true, "tb_acq_batch_ei_grad"));
+  if (B == 0) return 0;
+  if (gp->dtype == TB_F64)
+    return tb::run_qei_grad(gp, (const double*)Xc, B, q, w, S, eta, 0.0, (double*)out, (double*)grad, tb::QEI_TAIL_GENZ);
+  TB_CUDA(cudaSetDevice(gp->device));
+  tb::F32Bridge br(gp);
+  const double* xd;
+  double *od, *gd;
+  TB_TRY(br.in(Xc, B * q * gp->D, &xd));
+  TB_TRY(br.out(out, B, &od));
+  TB_TRY(br.out(grad, B * q * gp->D, &gd));
+  TB_TRY(tb::run_qei_grad(gp, xd, B, q, w, S, eta, 0.0, od, gd, tb::QEI_TAIL_GENZ));
+  return br.finish();
+}
+
+int tb_mvn_cdf(int device, const double* x, const double* mean, const double* cov, int64_t B, int Q, const double* w, int S,
+               double jitter, double* out) {
+  TB_CHECK(B >= 0, "tb_mvn_cdf: negative batch count");
+  TB_CHECK(B == 0 || (x && mean && cov && out), "tb_mvn_cdf: null argument");
+  TB_CHECK(Q >= 1 && Q <= 32, "tb_mvn_cdf: dimension Q must be in [1, 32]");
+  TB_CHECK(Q == 1 || w, "tb_mvn_cdf: Q >= 2 needs the Sobol points w [Q-1, S]");
+  TB_CHECK(S >= 1, "tb_mvn_cdf: need S >= 1 Sobol points");
+  if (B == 0) return 0;
+  TB_CUDA(cudaSetDevice(device));
+  tb::DevBuf bx, bm, bc, bw, bo, berr;
+  struct Release {
+    std::vector<tb::DevBuf*> v;
+    ~Release() { for (auto* b : v) b->release(); }
+  } rel{{&bx, &bm, &bc, &bw, &bo, &berr}};
+  auto stage = [](tb::DevBuf& buf, const double* p, size_t n, const double** dev) -> int {
+    if (!p || is_device_ptr(p)) {
+      *dev = p;
+      return 0;
+    }
+    TB_TRY(buf.reserve(sizeof(double) * n));
+    TB_CUDA(cudaMemcpy(buf.p, p, sizeof(double) * n, cudaMemcpyHostToDevice));
+    *dev = buf.as<double>();
+    return 0;
+  };
+  const double *xd, *md, *cd, *wd;
+  TB_TRY(stage(bx, x, (size_t)B * Q, &xd));
+  TB_TRY(stage(bm, mean, (size_t)B * Q, &md));
+  TB_TRY(stage(bc, cov, (size_t)B * Q * Q, &cd));
+  TB_TRY(stage(bw, Q >= 2 ? w : nullptr, (size_t)(Q - 1) * S, &wd));
+  const bool odev = is_device_ptr(out);
+  double* od = out;
+  if (!odev) {
+    TB_TRY(bo.reserve(sizeof(double) * B));
+    od = bo.as<double>();
+  }
+  TB_TRY(berr.reserve(sizeof(int)));
+  TB_CUDA(cudaMemset(berr.p, 0, sizeof(int)));
+  const size_t smem = (size_t)tb::BEI_MAX_WARPS * tb::bei_warp_doubles(Q) * sizeof(double);
+  TB_CUDA(cudaFuncSetAttribute(tb::mvn_cdf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  tb::mvn_cdf_kernel<<<(unsigned)((B + tb::BEI_MAX_WARPS - 1) / tb::BEI_MAX_WARPS), tb::BEI_MAX_WARPS * 32, smem>>>(
+      xd, md, cd, B, Q, wd, S, jitter, od, berr.as<int>());
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  int herr = 0;
+  TB_CUDA(cudaMemcpy(&herr, berr.p, sizeof(int), cudaMemcpyDeviceToHost));
+  if (!odev) TB_CUDA(cudaMemcpy(out, od, sizeof(double) * B, cudaMemcpyDeviceToHost));
+  TB_CUDA(cudaDeviceSynchronize());
+  TB_CHECK_CODE(herr == 0, "Cholesky decomposition was not successful. The input might not be valid "
+                      "(cov + jitter*I of a row is not positive definite)", tb::ERR_NUMERIC);
+  return 0;
 }
 
 int tb_gp_reparam_sample(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double jitter,

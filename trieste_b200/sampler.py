@@ -44,6 +44,21 @@ def qmc_normal_samples(num_samples: int, n_sample_dim: int, skip: int = 0, dtype
     return ndtri(gen.random(int(num_samples))).astype(dtype)
 
 
+def sobol_points(num_samples: int, dim: int, skip: int = 0) -> np.ndarray:
+    """``tf.math.sobol_sample(dim, num_samples, skip=skip)`` as MultivariateNormalCDF draws it (utils.py:147-152):
+    [num_samples, dim] points of the unscrambled Sobol sequence, on the convention of :func:`qmc_normal_samples` (first
+    point after ``fast_forward(skip + 1)``, never the origin) but without the normal quantile.  Column j is the same
+    sequence whatever ``dim`` is, so a dimension-(q-1) draw holds the points of every CDF of dimension q or q-1.
+    ``fast_forward`` is linear in ``skip`` (about 2 s at the largest skip, 1e9)."""
+    if num_samples == 0 or dim == 0:
+        return np.zeros((num_samples, dim))
+    from scipy.stats import qmc
+
+    gen = qmc.Sobol(d=int(dim), scramble=False)
+    gen.fast_forward(int(skip) + 1)
+    return gen.random(int(num_samples))
+
+
 class IndependentReparametrizationSampler:
     """sampler.py:82-164: ``x -> mu(x) + eps * sigma(x)`` with base samples eps [S, 1] fixed until
     :meth:`reset_sampler`; batch size one only.  One batched GPU ``predict`` per call; the S-fold broadcast is host
