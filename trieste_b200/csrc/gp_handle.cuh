@@ -128,6 +128,9 @@ struct tb_gp {
   uint64_t gib_gen = ~(uint64_t)0;      // cache_gen the derived GIBBON state was built for
   tb::DevBuf dGibPs, dGibLinv, dGibWhat;
   tb::DevBuf sGib;                      // per chunk: |u|^2 [mc], -w / V_det [mc], u [mp][mc] (gradient path)
+  // screened argmax (tb_api.cu, argmax_screened): means of all M candidates, the survivors' coordinates / means / global
+  // indices, and the screen's per-block winners + probe pair + survivor count
+  tb::DevBuf sScrMean, sScrX, sScrMu, sScrIdx, sScrBlk;
 
   // profiling of the dominant kernel
   bool profile = false;

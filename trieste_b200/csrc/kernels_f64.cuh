@@ -501,14 +501,37 @@ struct TailPenalty {
   double gib_w = 0.0;
 };
 
+// first-max of the block's (value, index) pairs (blockDim.x <= 256) -> blk_best / blk_idx[blockIdx.x]
+__device__ __forceinline__ void block_best_store(double bv, int64_t bi, double* __restrict__ blk_best, int64_t* __restrict__ blk_idx) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    double v2 = __shfl_xor_sync(0xffffffffu, bv, o);
+    int64_t i2 = __shfl_xor_sync(0xffffffffu, bi, o);
+    best_merge(bv, bi, v2, i2);
+  }
+  __shared__ double sv[8];
+  __shared__ int64_t si[8];
+  if ((threadIdx.x & 31) == 0) {
+    sv[threadIdx.x >> 5] = bv;
+    si[threadIdx.x >> 5] = bi;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) best_merge(bv, bi, sv[w], si[w]);
+    blk_best[blockIdx.x] = bv;
+    blk_idx[blockIdx.x] = bi;
+  }
+}
+
 // one thread per candidate of the chunk; block-level first-max argmax.  PEN: the value (and the gradient, when
-// pen.grad is set) is multiplied by the local penalty before the argmax.
+// pen.grad is set) is multiplied by the local penalty before the argmax.  The argmax index of candidate t is idx_map[t]
+// when idx_map is set (the compacted survivors of the screened argmax), else idx0 + t.
 template <bool PEN>
 __global__ void __launch_bounds__(256)
 tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const double* __restrict__ mean,
             int64_t Mc, int64_t idx0, double variance, int acq, double param, double aux,
             const double* __restrict__ samp, int nsamp, double* __restrict__ out_vals, double* __restrict__ out_mean, double* __restrict__ out_var,
-            double* __restrict__ blk_best, int64_t* __restrict__ blk_idx, const TailPenalty pen) {
+            double* __restrict__ blk_best, int64_t* __restrict__ blk_idx, const int64_t* __restrict__ idx_map, const TailPenalty pen) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   double bv = -INFINITY;
   int64_t bi = INT64_MAX;
@@ -529,7 +552,7 @@ tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const doub
         vb = v;
       } else {
         if (out_vals) out_vals[t] = v;
-        if (v == v) { bv = v; bi = idx0 + t; }
+        if (v == v) { bv = v; bi = idx_map ? idx_map[t] : idx0 + t; }
       }
     }
   }
@@ -583,28 +606,11 @@ tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const doub
           if (d < D) gr[d] = fma(prod, gr[d], prod == 0.0 ? 0.0 : vb * (prod * g[d]));
       }
       if (out_vals) out_vals[t] = v;
-      if (v == v) { bv = v; bi = idx0 + t; }
+      if (v == v) { bv = v; bi = idx_map ? idx_map[t] : idx0 + t; }
     }
   }
   if (blk_best == nullptr) return;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    double v2 = __shfl_xor_sync(0xffffffffu, bv, o);
-    int64_t i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-    best_merge(bv, bi, v2, i2);
-  }
-  __shared__ double sv[8];
-  __shared__ int64_t si[8];
-  if ((threadIdx.x & 31) == 0) {
-    sv[threadIdx.x >> 5] = bv;
-    si[threadIdx.x >> 5] = bi;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) best_merge(bv, bi, sv[w], si[w]);
-    blk_best[blockIdx.x] = bv;
-    blk_idx[blockIdx.x] = bi;
-  }
+  block_best_store(bv, bi, blk_best, blk_idx);
 }
 
 // fold the per-block winners of one chunk into the running best (single block)
@@ -635,6 +641,73 @@ argmax_fold_kernel(const double* __restrict__ blk_best, const int64_t* __restric
     *run_best = rv;
     *run_idx = ri;
   }
+}
+
+// ---- screened argmax of EI / log-EI (tb_api.cu, argmax_screened) ----
+// Both grow with the variance at a fixed mean, and the tail's variance fmax(variance - ss, 1e-12) (ss: a sum of squares, >= 0
+// or NaN) never exceeds var_ub = fmax(variance, 1e-12).  ub = acq_value(mean, var_ub) therefore bounds the value the tail
+// computes for the candidate, up to rounding: a candidate with ub < tau - screen_margin cannot reach tau.  The margin covers
+// the rounding of both evaluations.  EI: its absolute error is a few ulp of (eta - mean) Phi(z) + sigma phi(z) <= max(2 EI,
+// 0.7 sigma) (z^2 phi(z) <= 0.3 bounds the error carried by z), so 2^-20 |tau| + 2^-36 sigma_ub.  log-EI: the error is a few
+// ulp of max(1, z^2) ~ max(1, |value|), so 2^-20 max(1, |tau|).
+__device__ __forceinline__ double screen_threshold(int acq, double tau, double var_ub) {
+  const double m = acq == TB_ACQ_EI ? fma(0x1p-20, fabs(tau), 0x1p-36 * sqrt(var_ub)) : 0x1p-20 * fmax(1.0, fabs(tau));
+  return tau - m;  // tau = -inf: -inf (nothing is pruned); tau = +inf: NaN (nothing is pruned)
+}
+
+// ub of every candidate, per-block first-max (NaN skipped, as in the tail)
+__global__ void __launch_bounds__(256)
+screen_ub_kernel(const double* __restrict__ mean, int64_t M, double var_ub, int acq, double param, double* __restrict__ blk_best,
+                 int64_t* __restrict__ blk_idx) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  double bv = -INFINITY;
+  int64_t bi = INT64_MAX;
+  if (t < M) {
+    const double v = acq_value(acq, param, 0.0, mean[t], var_ub);
+    if (v == v) { bv = v; bi = t; }
+  }
+  block_best_store(bv, bi, blk_best, blk_idx);
+}
+
+// the screen's winner as a one-candidate set (coordinates, mean, global index); if every ub was NaN, candidate 0
+__global__ void screen_probe_kernel(const double* __restrict__ Xc, const double* __restrict__ mean, int D,
+                                    const int64_t* __restrict__ probe, double* __restrict__ xsel, double* __restrict__ msel,
+                                    int64_t* __restrict__ isel) {
+  int64_t p = *probe;
+  if (p == INT64_MAX) p = 0;
+  for (int d = threadIdx.x; d < D; d += blockDim.x) xsel[d] = Xc[p * D + d];
+  if (threadIdx.x == 0) {
+    msel[0] = mean[p];
+    isel[0] = p;
+  }
+}
+
+// the survivors (ub >= threshold, or ub NaN) written densely: coordinates, mean, global index; *count counts them all, the
+// first cap are stored.  Their order depends on the scheduling; the first-max fold over global indices does not.
+__global__ void __launch_bounds__(256)
+screen_compact_kernel(const double* __restrict__ Xc, const double* __restrict__ mean, int64_t M, int D, double var_ub, int acq,
+                      double param, const double* __restrict__ run_best, int64_t cap, unsigned long long* __restrict__ count,
+                      double* __restrict__ xsel, double* __restrict__ msel, int64_t* __restrict__ isel) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const double thr = screen_threshold(acq, *run_best, var_ub);
+  bool keep = false;
+  double mu = 0.0;
+  if (t < M) {
+    mu = mean[t];
+    keep = !(acq_value(acq, param, 0.0, mu, var_ub) < thr);
+  }
+  const unsigned ball = __ballot_sync(0xffffffffu, keep);
+  if (ball == 0u) return;
+  const int lane = threadIdx.x & 31;
+  unsigned long long base = 0;
+  if (lane == 0) base = atomicAdd(count, (unsigned long long)__popc(ball));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (!keep) return;
+  const int64_t pos = (int64_t)(base + (unsigned long long)__popc(ball & ((1u << lane) - 1u)));
+  if (pos >= cap) return;
+  for (int d = 0; d < D; ++d) xsel[pos * D + d] = Xc[t * D + d];
+  msel[pos] = mu;
+  isel[pos] = t;
 }
 
 }  // namespace tb

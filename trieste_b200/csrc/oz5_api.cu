@@ -170,9 +170,12 @@ static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int6
     TB_TRY(gp->sMeanPart.reserve(sizeof(double) * (size_t)ksplit * mstride));
     mean_dst = gp->sMeanPart.as<double>();
   }
-#define TB_KD(KIND, DPV)                                                                                                            \
-  oz5::kstar_digits_kernel<KIND, DPV, S><<<dim3(ctas, ksplit), TH, 0, st>>>(Xs, X2, al, Xc_dev, il, N, nst, D, mc, var, inv_b, dig_c, mc0, \
-                                                                            fm::Consts(), tiles, kc_per, BS, mean_dst)
+#define TB_KD_S(KIND, DPV, STORE)                                                                                                    \
+  oz5::kstar_digits_kernel<KIND, DPV, S, STORE><<<dim3(ctas, ksplit), TH, 0, st>>>(Xs, X2, al, Xc_dev, il, N, nst, D, mc, var, inv_b, \
+                                                                                   dig_c, mc0, fm::Consts(), tiles, kc_per, BS, mean_dst)
+#define TB_KD(KIND, DPV)          \
+  if (BS) TB_KD_S(KIND, DPV, true); \
+  else TB_KD_S(KIND, DPV, false)
 #define TB_KD_DP(KIND)                 \
   switch (gp->DP) {                    \
     case 2: TB_KD(KIND, 2); break;     \
@@ -194,6 +197,7 @@ static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int6
   }
 #undef TB_KD_DP
 #undef TB_KD
+#undef TB_KD_S
   TB_LAUNCHED();
   if (ksplit > 1) {
     oz5::mean_reduce_kernel<<<(unsigned)((mstride + 255) / 256), 256, 0, st>>>(mean_dst, ksplit, mstride, mc0, mean);
@@ -203,6 +207,7 @@ static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int6
   return 0;
 }
 
+// BS == nullptr: the posterior mean alone (no digit is stored), bit-identical to the mean of the full launch
 int oz5_launch_kstar(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean) {
   return gp->oz5_planes == 5 ? launch_kstar_s<5>(gp, st, Xc_dev, mc, tiles, BS, mean) : launch_kstar_s<4>(gp, st, Xc_dev, mc, tiles, BS, mean);
 }

@@ -293,7 +293,7 @@ int tb_gp_destroy(tb_gp* gp) {
                         &gp->sA, &gp->sV, &gp->sGrad, &gp->sMisc, &gp->dMes, &gp->dXspare, &gp->dyspare, &gp->dLspare, &gp->dLinvSpare,
                         &gp->dAS5, &gp->dRowScale5, &gp->dRowSum5, &gp->dX2, &gp->dKinvS5, &gp->dKinvScale5, &gp->dKinvSum5,
                         &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->sXc2, &gp->dGibPs, &gp->dGibLinv, &gp->dGibWhat,
-                        &gp->sGib})
+                        &gp->sGib, &gp->sScrMean, &gp->sScrX, &gp->sScrMu, &gp->sScrIdx, &gp->sScrBlk})
     b->release();
   for (auto& ev : gp->prof_events) {
     cudaEventDestroy(ev.first);
@@ -863,7 +863,7 @@ static int launch_partials(tb_gp* gp, cudaStream_t st, int acq, double param, co
 // (launch_partials) and its |u|^2 gradient part is added to gd here.
 static int launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const double* partial, int G, int64_t McPad,
                        const double* mean, int64_t mc, int64_t c0, double* d_vals, double* d_mean, double* d_var,
-                       const double* xc, double* gd) {
+                       const double* xc, double* gd, const int64_t* idx_map = nullptr) {
   const int blocks = (int)((mc + 255) / 256);
   double* bb = rq.want_argmax ? gp->sBlkBest.as<double>() : nullptr;
   int64_t* bi = rq.want_argmax ? gp->sBlkIdx.as<int64_t>() : nullptr;
@@ -886,10 +886,10 @@ static int launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const 
     pen.D = gp->D;
     pen.kind = gp->penKind;
     tail_kernel<true><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, gp->noise,
-                                              gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, pen);
+                                              gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, idx_map, pen);
   } else {
     tail_kernel<false><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, gp->noise,
-                                               gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, pen);
+                                               gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, idx_map, pen);
   }
   TB_LAUNCHED();
   return 0;
@@ -1017,6 +1017,7 @@ static int gradient_chunk_oz(tb_gp* gp, int acq, double param, const double* xc,
   return 0;
 }
 
+// BS == nullptr: the posterior mean alone (no digit is stored), bit-identical to the mean of the full launch
 static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean) {
   const double* Xs = gp->dXs.as<double>();
   const double* al = gp->dAlpha.as<double>();
@@ -1025,8 +1026,11 @@ static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int 
   const double var = gp->variance, mc0 = gp->mean_const;
   const double inv_b = std::ldexp(1.0, 48 - gp->oz_bscale_exp);
   cudaStream_t st = gp->stream;
-#define TB_KD(KIND, DPV) \
-  oz::kstar_digits_kernel<KIND, DPV><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nst, D, mc, var, inv_b, mc0, BS, mean)
+#define TB_KD_S(KIND, DPV, STORE) \
+  oz::kstar_digits_kernel<KIND, DPV, STORE><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nst, D, mc, var, inv_b, mc0, BS, mean)
+#define TB_KD(KIND, DPV)          \
+  if (BS) TB_KD_S(KIND, DPV, true); \
+  else TB_KD_S(KIND, DPV, false)
 #define TB_KD_DP(KIND)                                   \
   switch (gp->DP) {                                      \
     case 2: TB_KD(KIND, 2); break;                       \
@@ -1048,8 +1052,136 @@ static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int 
   }
 #undef TB_KD_DP
 #undef TB_KD
+#undef TB_KD_S
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Does this argmax call take the screened path (argmax_screened)?  EI / log-EI, unpenalised, nothing but the winner out, and
+// device candidates (the survivors are gathered from them).  TB_ARGMAX_SCREEN=0: never; =1: always (small M too);
+// unset: from SCREEN_MIN_M candidates (a conservative bound, not tuned: below it a call takes a few ms at most, and the
+// screen's extra launches and host round trip are a larger share of it).
+constexpr int64_t SCREEN_MIN_M = 16384;
+static bool argmax_screen_wanted(const EvalRequest& rq, bool xc_dev) {
+  if (!rq.want_argmax || rq.out_vals || rq.out_mean || rq.out_var || rq.out_grad || rq.pen || !xc_dev) return false;
+  if (rq.acq != TB_ACQ_EI && rq.acq != TB_ACQ_LOG_EI) return false;
+  if (const char* e = std::getenv("TB_ARGMAX_SCREEN"))
+    if (*e) return std::atoi(e) != 0;
+  return rq.M >= SCREEN_MIN_M;
+}
+
+// Exact value of n <= chunk_cap gathered candidates (coordinates xs [n][D], means ms [n] from the screening pass, global
+// indices is [n]) folded into the running best gp->sRun: K* digits from the coordinates (the mean this launch writes is not
+// used), the digit GEMM with the row-block groups G of the unscreened call, the tail and the fold.  A candidate's digits,
+// its sum of squares over G groups and its mean are what the unscreened call computes for it, so its value is too.
+static int argmax_eval_gathered(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, int G, const double* xs, const double* ms,
+                                const int64_t* is, int64_t n) {
+  cudaStream_t st = gp->stream;
+  const int tiles = (int)((n + nt - 1) / nt);
+  const int64_t McPad = (int64_t)tiles * nt;
+  int8_t* ks = gp->sKs.as<int8_t>();
+  double* partial = gp->sPartial.as<double>();
+  if (fast)
+    TB_TRY(oz5_launch_kstar(gp, st, xs, n, tiles, ks, gp->sMean.as<double>()));
+  else
+    TB_TRY(launch_kstar_digits(gp, xs, n, tiles, ks, gp->sMean.as<double>()));
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (gp->profile) {
+    TB_CUDA(cudaEventCreate(&e0));
+    TB_CUDA(cudaEventCreate(&e1));
+    TB_CUDA(cudaEventRecord(e0, st));
+  }
+  if (fast) {
+    TB_TRY(oz5_launch_gemm(gp, st, ks, tiles, G, McPad, partial));
+  } else {
+    TB_TRY(oz::launch_trigemm<oz::OZ_SUMSQ>(st, tiles, gp->dAS.as<int8_t>(), ks, gp->dRowScale.as<double>(), gp->NB, gp->nst, G, McPad,
+                                            gp->oz_out_scale, oz_npass(gp), 0, partial, nullptr, 0));
+    TB_LAUNCHED();
+  }
+  if (gp->profile) {
+    TB_CUDA(cudaEventRecord(e1, st));
+    gp->prof_events.emplace_back(e0, e1);
+    gp->prof_event_flops.push_back((double)McPad * (double)gp->N * (double)gp->N);
+  }
+  TB_CUDA(cudaGetLastError());
+  TB_TRY(launch_tail(gp, st, rq, partial, G, McPad, ms, n, 0, nullptr, nullptr, nullptr, xs, nullptr, is));
+  argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), (int)((n + 255) / 256),
+                                        gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
+  TB_LAUNCHED();
+  return 0;
+}
+
+// Screened argmax of EI / log-EI (argmax_screen_wanted): the variance GEMM runs only for candidates that can still win.
+//   1. mean pass: the K* generation of the unscreened chunking (chunk_cap, tiles, k-split) with the digit stores compiled
+//      out -> the means of all M candidates, bit-identical to the unscreened call's
+//   2. screen: ub = acq(mean, fmax(variance, 1e-12)) bounds the value from above (screen_threshold); its first-max is the probe
+//   3. the probe's exact value tau -> gp->sRun
+//   4. compaction of the survivors (ub >= tau - margin, or ub NaN); the host reads their count (one synchronisation)
+//   5. exact values of the survivors (argmax_eval_gathered), folded on their global indices into gp->sRun
+// More than M / 4 survivors: *done stays false, gp->sRun is reset and the caller runs the unscreened chunk loop.
+static int argmax_screened(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, int64_t chunk_cap, int G, bool* done) {
+  *done = false;
+  cudaStream_t st = gp->stream;
+  const int D = gp->D;
+  const int64_t M = rq.M;
+  const int64_t cap = std::max<int64_t>(1, M / 4);
+  const int sblocks = (int)((M + 255) / 256);
+  TB_TRY(gp->sScrMean.reserve(sizeof(double) * (size_t)(((M + nt - 1) / nt) * nt)));  // the last chunk writes its padding too
+  TB_TRY(gp->sScrX.reserve(sizeof(double) * (size_t)cap * D));
+  TB_TRY(gp->sScrMu.reserve(sizeof(double) * (size_t)cap));
+  TB_TRY(gp->sScrIdx.reserve(sizeof(int64_t) * (size_t)cap));
+  TB_TRY(gp->sScrBlk.reserve(16 * (size_t)sblocks + 24));
+  double* mu = gp->sScrMean.as<double>();
+  double* xsel = gp->sScrX.as<double>();
+  double* msel = gp->sScrMu.as<double>();
+  int64_t* isel = gp->sScrIdx.as<int64_t>();
+  double* bb = gp->sScrBlk.as<double>();
+  int64_t* bi = reinterpret_cast<int64_t*>(bb + sblocks);
+  double* probe_v = reinterpret_cast<double*>(bi + sblocks);
+  int64_t* probe_i = reinterpret_cast<int64_t*>(probe_v + 1);
+  unsigned long long* count = reinterpret_cast<unsigned long long*>(probe_v + 2);
+  // 1. mean pass
+  for (int64_t c0 = 0; c0 < M; c0 += chunk_cap) {
+    const int64_t mc = std::min<int64_t>(chunk_cap, M - c0);
+    const int tiles = (int)((mc + nt - 1) / nt);
+    if (fast)
+      TB_TRY(oz5_launch_kstar(gp, st, rq.Xc + c0 * D, mc, tiles, nullptr, mu + c0));
+    else
+      TB_TRY(launch_kstar_digits(gp, rq.Xc + c0 * D, mc, tiles, nullptr, mu + c0));
+  }
+  // 2. screen
+  const double var_ub = std::fmax(gp->variance, 1e-12);
+  const double init_v = -INFINITY;
+  const int64_t init_i = INT64_MAX;
+  TB_CUDA(cudaMemcpyAsync(probe_v, &init_v, 8, cudaMemcpyHostToDevice, st));
+  TB_CUDA(cudaMemcpyAsync(probe_i, &init_i, 8, cudaMemcpyHostToDevice, st));
+  screen_ub_kernel<<<sblocks, 256, 0, st>>>(mu, M, var_ub, rq.acq, rq.param, bb, bi);
+  TB_LAUNCHED();
+  argmax_fold_kernel<<<1, 256, 0, st>>>(bb, bi, sblocks, probe_v, probe_i);
+  TB_LAUNCHED();
+  // 3. probe
+  screen_probe_kernel<<<1, 32, 0, st>>>(rq.Xc, mu, D, probe_i, xsel, msel, isel);
+  TB_LAUNCHED();
+  TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel, msel, isel, 1));
+  // 4. compaction
+  TB_CUDA(cudaMemsetAsync(count, 0, 8, st));
+  screen_compact_kernel<<<sblocks, 256, 0, st>>>(rq.Xc, mu, M, D, var_ub, rq.acq, rq.param, gp->sRun.as<double>(), cap, count, xsel,
+                                                 msel, isel);
+  TB_LAUNCHED();
+  unsigned long long n = 0;
+  TB_CUDA(cudaMemcpyAsync(&n, count, 8, cudaMemcpyDeviceToHost, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  TB_CUDA(cudaGetLastError());
+  if (n > (unsigned long long)cap) {
+    TB_CUDA(cudaMemcpyAsync(gp->sRun.p, &init_v, 8, cudaMemcpyHostToDevice, st));
+    TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, st));
+    return 0;
+  }
+  // 5. exact evaluation of the survivors
+  for (int64_t s0 = 0; s0 < (int64_t)n; s0 += chunk_cap)
+    TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel + s0 * D, msel + s0, isel + s0, std::min<int64_t>(chunk_cap, (int64_t)n - s0)));
+  *done = true;
   return 0;
 }
 
@@ -1129,8 +1261,12 @@ static int run_eval_oz(tb_gp* gp, EvalRequest& rq) {
     TB_TRY(gp->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
   }
 
+  bool screened = false;
+  if (argmax_screen_wanted(rq, xc_dev)) TB_TRY(argmax_screened(gp, rq, fast, nt, chunk_cap, G, &screened));
+  const int64_t m_loop = screened ? 0 : rq.M;  // the screened path has folded its survivors into gp->sRun already
+
   int64_t c = 0;
-  for (int64_t c0 = 0; c0 < rq.M; c0 += chunk_cap, ++c) {
+  for (int64_t c0 = 0; c0 < m_loop; c0 += chunk_cap, ++c) {
     const int slot = (int)(c & 1);
     const int64_t mc = std::min<int64_t>(chunk_cap, rq.M - c0);
     const int tiles = (int)((mc + nt - 1) / nt);
