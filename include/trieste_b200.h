@@ -255,6 +255,10 @@ int tb_gp_set_engine(tb_gp* gp, int engine);
  * 0 = native fp64 engine) and, for the reduced modes, the a-priori estimate of max |Δvar| / σ_f² that admitted them.
  * Needs a valid cache.  Either output may be NULL. */
 int tb_gp_engine_info(tb_gp* gp, int* digit_products, double* error_estimate);
+/* diagnostics of the screened argmax: the fp32 bound pass's interval [lo, hi] for the posterior mean of each of M candidates
+ * (Xc: [M, D] fp64; all pointers host or device).  The mean the predict path computes lies inside it; a bound that could not
+ * be trusted (non-finite or overflowing coordinates) is [NaN, NaN].  Needs a valid cache. */
+int tb_gp_mean_bounds(tb_gp* gp, const double* Xc, int64_t M, double* lo, double* hi);
 int tb_gp_profile(tb_gp* gp, int enable);
 /* the handle's CUDA stream (cudaStream_t as void*), so callers can record CUDA events on the stream the
  * kernels are launched on (torch.cuda.ExternalStream in bench.py). */

@@ -6,9 +6,11 @@
 
 For each: median time per fused_argmax call with TB_ARGMAX_SCREEN=1 and =0, the two alternated call by call in one
 process; the candidates that went through the variance GEMM (profile counters: the survivors padded to whole tiles, plus
-the probe's tile) against M; and, from one profiled screened call (torch.profiler, CUDA activities), the device time of
-the mean pass (the K* generation with the digit stores compiled out), of the screen / compaction kernels and of the rest
-(probe, survivors' K* digits, GEMM, tail, folds).  The card name and power limit are read in the same run.
+the probe's tile) against M; from one profiled screened call (torch.profiler, CUDA activities), the device time of the
+fp32 bound pass (mean_bounds_kernel), of the compaction and of the rest (probe, survivors' K* digits and means, GEMM, tail,
+folds); and the survivor count of the bound screen (acq(lo) >= tau - margin, lo from tb_gp_mean_bounds) next to the count
+the same screen gives on the exact fp64 means (predict), tau being the call's exact best value (EI only).  The card name
+and power limit are read in the same run.
 
     python tools/argmax_screen_time.py [--reps 7] [--out FILE]     (prints one JSON line)
 """
@@ -76,6 +78,26 @@ def main():
         torch.cuda.synchronize()
         return time.perf_counter() - t0, r
 
+    def survivors(m, fn, x, tau):
+        """candidates the screen keeps with the bound pass's lower mean bound, and with the exact fp64 mean (EI, as in
+        tb_api.cu: ub = EI(mean, sigma_ub) >= tau - 2^-20 |tau| - 2^-36 sigma_ub, NaN kept)"""
+        from scipy.special import ndtr
+
+        M = x.shape[0]
+        lo = torch.empty(M, dtype=torch.float64, device="cuda")
+        hi = torch.empty_like(lo)
+        _lib.check(lib.tb_gp_mean_bounds(m.handle, x.data_ptr(), M, lo.data_ptr(), hi.data_ptr()))
+        mu = np.asarray(m.predict(x.cpu().numpy())[0]).reshape(-1)
+        eta, sig = fn._param, float(np.sqrt(max(float(m._spec.kernel.variance), 1e-12)))
+        thr = tau - (2.0**-20 * abs(tau) + 2.0**-36 * sig)
+
+        def count(mean):
+            z = (eta - mean) / sig
+            ub = (eta - mean) * ndtr(z) + sig * np.exp(-0.5 * z * z) / np.sqrt(2 * np.pi)
+            return int(np.sum(~(ub < thr)))
+
+        return {"bound": count(lo.cpu().numpy()), "exact_mean": count(mu)}
+
     t = {k: {0: [], 1: []} for k in work}
     best = {k: {} for k in work}
     for k, (_, fn, x, _) in work.items():
@@ -101,24 +123,26 @@ def main():
         lib.tb_gp_profile(h, 0)
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             call(fn, x, 1)
-        mean_us = screen_us = rest_us = 0.0
+        bound_us = compact_us = rest_us = 0.0
         for e in prof.key_averages():
             us = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
             if us <= 0:
                 continue
-            if "kstar_digits_kernel" in e.key and ", false>" in e.key:
-                mean_us += us
-            elif "screen_" in e.key:
-                screen_us += us
+            if "mean_bounds_kernel" in e.key:
+                bound_us += us
+            elif "compact_kernel" in e.key:
+                compact_us += us
             else:
                 rest_us += us
+        surv = survivors(m, fn, x, best[k][1][1])
         row[k] = {
             "candidates": int(x.shape[0]),
             "screened_s": med(t[k][1]), "screened_spread": [min(t[k][1]), max(t[k][1])],
             "unscreened_s": med(t[k][0]), "unscreened_spread": [min(t[k][0]), max(t[k][0])],
             "speedup": med(t[k][0]) / med(t[k][1]),
             "gemm_candidates": fl.value / float(N) ** 2, "gemm_launches": int(n.value),
-            "device_ms": {"mean_pass": mean_us / 1e3, "screen_compact": screen_us / 1e3, "probe_survivors_rest": rest_us / 1e3},
+            "device_ms": {"bound_pass": bound_us / 1e3, "compaction": compact_us / 1e3, "probe_survivors_rest": rest_us / 1e3},
+            "survivors": surv,
             "best": list(best[k][1]),
         }
     line = json.dumps(row)

@@ -66,6 +66,7 @@ SIGNATURES = {
     "tb_launch_count_reset": (None, []),
     "tb_gp_set_engine": (_i32, [_vp, _i32]),
     "tb_gp_engine_info": (_i32, [_vp, C.POINTER(_i32), C.POINTER(_f64)]),
+    "tb_gp_mean_bounds": (_i32, [_vp, _vp, _i64, _vp, _vp]),
     "tb_gp_profile": (_i32, [_vp, _i32]),
     "tb_gp_stream": (_i32, [_vp, C.POINTER(_vp)]),
     "tb_gp_profile_read": (_i32, [_vp, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)]),

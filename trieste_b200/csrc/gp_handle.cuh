@@ -128,9 +128,14 @@ struct tb_gp {
   uint64_t gib_gen = ~(uint64_t)0;      // cache_gen the derived GIBBON state was built for
   tb::DevBuf dGibPs, dGibLinv, dGibWhat;
   tb::DevBuf sGib;                      // per chunk: |u|^2 [mc], -w / V_det [mc], u [mp][mc] (gradient path)
-  // screened argmax (tb_api.cu, argmax_screened): means of all M candidates, the survivors' coordinates / means / global
-  // indices, and the screen's per-block winners + probe pair + survivor count
-  tb::DevBuf sScrMean, sScrX, sScrMu, sScrIdx, sScrBlk;
+  // screened argmax (tb_api.cu, argmax_screened): the screen bound ub of all M candidates, the survivors' coordinates / global
+  // indices, and the bound pass's per-block winners + probe pair + survivor counts
+  tb::DevBuf sScrUb, sScrX, sScrIdx, sScrBlk;
+  // fp32 mirrors of the posterior for the bound pass (prescreen.cuh), rebuilt when cache_gen moves: rows [nst*64][W] of
+  // (x', |x'|^2, σ_f² α, |σ_f² α|), the centre [DP] subtracted from scaled inputs, and the constants of the bound
+  tb::DevBuf dPreRows, dPreCentre;
+  uint64_t pre_gen = ~(uint64_t)0;
+  double pre_scale = 1.0, pre_x2max = 0.0, pre_rel = 0.0, pre_lin = 0.0, pre_lin_max = 0.0, pre_abs = 0.0;
 
   // profiling of the dominant kernel
   bool profile = false;

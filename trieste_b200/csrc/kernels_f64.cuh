@@ -643,7 +643,7 @@ argmax_fold_kernel(const double* __restrict__ blk_best, const int64_t* __restric
   }
 }
 
-// ---- screened argmax of EI / log-EI (tb_api.cu, argmax_screened) ----
+// ---- screened argmax of EI / log-EI (tb_api.cu, argmax_screened; prescreen.cuh) ----
 // Both grow with the variance at a fixed mean, and the tail's variance fmax(variance - ss, 1e-12) (ss: a sum of squares, >= 0
 // or NaN) never exceeds var_ub = fmax(variance, 1e-12).  ub = acq_value(mean, var_ub) therefore bounds the value the tail
 // computes for the candidate, up to rounding: a candidate with ub < tau - screen_margin cannot reach tau.  The margin covers
@@ -653,61 +653,6 @@ argmax_fold_kernel(const double* __restrict__ blk_best, const int64_t* __restric
 __device__ __forceinline__ double screen_threshold(int acq, double tau, double var_ub) {
   const double m = acq == TB_ACQ_EI ? fma(0x1p-20, fabs(tau), 0x1p-36 * sqrt(var_ub)) : 0x1p-20 * fmax(1.0, fabs(tau));
   return tau - m;  // tau = -inf: -inf (nothing is pruned); tau = +inf: NaN (nothing is pruned)
-}
-
-// ub of every candidate, per-block first-max (NaN skipped, as in the tail)
-__global__ void __launch_bounds__(256)
-screen_ub_kernel(const double* __restrict__ mean, int64_t M, double var_ub, int acq, double param, double* __restrict__ blk_best,
-                 int64_t* __restrict__ blk_idx) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  double bv = -INFINITY;
-  int64_t bi = INT64_MAX;
-  if (t < M) {
-    const double v = acq_value(acq, param, 0.0, mean[t], var_ub);
-    if (v == v) { bv = v; bi = t; }
-  }
-  block_best_store(bv, bi, blk_best, blk_idx);
-}
-
-// the screen's winner as a one-candidate set (coordinates, mean, global index); if every ub was NaN, candidate 0
-__global__ void screen_probe_kernel(const double* __restrict__ Xc, const double* __restrict__ mean, int D,
-                                    const int64_t* __restrict__ probe, double* __restrict__ xsel, double* __restrict__ msel,
-                                    int64_t* __restrict__ isel) {
-  int64_t p = *probe;
-  if (p == INT64_MAX) p = 0;
-  for (int d = threadIdx.x; d < D; d += blockDim.x) xsel[d] = Xc[p * D + d];
-  if (threadIdx.x == 0) {
-    msel[0] = mean[p];
-    isel[0] = p;
-  }
-}
-
-// the survivors (ub >= threshold, or ub NaN) written densely: coordinates, mean, global index; *count counts them all, the
-// first cap are stored.  Their order depends on the scheduling; the first-max fold over global indices does not.
-__global__ void __launch_bounds__(256)
-screen_compact_kernel(const double* __restrict__ Xc, const double* __restrict__ mean, int64_t M, int D, double var_ub, int acq,
-                      double param, const double* __restrict__ run_best, int64_t cap, unsigned long long* __restrict__ count,
-                      double* __restrict__ xsel, double* __restrict__ msel, int64_t* __restrict__ isel) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const double thr = screen_threshold(acq, *run_best, var_ub);
-  bool keep = false;
-  double mu = 0.0;
-  if (t < M) {
-    mu = mean[t];
-    keep = !(acq_value(acq, param, 0.0, mu, var_ub) < thr);
-  }
-  const unsigned ball = __ballot_sync(0xffffffffu, keep);
-  if (ball == 0u) return;
-  const int lane = threadIdx.x & 31;
-  unsigned long long base = 0;
-  if (lane == 0) base = atomicAdd(count, (unsigned long long)__popc(ball));
-  base = __shfl_sync(0xffffffffu, base, 0);
-  if (!keep) return;
-  const int64_t pos = (int64_t)(base + (unsigned long long)__popc(ball & ((1u << lane) - 1u)));
-  if (pos >= cap) return;
-  for (int d = 0; d < D; ++d) xsel[pos * D + d] = Xc[t * D + d];
-  msel[pos] = mu;
-  isel[pos] = t;
 }
 
 }  // namespace tb

@@ -145,7 +145,28 @@ template <int S>
 static double oz5_h_eff(double variance) { return 0.5 * variance * oz5_centre_int<S>() / (oz5::FILL * oz5::two_pow_8S<S>()); }
 
 template <int S>
-static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean) {
+static unsigned kstar_ctas(int tiles) {
+  return (unsigned)(((int64_t)tiles * (oz5::Geo<S>::NT / 8) + oz5::KGEN_WARPS - 1) / oz5::KGEN_WARPS);
+}
+
+KSplit oz5_kstar_split(const tb_gp* gp, int tiles) {
+  const int nst = gp->nst;
+  const unsigned ctas = gp->oz5_planes == 5 ? kstar_ctas<5>(tiles) : kstar_ctas<4>(tiles);
+  // few tiles (the late rounds of the multi-start optimiser, small predict calls): split the training rows over blockIdx.y so
+  // that ~4 CTAs per SM exist; each split covers >= 2 stages
+  KSplit s;
+  s.kc_per = nst;
+  if (ctas < NUM_SMS && nst >= 4) {
+    s.ksplit = std::min<int>(nst / 2, (int)((4 * NUM_SMS + ctas - 1) / ctas));
+    s.kc_per = (nst + s.ksplit - 1) / s.ksplit;
+    s.ksplit = (nst + s.kc_per - 1) / s.kc_per;
+  }
+  return s;
+}
+
+template <int S>
+static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean,
+                          const KSplit* split) {
   const double* Xs = gp->dXs.as<double>();
   const double* al = gp->dAlpha.as<double>();
   const double* il = gp->dInvLs.as<double>();
@@ -155,27 +176,18 @@ static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int6
   const double dig_c = fm::MAGIC + oz5::dig_koff<S>() - oz5_centre_int<S>();
   const double* X2 = gp->dX2.as<double>();
   constexpr int TH = oz5::KGEN_WARPS * 32;
-  const unsigned ctas = (unsigned)(((int64_t)tiles * (oz5::Geo<S>::NT / 8) + oz5::KGEN_WARPS - 1) / oz5::KGEN_WARPS);
-  // few tiles (the late rounds of the multi-start optimiser, small predict calls): split the training rows over blockIdx.y so
-  // that ~4 CTAs per SM exist; each split covers >= 2 stages
-  int ksplit = 1, kc_per = nst;
-  if (ctas < NUM_SMS && nst >= 4) {
-    ksplit = std::min<int>(nst / 2, (int)((4 * NUM_SMS + ctas - 1) / ctas));
-    kc_per = (nst + ksplit - 1) / ksplit;
-    ksplit = (nst + kc_per - 1) / kc_per;
-  }
+  const unsigned ctas = kstar_ctas<S>(tiles);
+  const KSplit ks = split ? *split : oz5_kstar_split(gp, tiles);
+  const int ksplit = ks.ksplit, kc_per = ks.kc_per;
   const int64_t mstride = (int64_t)tiles * oz5::Geo<S>::NT;
   double* mean_dst = mean;
   if (ksplit > 1) {
     TB_TRY(gp->sMeanPart.reserve(sizeof(double) * (size_t)ksplit * mstride));
     mean_dst = gp->sMeanPart.as<double>();
   }
-#define TB_KD_S(KIND, DPV, STORE)                                                                                                    \
-  oz5::kstar_digits_kernel<KIND, DPV, S, STORE><<<dim3(ctas, ksplit), TH, 0, st>>>(Xs, X2, al, Xc_dev, il, N, nst, D, mc, var, inv_b, \
-                                                                                   dig_c, mc0, fm::Consts(), tiles, kc_per, BS, mean_dst)
-#define TB_KD(KIND, DPV)          \
-  if (BS) TB_KD_S(KIND, DPV, true); \
-  else TB_KD_S(KIND, DPV, false)
+#define TB_KD(KIND, DPV)                                                                                                      \
+  oz5::kstar_digits_kernel<KIND, DPV, S><<<dim3(ctas, ksplit), TH, 0, st>>>(Xs, X2, al, Xc_dev, il, N, nst, D, mc, var, inv_b, \
+                                                                            dig_c, mc0, fm::Consts(), tiles, kc_per, BS, mean_dst)
 #define TB_KD_DP(KIND)                 \
   switch (gp->DP) {                    \
     case 2: TB_KD(KIND, 2); break;     \
@@ -197,7 +209,6 @@ static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int6
   }
 #undef TB_KD_DP
 #undef TB_KD
-#undef TB_KD_S
   TB_LAUNCHED();
   if (ksplit > 1) {
     oz5::mean_reduce_kernel<<<(unsigned)((mstride + 255) / 256), 256, 0, st>>>(mean_dst, ksplit, mstride, mc0, mean);
@@ -207,9 +218,10 @@ static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int6
   return 0;
 }
 
-// BS == nullptr: the posterior mean alone (no digit is stored), bit-identical to the mean of the full launch
-int oz5_launch_kstar(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean) {
-  return gp->oz5_planes == 5 ? launch_kstar_s<5>(gp, st, Xc_dev, mc, tiles, BS, mean) : launch_kstar_s<4>(gp, st, Xc_dev, mc, tiles, BS, mean);
+int oz5_launch_kstar(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean,
+                     const KSplit* split) {
+  return gp->oz5_planes == 5 ? launch_kstar_s<5>(gp, st, Xc_dev, mc, tiles, BS, mean, split)
+                             : launch_kstar_s<4>(gp, st, Xc_dev, mc, tiles, BS, mean, split);
 }
 
 // The K* digits are cut against sB = h / FILL with 2^(8 planes) steps; a GEMM that computes with S < planes leading digits sees

@@ -162,9 +162,9 @@ __global__ void sym_digits_kernel(const double* __restrict__ A, int64_t N, int n
 // ------------------------------------------------------------------------------------------------
 // K* digit tiles + posterior mean.  grid = candidate tiles x (512 / blockDim); warp w (0..15 within a tile) owns candidates
 // [8w, 8w+8); lane l <-> (candidate l % 8, 16-wide k chunk l / 8): every digit store of a warp is 512
-// contiguous bytes (four adjacent core matrices).  STORE = false: the mean alone (the argmax screening pass), bit-identical.
+// contiguous bytes (four adjacent core matrices).  A candidate's mean does not depend on the other candidates of the launch.
 // ------------------------------------------------------------------------------------------------
-template <int KIND, int DP, bool STORE = true>
+template <int KIND, int DP>
 __global__ void __launch_bounds__(512, 2)
 kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ alpha, const double* __restrict__ Xc,
                     const double* __restrict__ inv_ls, int N, int nst, int D, int64_t M, double variance,
@@ -225,11 +225,9 @@ kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ al
       digit_bytes6(__double2ll_rn(kval * inv_bscale_2p48), wl, wh);
       scatter_digits_rt(pk, j, wl, wh);
     }
-    if (STORE) {
 #pragma unroll
-      for (int p = 0; p < S; ++p)
-        *reinterpret_cast<uint4*>(tile + (int64_t)kc * (S * TILE) + p * TILE) = make_uint4(pk[p][0], pk[p][1], pk[p][2], pk[p][3]);
-    }
+    for (int p = 0; p < S; ++p)
+      *reinterpret_cast<uint4*>(tile + (int64_t)kc * (S * TILE) + p * TILE) = make_uint4(pk[p][0], pk[p][1], pk[p][2], pk[p][3]);
     __syncthreads();  // everyone is done with xs_s[buf] before the next iteration's prefetch overwrites it
   }
   macc += __shfl_xor_sync(0xffffffffu, macc, 8);

@@ -211,11 +211,11 @@ __global__ void sym_digits_kernel(const double* __restrict__ A, int64_t N, int n
 // [8 (wg % (NT/8)), +8) of candidate tile wg / (NT/8); lane l <-> (candidate l % 8, 16-wide k chunk l / 8): every digit
 // store of a warp is 512 contiguous bytes.  The training rows of a stage are staged per CTA (they do not depend on the tile).
 //   inv_bscale_2p = 2^(8S) / sB,  sB = h / FILL,  h = variance / 2
-// STORE = false: the mean alone (the screening pass of the argmax, tb_api.cu): same grid, k-split and summation order, so the
-// means are bit-identical, and no digit reaches memory.
+// A candidate's mean depends on (ksplit = gridDim.y, kc_per) only: the screened argmax (tb_api.cu) reproduces the mean of a
+// candidate of an unscreened chunk by launching with that chunk's split.
 // ------------------------------------------------------------------------------------------------
 constexpr int KGEN_WARPS = 8;
-template <int KIND, int DP, int S, bool STORE = true>
+template <int KIND, int DP, int S>
 __global__ void __launch_bounds__(KGEN_WARPS * 32, DP <= 12 ? 4 : 3)  // 64 registers / 32 warps per SM (80 / 24 for D > 12: no spills)
 kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2, const double* __restrict__ alpha,
                     const double* __restrict__ Xc, const double* __restrict__ inv_ls, int N, int nst, int D, int64_t M, double variance,
@@ -324,7 +324,7 @@ kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2
       const uint32_t wl = (uint32_t)__double2loint(tb) ^ 0x80808080u, wh = (uint32_t)__double2hiint(tb) ^ 0x80u;
       scatter_rt<S>(pk, j, wl, wh);
     }
-    if (STORE && tile_id < ntiles) {
+    if (tile_id < ntiles) {
 #pragma unroll
       for (int p = 0; p < S; ++p)
         *reinterpret_cast<uint4*>(tile + (int64_t)kc * (S * BTILE) + p * BTILE) = make_uint4(pk[p][0], pk[p][1], pk[p][2], pk[p][3]);

@@ -2,6 +2,7 @@
 // runs in the kernels of kernels_f64.cuh / kernels_extra.cuh.
 #include "gp_handle.cuh"
 #include "kernels_extra.cuh"
+#include "prescreen.cuh"
 #include "batch_ei.cuh"
 #include "ozaki.cuh"
 #include "oz5_api.h"
@@ -293,7 +294,7 @@ int tb_gp_destroy(tb_gp* gp) {
                         &gp->sA, &gp->sV, &gp->sGrad, &gp->sMisc, &gp->dMes, &gp->dXspare, &gp->dyspare, &gp->dLspare, &gp->dLinvSpare,
                         &gp->dAS5, &gp->dRowScale5, &gp->dRowSum5, &gp->dX2, &gp->dKinvS5, &gp->dKinvScale5, &gp->dKinvSum5,
                         &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->sXc2, &gp->dGibPs, &gp->dGibLinv, &gp->dGibWhat,
-                        &gp->sGib, &gp->sScrMean, &gp->sScrX, &gp->sScrMu, &gp->sScrIdx, &gp->sScrBlk})
+                        &gp->sGib, &gp->sScrUb, &gp->sScrX, &gp->sScrIdx, &gp->sScrBlk, &gp->dPreRows, &gp->dPreCentre})
     b->release();
   for (auto& ev : gp->prof_events) {
     cudaEventDestroy(ev.first);
@@ -1017,7 +1018,6 @@ static int gradient_chunk_oz(tb_gp* gp, int acq, double param, const double* xc,
   return 0;
 }
 
-// BS == nullptr: the posterior mean alone (no digit is stored), bit-identical to the mean of the full launch
 static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean) {
   const double* Xs = gp->dXs.as<double>();
   const double* al = gp->dAlpha.as<double>();
@@ -1026,12 +1026,9 @@ static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int 
   const double var = gp->variance, mc0 = gp->mean_const;
   const double inv_b = std::ldexp(1.0, 48 - gp->oz_bscale_exp);
   cudaStream_t st = gp->stream;
-#define TB_KD_S(KIND, DPV, STORE) \
-  oz::kstar_digits_kernel<KIND, DPV, STORE><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nst, D, mc, var, inv_b, mc0, BS, mean)
-#define TB_KD(KIND, DPV)          \
-  if (BS) TB_KD_S(KIND, DPV, true); \
-  else TB_KD_S(KIND, DPV, false)
-#define TB_KD_DP(KIND)                                   \
+#define TB_KD(KIND, DPV) \
+  oz::kstar_digits_kernel<KIND, DPV><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nst, D, mc, var, inv_b, mc0, BS, mean)
+#define TB_KD_DP(KIND)                                 \
   switch (gp->DP) {                                      \
     case 2: TB_KD(KIND, 2); break;                       \
     case 4: TB_KD(KIND, 4); break;                       \
@@ -1052,7 +1049,6 @@ static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int 
   }
 #undef TB_KD_DP
 #undef TB_KD
-#undef TB_KD_S
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;
@@ -1071,21 +1067,175 @@ static bool argmax_screen_wanted(const EvalRequest& rq, bool xc_dev) {
   return rq.M >= SCREEN_MIN_M;
 }
 
-// Exact value of n <= chunk_cap gathered candidates (coordinates xs [n][D], means ms [n] from the screening pass, global
-// indices is [n]) folded into the running best gp->sRun: K* digits from the coordinates (the mean this launch writes is not
-// used), the digit GEMM with the row-block groups G of the unscreened call, the tail and the fold.  A candidate's digits,
-// its sum of squares over G groups and its mean are what the unscreened call computes for it, so its value is too.
-static int argmax_eval_gathered(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, int G, const double* xs, const double* ms,
-                                const int64_t* is, int64_t n) {
+// fp32 mirrors of the posterior for the bound pass (prescreen.cuh) and the constants of its error bound (DESIGN.md §4d),
+// rebuilt on the host whenever the posterior cache moves (cache_gen: refits and appends).  x' = (x / l - centre) * pre: the
+// centre is the midpoint of the training rows' bounding box (a shift leaves distances alone and shrinks the norms the
+// expansion form cancels), pre folds the kernel's distance scale and log2(e) into the coordinates.
+static int prescreen_ensure(tb_gp* gp) {
+  if (gp->pre_gen == gp->cache_gen) return 0;
+  const int64_t N = gp->N;
+  const int D = gp->D, DP = gp->DP;
+  const int W = ((DP + 3 + 3) / 4) * 4;
+  const int64_t rows = ((N + pre::KS - 1) / pre::KS) * pre::KS;
+  cudaStream_t st = gp->stream;
+  std::vector<double> xs((size_t)N * DP), al((size_t)N);
+  TB_CUDA(cudaMemcpyAsync(xs.data(), gp->dXs.p, sizeof(double) * N * DP, cudaMemcpyDeviceToHost, st));
+  TB_CUDA(cudaMemcpyAsync(al.data(), gp->dAlpha.p, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  const double LOG2E = 1.4426950408889634, LN2 = 0.6931471805599453;
+  double pre2, cq;  // pre^2, and |d ln k / dq| in pre-scaled units (expansion-form kernels)
+  switch (gp->kernel) {
+    case TB_RBF: pre2 = 0.5 * LOG2E, cq = LN2; break;
+    case TB_MATERN12: pre2 = LOG2E * LOG2E, cq = 0.0; break;
+    case TB_MATERN32: pre2 = 3.0 * LOG2E * LOG2E, cq = 0.5 * LN2 * LN2; break;
+    default: pre2 = 5.0 * LOG2E * LOG2E, cq = LN2 * LN2 / 6.0; break;
+  }
+  const double pre = std::sqrt(pre2);
+  std::vector<double> centre((size_t)DP, 0.0);
+  double unc2 = 0.0;  // max_j |x_j / l|^2, uncentred (the fp64 path's own cancellation)
+  for (int d = 0; d < D; ++d) {
+    double lo = INFINITY, hi = -INFINITY;
+    for (int64_t j = 0; j < N; ++j) lo = std::min(lo, xs[j * DP + d]), hi = std::max(hi, xs[j * DP + d]);
+    centre[d] = 0.5 * (lo + hi);
+  }
+  std::vector<float> h((size_t)rows * W, 0.0f);
+  double x2max = 0.0, asum = 0.0, c2 = 0.0;
+  for (int d = 0; d < D; ++d) c2 += centre[d] * centre[d];
+  for (int64_t j = 0; j < N; ++j) {
+    float* r = &h[(size_t)j * W];
+    double n2 = 0.0, u2 = 0.0;
+    for (int d = 0; d < D; ++d) {
+      r[d] = (float)((xs[j * DP + d] - centre[d]) * pre);
+      n2 += (double)r[d] * (double)r[d];
+      u2 += xs[j * DP + d] * xs[j * DP + d];
+    }
+    r[DP] = (float)n2;
+    const float a = (float)(gp->variance * al[j]);
+    r[DP + 1] = a;
+    r[DP + 2] = std::fabs(a);
+    x2max = std::max(x2max, (double)r[DP]);
+    unc2 = std::max(unc2, u2);
+    asum += std::fabs((double)a);
+  }
+  // the bound (DESIGN.md §4d): E = safety ((rel + lin * norms) S + abs)
+  const double u = std::ldexp(1.0, -24), mufu = std::ldexp(1.0, -21);
+  const bool expand = gp->kernel != TB_MATERN12;
+  // s-proportional part (Matern): the error of sqrt(q) = q rsqrt(q) (and, for Matern12, of the difference form's q) is
+  // relative, kappa s on the exp argument; split at s0: kappa (s0 S + T(s0) sum |a|), T(s0) = sup_{s >= s0} s k(s) / σ_f²
+  double kappa = 0.0, s0 = 0.0, tail = 0.0;
+  if (gp->kernel != TB_RBF) {
+    kappa = 1.01 * (mufu + u + (expand ? 0.0 : (2 * DP + 2) * u / 2));
+    auto T = [&](double s) {
+      const double p = gp->kernel == TB_MATERN12 ? 1.0 : gp->kernel == TB_MATERN32 ? 1.0 + s : 1.0 + s + s * s / 3.0;
+      return s * p * std::exp(-s);  // decreasing for s >= 4 in all three
+    };
+    double best = INFINITY;
+    for (double s = 4.0; s <= 48.0; s += 1.0) {
+      const double cost = s * 0.01 * asum + T(s) * asum;  // against a typical S of 1 % of sum |a|
+      if (cost < best) best = cost, s0 = s;
+    }
+    tail = T(s0);
+  }
+  double rel = mufu + 4 * u                                 // ex2, polynomial, product, rounding of a
+               + 32 * u / (1 - 32 * u)                      // fp32 partial sums of KH = 32 terms
+               + kappa * s0                                 // s-proportional part up to s0
+               + (double)(N + 64) * std::ldexp(1.0, -52)    // the fp64 path's own kernel values and sum, the fp64 folds
+               + 1e-15;                                     // the clamp q >= 1e-30
+  double lin;
+  if (expand) {
+    lin = cq * (2 * DP + 10) * u;  // expansion-form cancellation and input rounding: |dq| <= (2 DP + 10) u (|x'|^2 + max|X'|^2)
+    const double l64 = cq * (2 * DP + 10) * std::ldexp(1.0, -52);  // the fp64 path's expansion form on uncentred inputs
+    lin += l64;
+    rel += l64 * pre2 * (c2 + unc2);
+  } else {
+    lin = LN2 * u;  // Matern12: |dr'| <= u (|x'| + max|X'|) from the input rounding
+  }
+  gp->pre_rel = 1.01 * rel;
+  gp->pre_lin = 1.01 * lin;
+  gp->pre_lin_max = std::ldexp(1.0, -10);
+  gp->pre_abs = 1.01 * (asum * (2700.0 * std::ldexp(1.0, -126) + kappa * tail) + 2.0 * (double)rows * std::ldexp(1.0, -149));
+  gp->pre_scale = pre;
+  gp->pre_x2max = 1.01 * x2max;
+  TB_TRY(gp->dPreRows.reserve(sizeof(float) * h.size()));
+  TB_TRY(gp->dPreCentre.reserve(sizeof(double) * DP));
+  TB_CUDA(cudaMemcpyAsync(gp->dPreRows.p, h.data(), sizeof(float) * h.size(), cudaMemcpyHostToDevice, st));
+  TB_CUDA(cudaMemcpyAsync(gp->dPreCentre.p, centre.data(), sizeof(double) * DP, cudaMemcpyHostToDevice, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  gp->pre_gen = gp->cache_gen;
+  return 0;
+}
+
+static int prescreen_cpt(int DP) { return DP <= 12 ? 4 : DP <= 20 ? 2 : 1; }
+static int prescreen_blocks(const tb_gp* gp, int64_t M) {
+  const int64_t per = (int64_t)pre::TH * prescreen_cpt(gp->DP);
+  return (int)((M + per - 1) / per);
+}
+
+// the bound pass over M device candidates: acq >= 0: out0 = ub, per-CTA first-max of acq(μ̃) into blk_best / blk_idx;
+// acq < 0: out0 / out1 = μ̃ -/+ E
+static int launch_mean_bounds(tb_gp* gp, cudaStream_t st, const double* Xc, int64_t M, int acq, double param, double var_ub,
+                              double* out0, double* out1, double* blk_best, int64_t* blk_idx) {
+  TB_TRY(prescreen_ensure(gp));
+  pre::Bound b;
+  b.rel = gp->pre_rel;
+  b.lin = gp->pre_lin;
+  b.lin_max = gp->pre_lin_max;
+  b.abs = gp->pre_abs;
+  b.safety = 4.0;
+  b.x2max = gp->pre_x2max;
+  b.mean_const = gp->mean_const;
+  b.pre = gp->pre_scale;
+  const float* rows = gp->dPreRows.as<float>();
+  const int nst = (int)((gp->N + pre::KS - 1) / pre::KS), D = gp->D;
+  const double* il = gp->dInvLs.as<double>();
+  const double* cen = gp->dPreCentre.as<double>();
+  const unsigned blocks = (unsigned)prescreen_blocks(gp, M);
+#define TB_MB(KIND, DPV)                                                                                                         \
+  pre::mean_bounds_kernel<KIND, DPV><<<blocks, pre::TH, 0, st>>>(rows, nst, Xc, il, cen, D, M, b, acq, param, var_ub, out0, out1, \
+                                                                 blk_best, blk_idx)
+#define TB_MB_DP(KIND)               \
+  switch (gp->DP) {                  \
+    case 2: TB_MB(KIND, 2); break;   \
+    case 4: TB_MB(KIND, 4); break;   \
+    case 6: TB_MB(KIND, 6); break;   \
+    case 8: TB_MB(KIND, 8); break;   \
+    case 10: TB_MB(KIND, 10); break; \
+    case 12: TB_MB(KIND, 12); break; \
+    case 16: TB_MB(KIND, 16); break; \
+    case 20: TB_MB(KIND, 20); break; \
+    case 24: TB_MB(KIND, 24); break; \
+    default: TB_MB(KIND, 32); break; \
+  }
+  switch (gp->kernel) {
+    case TB_RBF: TB_MB_DP(TB_RBF); break;
+    case TB_MATERN12: TB_MB_DP(TB_MATERN12); break;
+    case TB_MATERN32: TB_MB_DP(TB_MATERN32); break;
+    default: TB_MB_DP(TB_MATERN52); break;
+  }
+#undef TB_MB_DP
+#undef TB_MB
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Exact value of n <= chunk_cap gathered candidates (coordinates xs [n][D], global indices is [n]) folded into the running
+// best gp->sRun: K* digits and means from the coordinates, the digit GEMM with the row-block groups G of the unscreened call,
+// the tail and the fold.  split: the k-split of the unscreened chunk the candidates come from (single-pass engine), so the
+// launch's means are that chunk's; a candidate's digits, its sum of squares over G groups and its mean are what the unscreened
+// call computes for it, so its value is too.
+static int argmax_eval_gathered(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, int G, const double* xs, const int64_t* is,
+                                int64_t n, const KSplit* split) {
   cudaStream_t st = gp->stream;
   const int tiles = (int)((n + nt - 1) / nt);
   const int64_t McPad = (int64_t)tiles * nt;
   int8_t* ks = gp->sKs.as<int8_t>();
   double* partial = gp->sPartial.as<double>();
+  double* mean = gp->sMean.as<double>();
   if (fast)
-    TB_TRY(oz5_launch_kstar(gp, st, xs, n, tiles, ks, gp->sMean.as<double>()));
+    TB_TRY(oz5_launch_kstar(gp, st, xs, n, tiles, ks, mean, split));
   else
-    TB_TRY(launch_kstar_digits(gp, xs, n, tiles, ks, gp->sMean.as<double>()));
+    TB_TRY(launch_kstar_digits(gp, xs, n, tiles, ks, mean));
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (gp->profile) {
     TB_CUDA(cudaEventCreate(&e0));
@@ -1105,7 +1255,7 @@ static int argmax_eval_gathered(tb_gp* gp, const EvalRequest& rq, bool fast, int
     gp->prof_event_flops.push_back((double)McPad * (double)gp->N * (double)gp->N);
   }
   TB_CUDA(cudaGetLastError());
-  TB_TRY(launch_tail(gp, st, rq, partial, G, McPad, ms, n, 0, nullptr, nullptr, nullptr, xs, nullptr, is));
+  TB_TRY(launch_tail(gp, st, rq, partial, G, McPad, mean, n, 0, nullptr, nullptr, nullptr, xs, nullptr, is));
   argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), (int)((n + 255) / 256),
                                         gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
   TB_LAUNCHED();
@@ -1113,12 +1263,12 @@ static int argmax_eval_gathered(tb_gp* gp, const EvalRequest& rq, bool fast, int
 }
 
 // Screened argmax of EI / log-EI (argmax_screen_wanted): the variance GEMM runs only for candidates that can still win.
-//   1. mean pass: the K* generation of the unscreened chunking (chunk_cap, tiles, k-split) with the digit stores compiled
-//      out -> the means of all M candidates, bit-identical to the unscreened call's
-//   2. screen: ub = acq(mean, fmax(variance, 1e-12)) bounds the value from above (screen_threshold); its first-max is the probe
-//   3. the probe's exact value tau -> gp->sRun
-//   4. compaction of the survivors (ub >= tau - margin, or ub NaN); the host reads their count (one synchronisation)
-//   5. exact values of the survivors (argmax_eval_gathered), folded on their global indices into gp->sRun
+//   1. bound pass (prescreen.cuh): fp32 means with a rigorous error bound E -> ub = acq(μ̃ - E, var_ub) >= the exact value,
+//      and the first-max of acq(μ̃, var_ub): the probe
+//   2. the probe's exact value tau -> gp->sRun
+//   3. compaction of the survivors (ub >= tau - margin, or ub NaN), grouped by the k-split of their unscreened chunk; the host
+//      reads their counts (one synchronisation)
+//   4. exact values of the survivors (argmax_eval_gathered, with their chunk's k-split), folded on their global indices
 // More than M / 4 survivors: *done stays false, gp->sRun is reset and the caller runs the unscreened chunk loop.
 static int argmax_screened(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, int64_t chunk_cap, int G, bool* done) {
   *done = false;
@@ -1126,61 +1276,66 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, 
   const int D = gp->D;
   const int64_t M = rq.M;
   const int64_t cap = std::max<int64_t>(1, M / 4);
-  const int sblocks = (int)((M + 255) / 256);
-  TB_TRY(gp->sScrMean.reserve(sizeof(double) * (size_t)(((M + nt - 1) / nt) * nt)));  // the last chunk writes its padding too
+  const int sblocks = (int)((M + 255) / 256), bblocks = prescreen_blocks(gp, M);
+  TB_TRY(gp->sScrUb.reserve(sizeof(double) * (size_t)M));
   TB_TRY(gp->sScrX.reserve(sizeof(double) * (size_t)cap * D));
-  TB_TRY(gp->sScrMu.reserve(sizeof(double) * (size_t)cap));
   TB_TRY(gp->sScrIdx.reserve(sizeof(int64_t) * (size_t)cap));
-  TB_TRY(gp->sScrBlk.reserve(16 * (size_t)sblocks + 24));
-  double* mu = gp->sScrMean.as<double>();
+  TB_TRY(gp->sScrBlk.reserve(16 * (size_t)bblocks + 32));
+  double* ub = gp->sScrUb.as<double>();
   double* xsel = gp->sScrX.as<double>();
-  double* msel = gp->sScrMu.as<double>();
   int64_t* isel = gp->sScrIdx.as<int64_t>();
   double* bb = gp->sScrBlk.as<double>();
-  int64_t* bi = reinterpret_cast<int64_t*>(bb + sblocks);
-  double* probe_v = reinterpret_cast<double*>(bi + sblocks);
+  int64_t* bi = reinterpret_cast<int64_t*>(bb + bblocks);
+  double* probe_v = reinterpret_cast<double*>(bi + bblocks);
   int64_t* probe_i = reinterpret_cast<int64_t*>(probe_v + 1);
   unsigned long long* count = reinterpret_cast<unsigned long long*>(probe_v + 2);
-  // 1. mean pass
-  for (int64_t c0 = 0; c0 < M; c0 += chunk_cap) {
-    const int64_t mc = std::min<int64_t>(chunk_cap, M - c0);
-    const int tiles = (int)((mc + nt - 1) / nt);
-    if (fast)
-      TB_TRY(oz5_launch_kstar(gp, st, rq.Xc + c0 * D, mc, tiles, nullptr, mu + c0));
-    else
-      TB_TRY(launch_kstar_digits(gp, rq.Xc + c0 * D, mc, tiles, nullptr, mu + c0));
+  // the unscreened loop's chunks: whole ones over [0, split), the last over [split, M); only the last can have another k-split
+  const int64_t split = ((M - 1) / chunk_cap) * chunk_cap;
+  KSplit ks_full, ks_last;
+  if (fast) {
+    ks_full = oz5_kstar_split(gp, (int)(chunk_cap / nt));
+    ks_last = oz5_kstar_split(gp, (int)((M - split + nt - 1) / nt));
   }
-  // 2. screen
+  const bool same_split = ks_full.ksplit == ks_last.ksplit && ks_full.kc_per == ks_last.kc_per;
+  // 1. bound pass
   const double var_ub = std::fmax(gp->variance, 1e-12);
   const double init_v = -INFINITY;
   const int64_t init_i = INT64_MAX;
   TB_CUDA(cudaMemcpyAsync(probe_v, &init_v, 8, cudaMemcpyHostToDevice, st));
   TB_CUDA(cudaMemcpyAsync(probe_i, &init_i, 8, cudaMemcpyHostToDevice, st));
-  screen_ub_kernel<<<sblocks, 256, 0, st>>>(mu, M, var_ub, rq.acq, rq.param, bb, bi);
+  TB_TRY(launch_mean_bounds(gp, st, rq.Xc, M, rq.acq, rq.param, var_ub, ub, nullptr, bb, bi));
+  argmax_fold_kernel<<<1, 256, 0, st>>>(bb, bi, bblocks, probe_v, probe_i);
   TB_LAUNCHED();
-  argmax_fold_kernel<<<1, 256, 0, st>>>(bb, bi, sblocks, probe_v, probe_i);
+  // 2. probe
+  pre::probe_kernel<<<1, 32, 0, st>>>(rq.Xc, D, probe_i, xsel, isel);
   TB_LAUNCHED();
-  // 3. probe
-  screen_probe_kernel<<<1, 32, 0, st>>>(rq.Xc, mu, D, probe_i, xsel, msel, isel);
+  bool probe_last = true;
+  if (!same_split) {  // the probe's chunk decides its k-split
+    int64_t p = 0;
+    TB_CUDA(cudaMemcpyAsync(&p, probe_i, 8, cudaMemcpyDeviceToHost, st));
+    TB_CUDA(cudaStreamSynchronize(st));
+    probe_last = (p == INT64_MAX ? 0 : p) >= split;
+  }
+  TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel, isel, 1, probe_last ? &ks_last : &ks_full));
+  // 3. compaction
+  TB_CUDA(cudaMemsetAsync(count, 0, 16, st));
+  pre::compact_kernel<<<sblocks, 256, 0, st>>>(rq.Xc, ub, M, split, D, var_ub, rq.acq, gp->sRun.as<double>(), cap, count, xsel, isel);
   TB_LAUNCHED();
-  TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel, msel, isel, 1));
-  // 4. compaction
-  TB_CUDA(cudaMemsetAsync(count, 0, 8, st));
-  screen_compact_kernel<<<sblocks, 256, 0, st>>>(rq.Xc, mu, M, D, var_ub, rq.acq, rq.param, gp->sRun.as<double>(), cap, count, xsel,
-                                                 msel, isel);
-  TB_LAUNCHED();
-  unsigned long long n = 0;
-  TB_CUDA(cudaMemcpyAsync(&n, count, 8, cudaMemcpyDeviceToHost, st));
+  unsigned long long n[2] = {0, 0};
+  TB_CUDA(cudaMemcpyAsync(n, count, 16, cudaMemcpyDeviceToHost, st));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
-  if (n > (unsigned long long)cap) {
+  if (n[0] + n[1] > (unsigned long long)cap) {
     TB_CUDA(cudaMemcpyAsync(gp->sRun.p, &init_v, 8, cudaMemcpyHostToDevice, st));
     TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, st));
     return 0;
   }
-  // 5. exact evaluation of the survivors
-  for (int64_t s0 = 0; s0 < (int64_t)n; s0 += chunk_cap)
-    TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel + s0 * D, msel + s0, isel + s0, std::min<int64_t>(chunk_cap, (int64_t)n - s0)));
+  // 4. exact evaluation of the survivors: whole-chunk ones in slots [0, n0), last-chunk ones in [cap - n1, cap)
+  const int64_t nf = (int64_t)n[0], nb = (int64_t)n[1];
+  for (int64_t s0 = 0; s0 < nf; s0 += chunk_cap)
+    TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel + s0 * D, isel + s0, std::min<int64_t>(chunk_cap, nf - s0), &ks_full));
+  for (int64_t s0 = cap - nb; s0 < cap; s0 += chunk_cap)
+    TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel + s0 * D, isel + s0, std::min<int64_t>(chunk_cap, cap - s0), &ks_last));
   *done = true;
   return 0;
 }
@@ -1948,6 +2103,25 @@ int tb_gp_engine_info(tb_gp* gp, int* digit_products, double* error_estimate) {
   }
   if (digit_products) *digit_products = products;
   if (error_estimate) *error_estimate = est;
+  return 0;
+}
+int tb_gp_mean_bounds(tb_gp* gp, const double* Xc, int64_t M, double* lo, double* hi) {
+  TB_CHECK(gp && Xc && lo && hi, "tb_gp_mean_bounds: null argument");
+  TB_CHECK(gp->cache_valid, "tb_gp_mean_bounds: posterior cache is not built");
+  TB_CHECK(M >= 0, "tb_gp_mean_bounds: negative candidate count");
+  if (M == 0) return 0;
+  TB_CUDA(cudaSetDevice(gp->device));
+  cudaStream_t st = gp->stream;
+  TB_TRY(gp->sXc.reserve(sizeof(double) * (size_t)M * gp->D));
+  TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * (size_t)M));
+  double* x = gp->sXc.as<double>();
+  double* b = gp->sMisc.as<double>();
+  TB_CUDA(cudaMemcpyAsync(x, Xc, sizeof(double) * (size_t)M * gp->D, cudaMemcpyDefault, st));
+  TB_TRY(tb::launch_mean_bounds(gp, st, x, M, -1, 0.0, 0.0, b, b + M, nullptr, nullptr));
+  TB_CUDA(cudaMemcpyAsync(lo, b, sizeof(double) * (size_t)M, cudaMemcpyDefault, st));
+  TB_CUDA(cudaMemcpyAsync(hi, b + M, sizeof(double) * (size_t)M, cudaMemcpyDefault, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  TB_CUDA(cudaGetLastError());
   return 0;
 }
 int tb_gp_kinv_apply(tb_gp* gp, const double* B, int nrhs, double* out) {
