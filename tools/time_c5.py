@@ -1,5 +1,4 @@
-"""Wall-clock timing of the C5 shape (N=8192, D=20, fp32 I/O): forward log-EI and value+gradient, several repetitions
-(TB_OZ_FAST=0 in the environment selects the two-pass 6-digit kernels for comparison)."""
+"""Wall-clock timing of the C5 shape (N=8192, D=20, fp32 I/O): forward log-EI and value+gradient, several repetitions."""
 import os, sys, time, math, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -23,7 +22,7 @@ m = tb.GaussianProcessRegression(tb.build_gpr(ds, tb.Box([0.0] * 20, [1.0] * 20)
 fn = LogExpectedImprovement().prepare_acquisition_function(m, ds)
 xs = torch.rand(12_500, 1, 20, dtype=torch.float32, device="cuda")
 xf = torch.rand(200_000, 1, 20, dtype=torch.float32, device="cuda")
-out = {"engine_info": m.engine_info(), "TB_OZ_FAST": os.environ.get("TB_OZ_FAST")}
+out = {"engine_info": m.engine_info()}
 for name, call in (("grad_ms", lambda: fn.value_and_gradient(xs)), ("forward_ms", lambda: fn(xf))):
     ts = []
     for _ in range(6):

@@ -2,8 +2,8 @@
 and ``MultivariateNormalCDF`` (acquisition/function/utils.py:29-199).
 
 In the reference these wrappers bound the memory of one TensorFlow evaluation by cutting the leading (candidate) axis into
-blocks.  Here the fused kernels already stream any batch through bounded scratch (``run_eval`` / ``run_eval_oz`` chunk at
-~1 GB of K* digits), so the wrappers are not needed for memory; they exist so that callers which wrap their functions or
+blocks.  Here the fused kernels already stream any batch through bounded scratch (``run_eval`` chunks at
+~1 GB of K* scratch), so the wrappers are not needed for memory; they exist so that callers which wrap their functions or
 optimisers keep working, with the reference's splitting rule and error behaviour."""
 from __future__ import annotations
 

@@ -311,6 +311,7 @@ inline int launch(cudaStream_t st, const int8_t* AS, const int8_t* BS, const dou
   if (grid <= 0) return 0;
   digit_gemm_kernel<S, EPI, NTB><<<grid, THREADS, smem_bytes<S>(), st>>>(AS, BS, rowscale, rowsum, NB, nst, G, tiles, McPad, out_scale,
                                                                          half_var, a_planes, b_planes, full_rows, partial, Aplain, lda);
+  TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;
 }

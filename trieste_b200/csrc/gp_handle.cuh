@@ -8,6 +8,8 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <type_traits>
+#include <utility>
 
 namespace tb {
 
@@ -42,12 +44,45 @@ inline bool is_device_ptr(const void* p) {
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
-// supported padded input dimensions of the distance loop (even, so rows load as double2)
-inline int pick_dp(int D) {
-  static const int opts[] = {2, 4, 6, 8, 10, 12, 16, 20, 24, 32};
-  for (int o : opts)
+// supported padded input dimensions of the distance loop (even, so rows load as double2), ascending
+template <int... V>
+struct DpList {};
+using SupportedDp = DpList<2, 4, 6, 8, 10, 12, 16, 20, 24, 32>;
+
+template <int... V>
+inline int pick_dp_in(DpList<V...>, int D) {
+  for (int o : {V...})
     if (D <= o) return o;
   return -1;
+}
+inline int pick_dp(int D) { return pick_dp_in(SupportedDp{}, D); }
+
+// f(std::integral_constant<int, DP>) for the supported DP equal to dp; any other value runs the largest
+template <int V, int... Rest, class F>
+inline decltype(auto) with_dp_in(DpList<V, Rest...>, int dp, F&& f) {
+  if constexpr (sizeof...(Rest) == 0) {
+    return f(std::integral_constant<int, V>{});
+  } else {
+    if (dp == V) return f(std::integral_constant<int, V>{});
+    return with_dp_in(DpList<Rest...>{}, dp, std::forward<F>(f));
+  }
+}
+template <class F>
+inline decltype(auto) with_dp(int dp, F&& f) { return with_dp_in(SupportedDp{}, dp, std::forward<F>(f)); }
+
+// f(std::integral_constant<int, KIND>) for the kernel kind; an unknown kind runs Matern52
+template <class F>
+inline decltype(auto) with_kind(int kernel, F&& f) {
+  switch (kernel) {
+    case TB_RBF: return f(std::integral_constant<int, TB_RBF>{});
+    case TB_MATERN12: return f(std::integral_constant<int, TB_MATERN12>{});
+    case TB_MATERN32: return f(std::integral_constant<int, TB_MATERN32>{});
+    default: return f(std::integral_constant<int, TB_MATERN52>{});
+  }
+}
+template <class F>
+inline decltype(auto) with_kind_dp(int kernel, int dp, F&& f) {
+  return with_kind(kernel, [&](auto K) -> decltype(auto) { return with_dp(dp, [&](auto P) -> decltype(auto) { return f(K, P); }); });
 }
 
 }  // namespace tb
@@ -88,10 +123,7 @@ struct tb_gp {
   bool kinv_dense_valid = false; // dense K^-1 (dKinv, lower triangle, ld = kinv_dense_N) current: kept so that an append can
   int64_t kinv_dense_N = 0;      // update it by rank m (tb_gp_append_data) instead of rebuilding it in O(N^3)
   tb::DevBuf dKinvSpare;
-  tb::DevBuf sKs2, sMean2, sPartial2;  // second scratch slot of the pipelined driver
   tb::DevBuf sMeanPart;                // per-split mean partials of the k-split K* generation (few candidate tiles)
-  cudaStream_t stream2 = nullptr;      // K* digit generation stream (overlaps the digit GEMM)
-  cudaEvent_t evK[2] = {nullptr, nullptr}, evDone[2] = {nullptr, nullptr};
   bool oz_valid = false;
   int nst = 0, oz_bscale_exp = 0;
   double oz_out_scale = 1.0;
@@ -118,7 +150,6 @@ struct tb_gp {
   int mesS = 0;
   tb::DevBuf dPen;              // local penalisation (tb_acq_set_penalization): pending [P][D], radius [P], scale [P]
   int penP = 0, penKind = 0, penD = 0;
-  tb::DevBuf sXc2;              // second candidate staging slot of the pipelined driver (the penalised tail reads candidates)
   // GIBBON repulsion (tb_acq_set_gibbon_repulsion): raw pending points [m][D] and weight, and what is derived from them and
   // the posterior cache: scaled pending points [m][DP], L_B^-1 [mp][m] (zero rows past m), What = K^-1 k(X,P) L_B^-T [N][mp]
   std::vector<double> gibP;

@@ -1,5 +1,5 @@
 // Host side of the single-pass digit engine (ozaki5.cuh): mode selection from an a-priori error bound, digit tiles of Linv,
-// launches of the centred K* digit generation and of the digit GEMM.  Called from tb_api.cu (run_eval_oz).
+// launches of the centred K* digit generation and of the digit GEMM.  Called from tb_api.cu (the engine operations).
 #include "gp_handle.cuh"
 #include "ozaki5.cuh"
 #include "oz5_api.h"
@@ -45,10 +45,9 @@ static int build_digits(tb_gp* gp, cudaStream_t st) {
 int oz5_ensure(tb_gp* gp) {
   if (gp->oz5_valid) return 0;
   gp->oz5_mode = 0;
+  gp->oz5_planes = 0;
   gp->oz5_est = 0.0;
-  int force = -1;  // TB_OZ_FAST=0: never; =1: always (experiments / tests of the fallback)
-  if (const char* e = std::getenv("TB_OZ_FAST")) force = std::atoi(e);
-  if (force == 0 || gp->oz_full || gp->N > 16384) {
+  if (gp->oz_full || gp->N > 16384) {
     gp->oz5_valid = true;
     return 0;
   }
@@ -77,10 +76,10 @@ int oz5_ensure(tb_gp* gp) {
   // if even 4 digits do not clear it the handle is treated like an fp64 one.  Otherwise: the 6-digit two-pass kernels.
   int mode = 0, planes = 0;
   if (gp->dtype == TB_F32) {
-    if (force == 1 || oz5_estimate(gp->variance, mx, gp->N, 3) <= 3e-5) mode = 3, planes = 4;
+    if (oz5_estimate(gp->variance, mx, gp->N, 3) <= 3e-5) mode = 3, planes = 4;
     else if (oz5_estimate(gp->variance, mx, gp->N, 4) <= 3e-5) mode = 4, planes = 4;
   }
-  if (mode == 0 && (force == 1 || oz5_estimate(gp->variance, mx, gp->N, 5) <= (gp->dtype == TB_F32 ? 3e-5 : 3e-10))) mode = 5, planes = 5;
+  if (mode == 0 && oz5_estimate(gp->variance, mx, gp->N, 5) <= (gp->dtype == TB_F32 ? 3e-5 : 3e-10)) mode = 5, planes = 5;
   if (planes == 5) TB_TRY(build_digits<5>(gp, st));
   if (planes == 4) TB_TRY(build_digits<4>(gp, st));
   if (mode) gp->oz5_est = oz5_estimate(gp->variance, mx, gp->N, mode);
@@ -117,9 +116,7 @@ int oz5_ensure_kinv(tb_gp* gp) {
   const int S = gp->oz5_planes;
   const double sB = 0.5 * gp->variance / oz5::FILL;
   const double eps_v = mx * sB * std::sqrt(6.0 * (double)N) * (65536.0 / 12.0) * std::ldexp(1.0, -8 * (S + 2));
-  int force = -1;
-  if (const char* e = std::getenv("TB_OZ_FAST")) force = std::atoi(e);
-  gp->kinv5_ok = force == 1 || eps_v <= (gp->dtype == TB_F32 ? 1e-4 : 1e-7);
+  gp->kinv5_ok = eps_v <= (gp->dtype == TB_F32 ? 1e-4 : 1e-7);
   if (gp->kinv5_ok) {
     const size_t bytes = (size_t)gp->NB * gp->nst * S * oz5::ATILE;
     TB_TRY(gp->dKinvS5.reserve(bytes));
@@ -185,30 +182,10 @@ static int launch_kstar_s(tb_gp* gp, cudaStream_t st, const double* Xc_dev, int6
     TB_TRY(gp->sMeanPart.reserve(sizeof(double) * (size_t)ksplit * mstride));
     mean_dst = gp->sMeanPart.as<double>();
   }
-#define TB_KD(KIND, DPV)                                                                                                      \
-  oz5::kstar_digits_kernel<KIND, DPV, S><<<dim3(ctas, ksplit), TH, 0, st>>>(Xs, X2, al, Xc_dev, il, N, nst, D, mc, var, inv_b, \
-                                                                            dig_c, mc0, fm::Consts(), tiles, kc_per, BS, mean_dst)
-#define TB_KD_DP(KIND)                 \
-  switch (gp->DP) {                    \
-    case 2: TB_KD(KIND, 2); break;     \
-    case 4: TB_KD(KIND, 4); break;     \
-    case 6: TB_KD(KIND, 6); break;     \
-    case 8: TB_KD(KIND, 8); break;     \
-    case 10: TB_KD(KIND, 10); break;   \
-    case 12: TB_KD(KIND, 12); break;   \
-    case 16: TB_KD(KIND, 16); break;   \
-    case 20: TB_KD(KIND, 20); break;   \
-    case 24: TB_KD(KIND, 24); break;   \
-    default: TB_KD(KIND, 32); break;   \
-  }
-  switch (gp->kernel) {
-    case TB_RBF: TB_KD_DP(TB_RBF); break;
-    case TB_MATERN12: TB_KD_DP(TB_MATERN12); break;
-    case TB_MATERN32: TB_KD_DP(TB_MATERN32); break;
-    default: TB_KD_DP(TB_MATERN52); break;
-  }
-#undef TB_KD_DP
-#undef TB_KD
+  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+    oz5::kstar_digits_kernel<decltype(K)::value, decltype(P)::value, S><<<dim3(ctas, ksplit), TH, 0, st>>>(
+        Xs, X2, al, Xc_dev, il, N, nst, D, mc, var, inv_b, dig_c, mc0, fm::Consts(), tiles, kc_per, BS, mean_dst);
+  });
   TB_LAUNCHED();
   if (ksplit > 1) {
     oz5::mean_reduce_kernel<<<(unsigned)((mstride + 255) / 256), 256, 0, st>>>(mean_dst, ksplit, mstride, mc0, mean);
@@ -241,7 +218,6 @@ int oz5_launch_gemm(tb_gp* gp, cudaStream_t st, const int8_t* BS, int tiles, int
   else if (gp->oz5_mode == 4) TB_TRY(TB_GEMM(4));
   else TB_TRY(TB_GEMM(3));
 #undef TB_GEMM
-  TB_LAUNCHED();
   return 0;
 }
 
@@ -257,7 +233,6 @@ int oz5_launch_gemm_store(tb_gp* gp, cudaStream_t st, int left, const int8_t* BS
   if (pl == 5) TB_TRY(TB_GEMM(5));
   else TB_TRY(TB_GEMM(4));
 #undef TB_GEMM
-  TB_LAUNCHED();
   return 0;
 }
 

@@ -271,10 +271,9 @@ int tb_gp_create(tb_gp** out, int device, int dtype) {
   gp->device = device;
   gp->dtype = dtype;
   if (const char* e = std::getenv("TB_FACTOR")) gp->factor_own = std::string(e) != "cusolver";
-  if (const char* e = std::getenv("TB_ENGINE")) gp->engine = (std::string(e) == "fp64") ? 0 : 1;
   {
-    // main stream at the highest priority: when the K*-generation stream (lowest) runs concurrently, GEMM CTAs are placed
-    // first and the generation CTAs only fill the register / thread slots a GEMM CTA leaves free
+    // the handle's stream at the highest priority: a caller that runs its own work on other streams (tb_gp_stream) gets the
+    // candidate GEMMs scheduled first
     int least = 0, greatest = 0;
     TB_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
     TB_CUDA(cudaStreamCreateWithPriority(&gp->stream, cudaStreamNonBlocking, greatest));
@@ -289,24 +288,16 @@ int tb_gp_destroy(tb_gp* gp) {
   cudaSetDevice(gp->device);
   cudaStreamSynchronize(gp->stream);
   for (tb::DevBuf* b : {&gp->dX, &gp->dy, &gp->dXs, &gp->dInvLs, &gp->dAlpha, &gp->dL, &gp->dLinv,
-                        &gp->dLinvP, &gp->dLinvTP, &gp->dAS, &gp->dRowScale, &gp->dKinv, &gp->dKinvS, &gp->dKinvScale, &gp->dDinv, &gp->sKs2, &gp->sMean2, &gp->sPartial2, &gp->dWork, &gp->dInfo, &gp->sKs, &gp->sPartial, &gp->sMean,
+                        &gp->dLinvP, &gp->dLinvTP, &gp->dAS, &gp->dRowScale, &gp->dKinv, &gp->dKinvS, &gp->dKinvScale, &gp->dDinv, &gp->dWork, &gp->dInfo, &gp->sKs, &gp->sPartial, &gp->sMean,
                         &gp->sVals, &gp->sVar, &gp->sXc, &gp->sBlkBest, &gp->sBlkIdx, &gp->sRun,
                         &gp->sA, &gp->sV, &gp->sGrad, &gp->sMisc, &gp->dMes, &gp->dXspare, &gp->dyspare, &gp->dLspare, &gp->dLinvSpare,
                         &gp->dAS5, &gp->dRowScale5, &gp->dRowSum5, &gp->dX2, &gp->dKinvS5, &gp->dKinvScale5, &gp->dKinvSum5,
-                        &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->sXc2, &gp->dGibPs, &gp->dGibLinv, &gp->dGibWhat,
+                        &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->dGibPs, &gp->dGibLinv, &gp->dGibWhat,
                         &gp->sGib, &gp->sScrUb, &gp->sScrX, &gp->sScrIdx, &gp->sScrBlk, &gp->dPreRows, &gp->dPreCentre})
     b->release();
   for (auto& ev : gp->prof_events) {
     cudaEventDestroy(ev.first);
     cudaEventDestroy(ev.second);
-  }
-  if (gp->stream2) {
-    cudaStreamSynchronize(gp->stream2);
-    for (int i = 0; i < 2; ++i) {
-      cudaEventDestroy(gp->evK[i]);
-      cudaEventDestroy(gp->evDone[i]);
-    }
-    cudaStreamDestroy(gp->stream2);
   }
   if (gp->cusolver) cusolverDnDestroy(gp->cusolver);
   if (gp->cublas) cublasDestroy(gp->cublas);
@@ -458,12 +449,7 @@ int tb_gp_update_posterior_cache(tb_gp* gp) {
     dim3 grid((unsigned)((N + 127) / 128), (unsigned)N);
     double* K = gp->dL.as<double>();
     const double* Xs = gp->dXs.as<double>();
-    switch (gp->kernel) {
-      case TB_RBF: gram_kernel<TB_RBF><<<grid, 128, 0, st>>>(Xs, N, DP, gp->variance, gp->noise, K); break;
-      case TB_MATERN12: gram_kernel<TB_MATERN12><<<grid, 128, 0, st>>>(Xs, N, DP, gp->variance, gp->noise, K); break;
-      case TB_MATERN32: gram_kernel<TB_MATERN32><<<grid, 128, 0, st>>>(Xs, N, DP, gp->variance, gp->noise, K); break;
-      default: gram_kernel<TB_MATERN52><<<grid, 128, 0, st>>>(Xs, N, DP, gp->variance, gp->noise, K); break;
-    }
+    with_kind(gp->kernel, [&](auto K_) { gram_kernel<decltype(K_)::value><<<grid, 128, 0, st>>>(Xs, N, DP, gp->variance, gp->noise, K); });
     TB_LAUNCHED();
   }
   TB_TRY(gp->dInfo.reserve(sizeof(int)));
@@ -605,12 +591,9 @@ static int tb_gp_append_data_f64(tb_gp* gp, const double* Xnew, const double* yn
   {
     dim3 grid((unsigned)((N + 127) / 128), (unsigned)m);
     const double* Xs = gp->dXs.as<double>();
-    switch (gp->kernel) {
-      case TB_RBF: append_cross_kernel<TB_RBF><<<grid, 128, 0, st>>>(Xs, DP, N0, N, gp->variance, gp->noise, W); break;
-      case TB_MATERN12: append_cross_kernel<TB_MATERN12><<<grid, 128, 0, st>>>(Xs, DP, N0, N, gp->variance, gp->noise, W); break;
-      case TB_MATERN32: append_cross_kernel<TB_MATERN32><<<grid, 128, 0, st>>>(Xs, DP, N0, N, gp->variance, gp->noise, W); break;
-      default: append_cross_kernel<TB_MATERN52><<<grid, 128, 0, st>>>(Xs, DP, N0, N, gp->variance, gp->noise, W); break;
-    }
+    with_kind(gp->kernel, [&](auto K) {
+      append_cross_kernel<decltype(K)::value><<<grid, 128, 0, st>>>(Xs, DP, N0, N, gp->variance, gp->noise, W);
+    });
     TB_LAUNCHED();
   }
   double* L = gp->dL.as<double>();
@@ -678,29 +661,10 @@ static int launch_kstar(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, 
   const int N = (int)gp->N, nkc = gp->nkc, D = gp->D;
   const double var = gp->variance, mc0 = gp->mean_const;
   cudaStream_t st = gp->stream;
-#define TB_KSTAR(KIND, DPV)                                                                               \
-  kstar_panels_kernel<KIND, DPV><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nkc, D, mc, 0, var, mc0, KsP, mean)
-#define TB_KSTAR_DP(KIND)                                   \
-  switch (gp->DP) {                                         \
-    case 2: TB_KSTAR(KIND, 2); break;                       \
-    case 4: TB_KSTAR(KIND, 4); break;                       \
-    case 6: TB_KSTAR(KIND, 6); break;                       \
-    case 8: TB_KSTAR(KIND, 8); break;                       \
-    case 10: TB_KSTAR(KIND, 10); break;                     \
-    case 12: TB_KSTAR(KIND, 12); break;                     \
-    case 16: TB_KSTAR(KIND, 16); break;                     \
-    case 20: TB_KSTAR(KIND, 20); break;                     \
-    case 24: TB_KSTAR(KIND, 24); break;                     \
-    default: TB_KSTAR(KIND, 32); break;                     \
-  }
-  switch (gp->kernel) {
-    case TB_RBF: TB_KSTAR_DP(TB_RBF); break;
-    case TB_MATERN12: TB_KSTAR_DP(TB_MATERN12); break;
-    case TB_MATERN32: TB_KSTAR_DP(TB_MATERN32); break;
-    default: TB_KSTAR_DP(TB_MATERN52); break;
-  }
-#undef TB_KSTAR_DP
-#undef TB_KSTAR
+  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+    kstar_panels_kernel<decltype(K)::value, decltype(P)::value><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nkc, D, mc, 0, var, mc0,
+                                                                                        KsP, mean);
+  });
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;
@@ -714,12 +678,6 @@ static int64_t chunk_tiles(const tb_gp* gp) {
   t = std::max<int64_t>(t, 1);
   if (t >= NUM_SMS) t = (t / NUM_SMS) * NUM_SMS;
   return std::min<int64_t>(t, NUM_SMS * 16);
-}
-
-static int pick_groups(const tb_gp* gp, int tiles) {
-  if (tiles >= NUM_SMS) return 1;
-  int G = (2 * NUM_SMS + tiles - 1) / tiles;
-  return std::max(1, std::min(G, gp->NB));
 }
 
 int kernels_init() {
@@ -753,8 +711,9 @@ static int ensure_upper_panels(tb_gp* gp) {
   return 0;
 }
 
-template <int KIND>
-static void launch_grad_dp(tb_gp* gp, const double* xc, int64_t mc, double* grad_dev) {
+// gradient assembly of one chunk (grad_kernel): the training-point sums over V = K^-1 K* in gp->sV, with the partials
+// d acq / d (mean, var) in gp->sMisc
+static int launch_grad(tb_gp* gp, const double* xc, int64_t mc, double* grad_dev) {
   const bool wide = mc <= 2048;  // one CTA (8 warps) per candidate when one warp each would leave SMs idle
   const int blocks = wide ? (int)mc : (int)((mc + 7) / 8);
   const double* Xs = gp->dXs.as<double>();
@@ -764,50 +723,21 @@ static void launch_grad_dp(tb_gp* gp, const double* xc, int64_t mc, double* grad
   const int64_t ldv = (int64_t)gp->NB * BM;
   const double* cmu = gp->sMisc.as<double>();
   const double* cvar = cmu + mc;
-#define TB_GRAD(DPV)                                                                                                                     \
-  if (wide)                                                                                                                              \
-    grad_kernel<KIND, DPV, 8><<<blocks, 256, 0, gp->stream>>>(Xs, al, xc, il, (int)gp->N, gp->D, mc, V, ldv, cmu, cvar, gp->variance,     \
-                                                              fm::Consts(), grad_dev);                                                   \
-  else                                                                                                                                   \
-    grad_kernel<KIND, DPV, 1><<<blocks, 256, 0, gp->stream>>>(Xs, al, xc, il, (int)gp->N, gp->D, mc, V, ldv, cmu, cvar, gp->variance,     \
-                                                              fm::Consts(), grad_dev)
-  switch (gp->DP) {
-    case 2: TB_GRAD(2); break;
-    case 4: TB_GRAD(4); break;
-    case 6: TB_GRAD(6); break;
-    case 8: TB_GRAD(8); break;
-    case 10: TB_GRAD(10); break;
-    case 12: TB_GRAD(12); break;
-    case 16: TB_GRAD(16); break;
-    case 20: TB_GRAD(20); break;
-    case 24: TB_GRAD(24); break;
-    default: TB_GRAD(32); break;
-  }
-#undef TB_GRAD
+  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+    constexpr int KIND = decltype(K)::value, DP = decltype(P)::value;
+    if (wide)
+      grad_kernel<KIND, DP, 8><<<blocks, 256, 0, gp->stream>>>(Xs, al, xc, il, (int)gp->N, gp->D, mc, V, ldv, cmu, cvar, gp->variance,
+                                                               fm::Consts(), grad_dev);
+    else
+      grad_kernel<KIND, DP, 1><<<blocks, 256, 0, gp->stream>>>(Xs, al, xc, il, (int)gp->N, gp->D, mc, V, ldv, cmu, cvar, gp->variance,
+                                                               fm::Consts(), grad_dev);
+  });
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 static inline bool gibbon_repulsion_kind(int acq) { return acq == TB_ACQ_GIBBON_REPULSION || acq == TB_ACQ_GIBBON; }
-
-#define TB_GIB_DP(LAUNCH, KIND) \
-  switch (gp->DP) {             \
-    case 2: LAUNCH(KIND, 2); break;   \
-    case 4: LAUNCH(KIND, 4); break;   \
-    case 6: LAUNCH(KIND, 6); break;   \
-    case 8: LAUNCH(KIND, 8); break;   \
-    case 10: LAUNCH(KIND, 10); break; \
-    case 12: LAUNCH(KIND, 12); break; \
-    case 16: LAUNCH(KIND, 16); break; \
-    case 20: LAUNCH(KIND, 20); break; \
-    case 24: LAUNCH(KIND, 24); break; \
-    default: LAUNCH(KIND, 32); break; \
-  }
-#define TB_GIB_KIND(LAUNCH)                           \
-  switch (gp->kernel) {                               \
-    case TB_RBF: TB_GIB_DP(LAUNCH, TB_RBF); break;           \
-    case TB_MATERN12: TB_GIB_DP(LAUNCH, TB_MATERN12); break; \
-    case TB_MATERN32: TB_GIB_DP(LAUNCH, TB_MATERN32); break; \
-    default: TB_GIB_DP(LAUNCH, TB_MATERN52); break;          \
-  }
 
 // GIBBON cross term of one chunk (ensure_gibbon has run): |u|^2 into sGib[0, mc); with keep_u also u into sGib[2 mc, ...) for
 // gibbon_grad_kernel.  One launch whatever m.
@@ -816,12 +746,11 @@ static int launch_gibbon_cross(tb_gp* gp, cudaStream_t st, const double* xc, int
   double* uu = gp->sGib.as<double>();
   double* U = keep_u ? uu + 2 * mc : nullptr;
   const unsigned blocks = (unsigned)((mc + 127) / 128);
-#define TB_GIB_CROSS(KIND, DPV)                                                                                                  \
-  gibbon_cross_kernel<KIND, DPV><<<blocks, 128, 0, st>>>(gp->dXs.as<double>(), gp->dGibWhat.as<double>(), gp->dGibPs.as<double>(), \
-                                                         gp->dGibLinv.as<double>(), xc, gp->dInvLs.as<double>(), (int)gp->N, gp->D,  \
-                                                         gp->gibM, gp->gibMp, mc, gp->variance, fm::Consts(), uu, U)
-  TB_GIB_KIND(TB_GIB_CROSS)
-#undef TB_GIB_CROSS
+  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+    gibbon_cross_kernel<decltype(K)::value, decltype(P)::value><<<blocks, 128, 0, st>>>(
+        gp->dXs.as<double>(), gp->dGibWhat.as<double>(), gp->dGibPs.as<double>(), gp->dGibLinv.as<double>(), xc, gp->dInvLs.as<double>(),
+        (int)gp->N, gp->D, gp->gibM, gp->gibMp, mc, gp->variance, fm::Consts(), uu, U);
+  });
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;
@@ -831,12 +760,11 @@ static int launch_gibbon_cross(tb_gp* gp, cudaStream_t st, const double* xc, int
 static int launch_gibbon_grad(tb_gp* gp, cudaStream_t st, const double* xc, int64_t mc, double* gd) {
   const double* uu = gp->sGib.as<double>();
   const unsigned blocks = (unsigned)((mc + 7) / 8);
-#define TB_GIB_GRAD(KIND, DPV)                                                                                                  \
-  gibbon_grad_kernel<KIND, DPV><<<blocks, 256, 0, st>>>(gp->dXs.as<double>(), gp->dGibWhat.as<double>(), gp->dGibPs.as<double>(), \
-                                                        gp->dGibLinv.as<double>(), xc, gp->dInvLs.as<double>(), (int)gp->N, gp->D,  \
-                                                        gp->gibM, gp->gibMp, mc, gp->variance, uu + 2 * mc, uu + mc, gd)
-  TB_GIB_KIND(TB_GIB_GRAD)
-#undef TB_GIB_GRAD
+  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+    gibbon_grad_kernel<decltype(K)::value, decltype(P)::value><<<blocks, 256, 0, st>>>(
+        gp->dXs.as<double>(), gp->dGibWhat.as<double>(), gp->dGibPs.as<double>(), gp->dGibLinv.as<double>(), xc, gp->dInvLs.as<double>(),
+        (int)gp->N, gp->D, gp->gibM, gp->gibMp, mc, gp->variance, uu + 2 * mc, uu + mc, gd);
+  });
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;
@@ -896,28 +824,6 @@ static int launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const 
   return 0;
 }
 
-// after the lower GEMM (A stored as packed panels in sA, sum-of-squares in sPartial):
-// V = Linv^T A, then the gradient assembly
-static int gradient_chunk(tb_gp* gp, int acq, double param, const double* xc, int64_t mc, int tiles, int G,
-                          int64_t McPad, double* gd) {  // gd: device [mc][D]
-  cudaStream_t st = gp->stream;
-  TB_TRY(launch_partials(gp, st, acq, param, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), xc, mc));
-  const int nkB = gp->NB * (BM / BK);
-  trigemm_kernel<true, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-      gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB, nkB, G, McPad, nullptr, nullptr, gp->sV.as<double>(),
-      (int64_t)gp->NB * BM);
-  TB_LAUNCHED();
-  switch (gp->kernel) {
-    case TB_RBF: launch_grad_dp<TB_RBF>(gp, xc, mc, gd); break;
-    case TB_MATERN12: launch_grad_dp<TB_MATERN12>(gp, xc, mc, gd); break;
-    case TB_MATERN32: launch_grad_dp<TB_MATERN32>(gp, xc, mc, gd); break;
-    default: launch_grad_dp<TB_MATERN52>(gp, xc, mc, gd); break;
-  }
-  TB_LAUNCHED();
-  TB_CUDA(cudaGetLastError());
-  return 0;
-}
-
 // fp32 models (TB_F32 handles) run the HI pass only: 10 digit products, error ~1e-7 sigma_f^2 << the fp32 tolerance
 static inline int oz_npass(const tb_gp* gp) { return gp->dtype == TB_F32 ? 1 : 2; }
 
@@ -930,7 +836,6 @@ static int ensure_ozaki(tb_gp* gp) {
   gp->nst = (int)((gp->N + oz::KST - 1) / oz::KST);
   TB_TRY(gp->dRowScale.reserve(sizeof(double) * rows));
   oz::linv_rowscale_kernel<<<(unsigned)rows, 256, 0, st>>>(gp->dLinv.as<double>(), gp->N, rows, gp->dRowScale.as<double>());
-  TB_LAUNCHED();
   TB_LAUNCHED();
   const int64_t nstages = oz::a_stage_offset(gp->NB);
   TB_TRY(gp->dAS.reserve((size_t)nstages * oz::S * oz::TILE));
@@ -997,27 +902,6 @@ static int ensure_kinv_digits(tb_gp* gp) {
   return 0;
 }
 
-// int8 engine, gradient path: sum-of-squares is already in sPartial (variance GEMM); V = K^-1 k* on the tensor cores
-static int gradient_chunk_oz(tb_gp* gp, int acq, double param, const double* xc, int64_t mc, int tiles, int G, int64_t McPad,
-                             double* gd) {  // gd: device [mc][D]
-  cudaStream_t st = gp->stream;
-  TB_TRY(launch_partials(gp, st, acq, param, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), xc, mc));
-  const int Gv = std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)));
-  TB_TRY(oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dKinvS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dKinvScale.as<double>(), gp->NB,
-                                          gp->nst, Gv, McPad, gp->oz_out_scale, oz_npass(gp), 1, nullptr, gp->sV.as<double>(),
-                                          (int64_t)gp->NB * BM));
-  TB_LAUNCHED();
-  switch (gp->kernel) {
-    case TB_RBF: launch_grad_dp<TB_RBF>(gp, xc, mc, gd); break;
-    case TB_MATERN12: launch_grad_dp<TB_MATERN12>(gp, xc, mc, gd); break;
-    case TB_MATERN32: launch_grad_dp<TB_MATERN32>(gp, xc, mc, gd); break;
-    default: launch_grad_dp<TB_MATERN52>(gp, xc, mc, gd); break;
-  }
-  TB_LAUNCHED();
-  TB_CUDA(cudaGetLastError());
-  return 0;
-}
-
 static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean) {
   const double* Xs = gp->dXs.as<double>();
   const double* al = gp->dAlpha.as<double>();
@@ -1026,29 +910,10 @@ static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int 
   const double var = gp->variance, mc0 = gp->mean_const;
   const double inv_b = std::ldexp(1.0, 48 - gp->oz_bscale_exp);
   cudaStream_t st = gp->stream;
-#define TB_KD(KIND, DPV) \
-  oz::kstar_digits_kernel<KIND, DPV><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nst, D, mc, var, inv_b, mc0, BS, mean)
-#define TB_KD_DP(KIND)                                 \
-  switch (gp->DP) {                                      \
-    case 2: TB_KD(KIND, 2); break;                       \
-    case 4: TB_KD(KIND, 4); break;                       \
-    case 6: TB_KD(KIND, 6); break;                       \
-    case 8: TB_KD(KIND, 8); break;                       \
-    case 10: TB_KD(KIND, 10); break;                     \
-    case 12: TB_KD(KIND, 12); break;                     \
-    case 16: TB_KD(KIND, 16); break;                     \
-    case 20: TB_KD(KIND, 20); break;                     \
-    case 24: TB_KD(KIND, 24); break;                     \
-    default: TB_KD(KIND, 32); break;                     \
-  }
-  switch (gp->kernel) {
-    case TB_RBF: TB_KD_DP(TB_RBF); break;
-    case TB_MATERN12: TB_KD_DP(TB_MATERN12); break;
-    case TB_MATERN32: TB_KD_DP(TB_MATERN32); break;
-    default: TB_KD_DP(TB_MATERN52); break;
-  }
-#undef TB_KD_DP
-#undef TB_KD
+  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+    oz::kstar_digits_kernel<decltype(K)::value, decltype(P)::value><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nst, D, mc, var, inv_b,
+                                                                                            mc0, BS, mean);
+  });
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;
@@ -1190,76 +1055,253 @@ static int launch_mean_bounds(tb_gp* gp, cudaStream_t st, const double* Xc, int6
   const double* il = gp->dInvLs.as<double>();
   const double* cen = gp->dPreCentre.as<double>();
   const unsigned blocks = (unsigned)prescreen_blocks(gp, M);
-#define TB_MB(KIND, DPV)                                                                                                         \
-  pre::mean_bounds_kernel<KIND, DPV><<<blocks, pre::TH, 0, st>>>(rows, nst, Xc, il, cen, D, M, b, acq, param, var_ub, out0, out1, \
-                                                                 blk_best, blk_idx)
-#define TB_MB_DP(KIND)               \
-  switch (gp->DP) {                  \
-    case 2: TB_MB(KIND, 2); break;   \
-    case 4: TB_MB(KIND, 4); break;   \
-    case 6: TB_MB(KIND, 6); break;   \
-    case 8: TB_MB(KIND, 8); break;   \
-    case 10: TB_MB(KIND, 10); break; \
-    case 12: TB_MB(KIND, 12); break; \
-    case 16: TB_MB(KIND, 16); break; \
-    case 20: TB_MB(KIND, 20); break; \
-    case 24: TB_MB(KIND, 24); break; \
-    default: TB_MB(KIND, 32); break; \
-  }
-  switch (gp->kernel) {
-    case TB_RBF: TB_MB_DP(TB_RBF); break;
-    case TB_MATERN12: TB_MB_DP(TB_MATERN12); break;
-    case TB_MATERN32: TB_MB_DP(TB_MATERN32); break;
-    default: TB_MB_DP(TB_MATERN52); break;
-  }
-#undef TB_MB_DP
-#undef TB_MB
+  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+    pre::mean_bounds_kernel<decltype(K)::value, decltype(P)::value><<<blocks, pre::TH, 0, st>>>(rows, nst, Xc, il, cen, D, M, b, acq, param,
+                                                                                                 var_ub, out0, out1, blk_best, blk_idx);
+  });
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;
 }
 
-// Exact value of n <= chunk_cap gathered candidates (coordinates xs [n][D], global indices is [n]) folded into the running
-// best gp->sRun: K* digits and means from the coordinates, the digit GEMM with the row-block groups G of the unscreened call,
-// the tail and the fold.  split: the k-split of the unscreened chunk the candidates come from (single-pass engine), so the
-// launch's means are that chunk's; a candidate's digits, its sum of squares over G groups and its mean are what the unscreened
-// call computes for it, so its value is too.
-static int argmax_eval_gathered(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, int G, const double* xs, const int64_t* is,
-                                int64_t n, const KSplit* split) {
-  cudaStream_t st = gp->stream;
-  const int tiles = (int)((n + nt - 1) / nt);
-  const int64_t McPad = (int64_t)tiles * nt;
-  int8_t* ks = gp->sKs.as<int8_t>();
-  double* partial = gp->sPartial.as<double>();
+// =================================================================================================
+// GEMM engines of the candidate path.  select_engine decides which one a call runs; the operations below hold each
+// engine's launches.
+// =================================================================================================
+enum class Engine {
+  F64,   // native fp64 DMMA kernels (kernels_f64.cuh)
+  OZ21,  // two-pass 6-digit int8 engine, 21 digit products (ozaki.cuh)
+  OZ15,  // single-pass int8 engine (ozaki5.cuh): 15 digit products on fp64 handles, 6 or 10 on fp32 ones
+};
+
+// The engine of a call, after the lazy builds it needs.  need_v: the call also needs V = K^-1 K* (gradients).  The int8
+// engines' int32 accumulators are exact up to K = N = 16384; larger models and engine 0 run the fp64 kernels.  The
+// single-pass engine runs when its a-priori error estimate admits the handle (oz5_ensure) and, for V, when the V GEMM's own
+// estimate does too (oz5_ensure_kinv); otherwise the 21-product engine does.
+static int select_engine(tb_gp* gp, bool need_v, Engine* eng) {
+  if (!(gp->engine == 1 && gp->N <= 16384)) {
+    if (need_v) TB_TRY(ensure_upper_panels(gp));
+    *eng = Engine::F64;
+    return 0;
+  }
+  TB_TRY(oz5_ensure(gp));
+  // oz5_ensure sets oz5_mode (the digits the variance GEMM computes with) and oz5_planes (the digits stored) together, both
+  // zero or both non-zero, so either one says whether the single-pass engine is admitted
+  bool fast = gp->oz5_planes != 0;
+  if (fast && need_v) {
+    TB_TRY(ensure_kinv_dense(gp));
+    TB_TRY(oz5_ensure_kinv(gp));
+    fast = gp->kinv5_ok;
+  }
+  if (!fast) {
+    TB_TRY(ensure_ozaki(gp));
+    if (need_v) TB_TRY(ensure_kinv_digits(gp));
+  }
+  *eng = fast ? Engine::OZ15 : Engine::OZ21;
+  return 0;
+}
+
+// candidates per K* tile, and the K* scratch bytes per tile
+static int eng_tile_width(const tb_gp* gp, Engine e) { return e == Engine::OZ15 ? oz5_tile_width(gp) : BT; }
+static size_t eng_tile_bytes(const tb_gp* gp, Engine e) {
+  switch (e) {
+    case Engine::F64: return (size_t)gp->nkc * PANEL * sizeof(double);
+    case Engine::OZ21: return (size_t)gp->nst * oz::S * oz::TILE;
+    default: return oz5_tile_bytes(gp);
+  }
+}
+
+// Row-block groups per candidate tile of the Linv GEMMs.  int8 engines: ~4 row-blocks per CTA amortise the CTA prologue
+// while the co-resident CTAs share few enough candidate tiles for the K* digits to stay in L2; small batches get more
+// groups (>= 2 items per SM).  fp64 engine: one group from a full wave of tiles on.
+static int eng_groups(const tb_gp* gp, Engine e, int tiles) {
+  const int fill = (2 * NUM_SMS + tiles - 1) / tiles;
+  if (e == Engine::F64) return tiles >= NUM_SMS ? 1 : std::max(1, std::min(fill, gp->NB));
+  return std::max(std::max(1, (gp->NB + 3) / 4), std::min(gp->NB, fill));
+}
+
+// K* of mc device candidates into gp->sKs (fp64 panels or digit tiles), their posterior means into gp->sMean.
+// split: the single-pass engine's k-split (nullptr: the one oz5_kstar_split gives for this many tiles)
+static int eng_kstar(tb_gp* gp, Engine e, const double* xc, int64_t mc, int tiles, const KSplit* split = nullptr) {
   double* mean = gp->sMean.as<double>();
-  if (fast)
-    TB_TRY(oz5_launch_kstar(gp, st, xs, n, tiles, ks, mean, split));
-  else
-    TB_TRY(launch_kstar_digits(gp, xs, n, tiles, ks, mean));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (gp->profile) {
-    TB_CUDA(cudaEventCreate(&e0));
-    TB_CUDA(cudaEventCreate(&e1));
-    TB_CUDA(cudaEventRecord(e0, st));
+  switch (e) {
+    case Engine::F64: return launch_kstar(gp, xc, mc, tiles, gp->sKs.as<double>(), mean);
+    case Engine::OZ21: return launch_kstar_digits(gp, xc, mc, tiles, gp->sKs.as<int8_t>(), mean);
+    default: return oz5_launch_kstar(gp, gp->stream, xc, mc, tiles, gp->sKs.as<int8_t>(), mean, split);
   }
-  if (fast) {
-    TB_TRY(oz5_launch_gemm(gp, st, ks, tiles, G, McPad, partial));
-  } else {
-    TB_TRY(oz::launch_trigemm<oz::OZ_SUMSQ>(st, tiles, gp->dAS.as<int8_t>(), ks, gp->dRowScale.as<double>(), gp->NB, gp->nst, G, McPad,
-                                            gp->oz_out_scale, oz_npass(gp), 0, partial, nullptr, 0));
-    TB_LAUNCHED();
+}
+
+// Variance GEMM: sums of squares of A = Linv K* over G row-block groups into gp->sPartial.  fp64 engine with packed_a: A
+// also goes to gp->sA as packed panels, the operand of its V GEMM.
+static int eng_variance(tb_gp* gp, Engine e, int tiles, int G, int64_t McPad, bool packed_a) {
+  cudaStream_t st = gp->stream;
+  double* partial = gp->sPartial.as<double>();
+  switch (e) {
+    case Engine::F64:
+      if (packed_a)
+        trigemm_kernel<false, EPI_SUMSQ_PACKED><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
+            gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, gp->sA.as<double>(), nullptr, 0);
+      else
+        trigemm_kernel<false, EPI_SUMSQ><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
+            gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, nullptr, nullptr, 0);
+      TB_LAUNCHED();
+      TB_CUDA(cudaGetLastError());
+      return 0;
+    case Engine::OZ21:
+      return oz::launch_trigemm<oz::OZ_SUMSQ>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
+                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 0, partial, nullptr, 0);
+    default: return oz5_launch_gemm(gp, st, gp->sKs.as<int8_t>(), tiles, G, McPad, partial);
   }
-  if (gp->profile) {
-    TB_CUDA(cudaEventRecord(e1, st));
-    gp->prof_events.emplace_back(e0, e1);
-    gp->prof_event_flops.push_back((double)McPad * (double)gp->N * (double)gp->N);
+}
+
+// A = Linv K* stored plain into out ([candidate][NB*128])
+static int eng_store_a(tb_gp* gp, Engine e, int tiles, int64_t McPad, double* out) {
+  cudaStream_t st = gp->stream;
+  const int64_t lda = (int64_t)gp->NB * BM;
+  const int G = eng_groups(gp, e, tiles);
+  switch (e) {
+    case Engine::F64:
+      trigemm_kernel<false, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB,
+                                                                                    gp->nkc, G, McPad, nullptr, nullptr, out, lda);
+      TB_LAUNCHED();
+      TB_CUDA(cudaGetLastError());
+      return 0;
+    case Engine::OZ21:
+      return oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
+                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 0, nullptr, out, lda);
+    default: return oz5_launch_gemm_store(gp, st, 0, gp->sKs.as<int8_t>(), tiles, G, out, lda);
   }
-  TB_CUDA(cudaGetLastError());
-  TB_TRY(launch_tail(gp, st, rq, partial, G, McPad, mean, n, 0, nullptr, nullptr, nullptr, xs, nullptr, is));
-  argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), (int)((n + 255) / 256),
-                                        gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
+}
+
+// V = K^-1 K* stored plain into gp->sV ([candidate][NB*128]).  fp64 engine: Linv^T A over the packed A that eng_variance left
+// in gp->sA; int8 engines: the digit tiles of the dense K^-1 times the same K* digits.
+static int eng_store_v(tb_gp* gp, Engine e, int tiles, int64_t McPad) {
+  cudaStream_t st = gp->stream;
+  const int64_t ldv = (int64_t)gp->NB * BM;
+  double* V = gp->sV.as<double>();
+  switch (e) {
+    case Engine::F64: {
+      const int G = eng_groups(gp, e, tiles);
+      trigemm_kernel<true, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB,
+                                                                                   gp->NB * (BM / BK), G, McPad, nullptr, nullptr, V, ldv);
+      TB_LAUNCHED();
+      TB_CUDA(cudaGetLastError());
+      return 0;
+    }
+    case Engine::OZ21: {
+      const int G = std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)));
+      return oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dKinvS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dKinvScale.as<double>(), gp->NB,
+                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 1, nullptr, V, ldv);
+    }
+    default: return oz5_launch_gemm_store(gp, st, 1, gp->sKs.as<int8_t>(), tiles, eng_groups(gp, e, tiles), V, ldv);
+  }
+}
+
+// =================================================================================================
+// per-candidate driver
+// =================================================================================================
+
+// the running argmax of a call in gp->sRun (best value, then its index)
+static int argmax_reset(tb_gp* gp) {
+  const double init_v = -INFINITY;  // a candidate worth -inf still beats "nothing seen" through the lower-index tie rule
+  const int64_t init_i = INT64_MAX;
+  TB_CUDA(cudaMemcpyAsync(gp->sRun.p, &init_v, 8, cudaMemcpyHostToDevice, gp->stream));
+  TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, gp->stream));
+  return 0;
+}
+static int argmax_fold(tb_gp* gp, int64_t n) {  // the tail's per-block winners of n candidates into gp->sRun
+  argmax_fold_kernel<<<1, 256, 0, gp->stream>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), (int)((n + 255) / 256),
+                                                gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
   TB_LAUNCHED();
   return 0;
+}
+static int argmax_read(tb_gp* gp, EvalRequest& rq) {
+  TB_CUDA(cudaMemcpyAsync(&rq.best_value, gp->sRun.p, 8, cudaMemcpyDeviceToHost, gp->stream));
+  TB_CUDA(cudaMemcpyAsync(&rq.best_index, (char*)gp->sRun.p + 8, 8, cudaMemcpyDeviceToHost, gp->stream));
+  return 0;
+}
+
+// tb_gp_profile: CUDA events around each variance GEMM, accumulated into the handle's counters by profile_fold once the
+// call has synchronised
+template <class F>
+static int profiled_gemm(tb_gp* gp, double flops, F&& launch) {
+  if (!gp->profile) return launch();
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  TB_CUDA(cudaEventCreate(&e0));
+  TB_CUDA(cudaEventCreate(&e1));
+  TB_CUDA(cudaEventRecord(e0, gp->stream));
+  TB_TRY(launch());
+  TB_CUDA(cudaEventRecord(e1, gp->stream));
+  gp->prof_events.emplace_back(e0, e1);
+  gp->prof_event_flops.push_back(flops);
+  return 0;
+}
+static int profile_fold(tb_gp* gp) {
+  for (size_t i = 0; i < gp->prof_events.size(); ++i) {
+    float ms = 0.f;
+    TB_CUDA(cudaEventElapsedTime(&ms, gp->prof_events[i].first, gp->prof_events[i].second));
+    gp->prof_ms += ms;
+    gp->prof_flops += gp->prof_event_flops[i];
+    gp->prof_launches += 1;
+    cudaEventDestroy(gp->prof_events[i].first);
+    cudaEventDestroy(gp->prof_events[i].second);
+  }
+  gp->prof_events.clear();
+  gp->prof_event_flops.clear();
+  return 0;
+}
+
+// where one chunk's outputs go (null: not requested)
+struct EvalOut {
+  double *vals = nullptr, *mean = nullptr, *var = nullptr, *grad = nullptr;
+};
+// The caller's device arrays are written in place; host arrays go through the handle's staging buffers (the means through
+// gp->sMean, which the K* step fills anyway) and copy_back brings them home.
+struct EvalRoutes {
+  bool xc, vals, mean, var, grad;  // device pointers?
+  explicit EvalRoutes(const EvalRequest& rq)
+      : xc(is_device_ptr(rq.Xc)), vals(is_device_ptr(rq.out_vals)), mean(is_device_ptr(rq.out_mean)), var(is_device_ptr(rq.out_var)),
+        grad(is_device_ptr(rq.out_grad)) {}
+  EvalOut chunk(tb_gp* gp, const EvalRequest& rq, int64_t c0) const {
+    EvalOut o;
+    if (rq.out_vals) o.vals = vals ? rq.out_vals + c0 : gp->sVals.as<double>();
+    if (rq.out_mean && mean) o.mean = rq.out_mean + c0;
+    if (rq.out_var) o.var = var ? rq.out_var + c0 : gp->sVar.as<double>();
+    if (rq.out_grad) o.grad = grad ? rq.out_grad + c0 * gp->D : gp->sGrad.as<double>();
+    return o;
+  }
+  int copy_back(tb_gp* gp, const EvalRequest& rq, int64_t c0, int64_t mc, const EvalOut& o) const {
+    cudaStream_t st = gp->stream;
+    if (rq.out_grad && !grad)
+      TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * gp->D, o.grad, sizeof(double) * mc * gp->D, cudaMemcpyDeviceToHost, st));
+    if (rq.out_vals && !vals) TB_CUDA(cudaMemcpyAsync(rq.out_vals + c0, o.vals, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+    if (rq.out_mean && !mean) TB_CUDA(cudaMemcpyAsync(rq.out_mean + c0, gp->sMean.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+    if (rq.out_var && !var) TB_CUDA(cudaMemcpyAsync(rq.out_var + c0, o.var, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+    return 0;
+  }
+};
+
+// One chunk of n device candidates at xc: K* and the means, the variance GEMM over G row-block groups, the gradient when
+// o.grad is set, the acquisition tail and the argmax fold.  c0: global index of the first candidate.  The screened argmax's
+// gathered candidates pass their global indices in idx_map instead, and the k-split of the chunk they come from.
+static int eval_chunk(tb_gp* gp, const EvalRequest& rq, Engine e, const double* xc, int64_t n, int64_t c0, int G, const EvalOut& o,
+                      const int64_t* idx_map = nullptr, const KSplit* split = nullptr) {
+  cudaStream_t st = gp->stream;
+  const int nt = eng_tile_width(gp, e);
+  const int tiles = (int)((n + nt - 1) / nt);
+  const int64_t McPad = (int64_t)tiles * nt;
+  const double* partial = gp->sPartial.as<double>();
+  const double* mean = gp->sMean.as<double>();
+  TB_TRY(eng_kstar(gp, e, xc, n, tiles, split));
+  TB_TRY(profiled_gemm(gp, (double)McPad * (double)gp->N * (double)gp->N,
+                       [&] { return eng_variance(gp, e, tiles, G, McPad, o.grad != nullptr); }));
+  if (o.grad) {
+    TB_TRY(launch_partials(gp, st, rq.acq, rq.param, partial, G, McPad, mean, xc, n));
+    TB_TRY(eng_store_v(gp, e, tiles, McPad));
+    TB_TRY(launch_grad(gp, xc, n, o.grad));
+  }
+  TB_TRY(launch_tail(gp, st, rq, partial, G, McPad, mean, n, c0, o.vals, o.mean, o.var, xc, o.grad, idx_map));
+  return rq.want_argmax ? argmax_fold(gp, n) : 0;
 }
 
 // Screened argmax of EI / log-EI (argmax_screen_wanted): the variance GEMM runs only for candidates that can still win.
@@ -1268,12 +1310,14 @@ static int argmax_eval_gathered(tb_gp* gp, const EvalRequest& rq, bool fast, int
 //   2. the probe's exact value tau -> gp->sRun
 //   3. compaction of the survivors (ub >= tau - margin, or ub NaN), grouped by the k-split of their unscreened chunk; the host
 //      reads their counts (one synchronisation)
-//   4. exact values of the survivors (argmax_eval_gathered, with their chunk's k-split), folded on their global indices
-// More than M / 4 survivors: *done stays false, gp->sRun is reset and the caller runs the unscreened chunk loop.
-static int argmax_screened(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, int64_t chunk_cap, int G, bool* done) {
+//   4. exact values of the survivors (eval_chunk with their chunk's k-split and the call's G), folded on their global indices
+// A gathered candidate's digits, its sum of squares over G groups and its mean are what the unscreened call computes for it,
+// so its value is too.  More than M / 4 survivors: *done stays false, gp->sRun is reset and the caller runs the unscreened
+// chunk loop.
+static int argmax_screened(tb_gp* gp, const EvalRequest& rq, Engine e, int64_t chunk_cap, int G, bool* done) {
   *done = false;
   cudaStream_t st = gp->stream;
-  const int D = gp->D;
+  const int D = gp->D, nt = eng_tile_width(gp, e);
   const int64_t M = rq.M;
   const int64_t cap = std::max<int64_t>(1, M / 4);
   const int sblocks = (int)((M + 255) / 256), bblocks = prescreen_blocks(gp, M);
@@ -1292,7 +1336,7 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, 
   // the unscreened loop's chunks: whole ones over [0, split), the last over [split, M); only the last can have another k-split
   const int64_t split = ((M - 1) / chunk_cap) * chunk_cap;
   KSplit ks_full, ks_last;
-  if (fast) {
+  if (e == Engine::OZ15) {
     ks_full = oz5_kstar_split(gp, (int)(chunk_cap / nt));
     ks_last = oz5_kstar_split(gp, (int)((M - split + nt - 1) / nt));
   }
@@ -1316,7 +1360,8 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, 
     TB_CUDA(cudaStreamSynchronize(st));
     probe_last = (p == INT64_MAX ? 0 : p) >= split;
   }
-  TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel, isel, 1, probe_last ? &ks_last : &ks_full));
+  const EvalOut none;
+  TB_TRY(eval_chunk(gp, rq, e, xsel, 1, 0, G, none, isel, probe_last ? &ks_last : &ks_full));
   // 3. compaction
   TB_CUDA(cudaMemsetAsync(count, 0, 16, st));
   pre::compact_kernel<<<sblocks, 256, 0, st>>>(rq.Xc, ub, M, split, D, var_ub, rq.acq, gp->sRun.as<double>(), cap, count, xsel, isel);
@@ -1325,459 +1370,111 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, bool fast, int nt, 
   TB_CUDA(cudaMemcpyAsync(n, count, 16, cudaMemcpyDeviceToHost, st));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
-  if (n[0] + n[1] > (unsigned long long)cap) {
-    TB_CUDA(cudaMemcpyAsync(gp->sRun.p, &init_v, 8, cudaMemcpyHostToDevice, st));
-    TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, st));
-    return 0;
-  }
+  if (n[0] + n[1] > (unsigned long long)cap) return argmax_reset(gp);
   // 4. exact evaluation of the survivors: whole-chunk ones in slots [0, n0), last-chunk ones in [cap - n1, cap)
   const int64_t nf = (int64_t)n[0], nb = (int64_t)n[1];
   for (int64_t s0 = 0; s0 < nf; s0 += chunk_cap)
-    TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel + s0 * D, isel + s0, std::min<int64_t>(chunk_cap, nf - s0), &ks_full));
+    TB_TRY(eval_chunk(gp, rq, e, xsel + s0 * D, std::min<int64_t>(chunk_cap, nf - s0), 0, G, none, isel + s0, &ks_full));
   for (int64_t s0 = cap - nb; s0 < cap; s0 += chunk_cap)
-    TB_TRY(argmax_eval_gathered(gp, rq, fast, nt, G, xsel + s0 * D, isel + s0, std::min<int64_t>(chunk_cap, cap - s0), &ks_last));
+    TB_TRY(eval_chunk(gp, rq, e, xsel + s0 * D, std::min<int64_t>(chunk_cap, cap - s0), 0, G, none, isel + s0, &ks_last));
   *done = true;
   return 0;
 }
 
-// Pipelined driver of the int8 engine: K* digit generation of chunk c+1 (fp64 / integer pipes, stream B) overlaps the
-// digit GEMM of chunk c (tensor pipe, stream A); scratch is double-buffered and nothing synchronises with the host until
-// the end of the call.
-static int run_eval_oz(tb_gp* gp, EvalRequest& rq) {
-  TB_CUDA(cudaSetDevice(gp->device));
-  cudaStream_t sa = gp->stream;
-  if (!gp->stream2) {
-    int lo = 0, hi = 0;
-    TB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    TB_CUDA(cudaStreamCreateWithPriority(&gp->stream2, cudaStreamNonBlocking, lo));  // lowest priority
-    for (int i = 0; i < 2; ++i) {
-      TB_CUDA(cudaEventCreateWithFlags(&gp->evK[i], cudaEventDisableTiming));
-      TB_CUDA(cudaEventCreateWithFlags(&gp->evDone[i], cudaEventDisableTiming));
-    }
+// Chunk geometry of run_eval: candidates per tile (nt), candidates per chunk (chunk_cap) and the row-block groups G, fixed
+// for the call when G > 0, else eng_groups of each chunk.  The screened argmax and the k-split of the single-pass engine
+// reproduce these chunks, so they must not drift.
+//   int8 engines, values: K* digit scratch within 1,280 MB, whole pairs of waves (or one wave), at most 8 waves; G of the
+//                         first chunk for the whole call
+//   single-pass engine, gradients: K* digits or V (NB*128 doubles per candidate), whichever is larger, within 1,280 MB,
+//                         whole waves
+//   fp64 engine, and the 21-product engine's gradients: chunk_tiles
+struct ChunkPlan {
+  int nt = BT;
+  int64_t chunk_cap = 0;
+  int G = 0;
+};
+static ChunkPlan plan_chunks(const tb_gp* gp, Engine e, bool grad, int64_t M) {
+  ChunkPlan p;
+  p.nt = eng_tile_width(gp, e);
+  const size_t budget = (size_t)1280 << 20;
+  int64_t max_tiles;
+  if (e != Engine::F64 && !grad) {
+    max_tiles = std::max<int64_t>(1, (int64_t)(budget / eng_tile_bytes(gp, e)));
+    if (max_tiles >= 2 * NUM_SMS) max_tiles = (max_tiles / (2 * NUM_SMS)) * (2 * NUM_SMS);
+    else if (max_tiles >= NUM_SMS) max_tiles = NUM_SMS;
+    max_tiles = std::min<int64_t>(max_tiles, 8 * NUM_SMS);
+  } else if (e == Engine::OZ15) {
+    const size_t v_bytes = (size_t)p.nt * gp->NB * BM * sizeof(double);
+    max_tiles = std::max<int64_t>(1, (int64_t)(budget / std::max(eng_tile_bytes(gp, e), v_bytes)));
+    if (max_tiles >= NUM_SMS) max_tiles = (max_tiles / NUM_SMS) * NUM_SMS;
+  } else {
+    max_tiles = chunk_tiles(gp);
   }
-  // K* generation on a second stream is an experiment switch (TB_OZ_OVERLAP=1): the generation kernel needs >= 8 resident
-  // warps per SM to keep pace, and a resident GEMM CTA leaves room for fewer
-  cudaStream_t sb = std::getenv("TB_OZ_OVERLAP") ? gp->stream2 : sa;
+  p.chunk_cap = std::min<int64_t>(max_tiles * p.nt, ((M + p.nt - 1) / p.nt) * p.nt);
+  if (e != Engine::F64 && !grad) p.G = eng_groups(gp, e, (int)(p.chunk_cap / p.nt));
+  return p;
+}
+
+// The driver behind predict, acquisition values and gradients and the fused argmax: the candidates in chunks (plan_chunks),
+// each through eval_chunk, all on the handle's stream.  Stream order protects the scratch that one chunk reuses from the
+// last, so the host waits once, at the end of the call.
+static int run_eval(tb_gp* gp, EvalRequest& rq) {
+  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_CHECK(rq.M >= 0, "negative candidate count");
+  TB_CUDA(cudaSetDevice(gp->device));
+  cudaStream_t st = gp->stream;
   const int D = gp->D;
+  const bool grad = rq.out_grad != nullptr;
   if (rq.want_argmax) {
     TB_CHECK(rq.M > 0, "argmax over an empty candidate set");
     TB_TRY(gp->sRun.reserve(16));
-    double init_v = -INFINITY;  // a candidate worth -inf still beats "nothing seen" through the lower-index tie rule
-    int64_t init_i = INT64_MAX;
-    TB_CUDA(cudaMemcpyAsync(gp->sRun.p, &init_v, 8, cudaMemcpyHostToDevice, sa));
-    TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, sa));
+    TB_TRY(argmax_reset(gp));
   }
   if (rq.M == 0) return 0;
-  // single-pass engine (15 / 6 digit products) when its a-priori error estimate clears the bar, else the 6-digit kernels
-  TB_TRY(oz5_ensure(gp));
-  const bool fast = gp->oz5_mode != 0;
-  if (!fast) TB_TRY(ensure_ozaki(gp));
-  TB_CUDA(cudaStreamSynchronize(sa));  // digit tiles of Linv are built on stream A; stream B reads model state too
-  const int nt = fast ? oz5_tile_width(gp) : BT;  // candidates per tile
-
-  const bool xc_dev = is_device_ptr(rq.Xc);
-  const bool vals_dev = is_device_ptr(rq.out_vals), mean_dev = is_device_ptr(rq.out_mean), var_dev = is_device_ptr(rq.out_var);
-  // half the usual scratch budget per slot (two slots are live)
-  const size_t per_tile = fast ? oz5_tile_bytes(gp) : (size_t)gp->nst * oz::S * oz::TILE;
-  int64_t max_tiles = std::max<int64_t>(1, (int64_t)(((size_t)1280 << 20) / per_tile));
-  // chunks of whole GEMM rounds (one CTA per SM, G items per tile), in multiples of two rounds
-  if (max_tiles >= 2 * NUM_SMS) max_tiles = (max_tiles / (2 * NUM_SMS)) * (2 * NUM_SMS);
-  else if (max_tiles >= NUM_SMS) max_tiles = NUM_SMS;
-  max_tiles = std::min<int64_t>(max_tiles, 2 * NUM_SMS * 4);
-  if (const char* e = std::getenv("TB_OZ_TILES")) max_tiles = std::max(1, std::atoi(e));  // experiment knob
-  const int64_t chunk_cap = std::min<int64_t>(max_tiles * nt, ((rq.M + nt - 1) / nt) * nt);
-  const int64_t tiles_cap = chunk_cap / nt;
-  // row-block groups per candidate tile: ~4 row-blocks per CTA amortise the CTA prologue while the co-resident CTAs still
-  // share few enough candidate tiles for the K* digits to live in L2; small batches get more groups to fill the GPU
-  int G = std::max(1, (gp->NB + 3) / 4);
-  {
-    const int64_t tiles_all = std::min<int64_t>(tiles_cap, (rq.M + nt - 1) / nt);
-    if (tiles_all * G < 2 * NUM_SMS) G = (int)std::min<int64_t>(gp->NB, (2 * NUM_SMS + tiles_all - 1) / tiles_all);
+  if (grad) TB_CHECK(rq.acq >= 0, "gradients need an acquisition kind");
+  Engine e;
+  TB_TRY(select_engine(gp, grad, &e));
+  const ChunkPlan cp = plan_chunks(gp, e, grad, rq.M);
+  const int64_t chunk_cap = cp.chunk_cap, tiles_cap = chunk_cap / cp.nt;
+  const EvalRoutes dev(rq);
+  TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
+  TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)(cp.G ? cp.G : gp->NB) * chunk_cap));
+  TB_TRY(gp->sMean.reserve(sizeof(double) * chunk_cap));
+  if (!dev.xc) TB_TRY(gp->sXc.reserve(sizeof(double) * chunk_cap * D));
+  if (rq.out_vals && !dev.vals) TB_TRY(gp->sVals.reserve(sizeof(double) * chunk_cap));
+  if (rq.out_var && !dev.var) TB_TRY(gp->sVar.reserve(sizeof(double) * chunk_cap));
+  if (grad) {
+    if (e == Engine::F64) TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));  // packed A
+    TB_TRY(gp->sV.reserve((size_t)chunk_cap * gp->NB * BM * sizeof(double)));
+    TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * chunk_cap));
+    if (!dev.grad) TB_TRY(gp->sGrad.reserve(sizeof(double) * chunk_cap * D));
   }
-  if (const char* e = std::getenv("TB_OZ_G")) G = std::max(1, std::min(std::atoi(e), gp->NB));  // experiment knob
-  tb::DevBuf* ks[2] = {&gp->sKs, &gp->sKs2};
-  tb::DevBuf* mean[2] = {&gp->sMean, &gp->sMean2};
-  tb::DevBuf* part[2] = {&gp->sPartial, &gp->sPartial2};
-  const int nslots = rq.M > chunk_cap ? 2 : 1;
-  for (int i = 0; i < nslots; ++i) {
-    TB_TRY(ks[i]->reserve((size_t)tiles_cap * per_tile));
-    TB_TRY(mean[i]->reserve(sizeof(double) * chunk_cap));
-    TB_TRY(part[i]->reserve(sizeof(double) * (size_t)G * chunk_cap));
-  }
-  // host candidates are staged per slot: the tail of chunk c (stream A) may read them while stream B stages chunk c + 1
-  tb::DevBuf* xs[2] = {&gp->sXc, &gp->sXc2};
-  if (!xc_dev)
-    for (int i = 0; i < nslots; ++i) TB_TRY(xs[i]->reserve(sizeof(double) * chunk_cap * D));
-  if (rq.out_vals && !vals_dev) TB_TRY(gp->sVals.reserve(sizeof(double) * chunk_cap));
-  if (rq.out_var && !var_dev) TB_TRY(gp->sVar.reserve(sizeof(double) * chunk_cap));
-  const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
   if (rq.want_argmax) {
+    const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
     TB_TRY(gp->sBlkBest.reserve(sizeof(double) * tail_blocks_cap));
     TB_TRY(gp->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
   }
 
   bool screened = false;
-  if (argmax_screen_wanted(rq, xc_dev)) TB_TRY(argmax_screened(gp, rq, fast, nt, chunk_cap, G, &screened));
+  if (e != Engine::F64 && argmax_screen_wanted(rq, dev.xc)) TB_TRY(argmax_screened(gp, rq, e, chunk_cap, cp.G, &screened));
   const int64_t m_loop = screened ? 0 : rq.M;  // the screened path has folded its survivors into gp->sRun already
-
-  int64_t c = 0;
-  for (int64_t c0 = 0; c0 < m_loop; c0 += chunk_cap, ++c) {
-    const int slot = (int)(c & 1);
+  for (int64_t c0 = 0; c0 < m_loop; c0 += chunk_cap) {
     const int64_t mc = std::min<int64_t>(chunk_cap, rq.M - c0);
-    const int tiles = (int)((mc + nt - 1) / nt);
-    const int64_t McPad = (int64_t)tiles * nt;
-    // ---- stream B: candidates in, K* digits + mean out ----
-    if (c >= 2) TB_CUDA(cudaStreamWaitEvent(sb, gp->evDone[slot], 0));
-    const double* xc_chunk;
-    if (xc_dev) {
-      xc_chunk = rq.Xc + c0 * D;
-    } else {
-      TB_CUDA(cudaMemcpyAsync(xs[slot]->p, rq.Xc + c0 * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, sb));
-      xc_chunk = xs[slot]->as<double>();
+    const double* xc = rq.Xc + c0 * D;
+    if (!dev.xc) {
+      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, xc, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
+      xc = gp->sXc.as<double>();
     }
-    if (fast) {
-      TB_TRY(oz5_launch_kstar(gp, sb, xc_chunk, mc, tiles, ks[slot]->as<int8_t>(), mean[slot]->as<double>()));
-    } else {
-      cudaStream_t keep = gp->stream;
-      gp->stream = sb;  // launch_kstar_digits launches on gp->stream
-      int rc = launch_kstar_digits(gp, xc_chunk, mc, tiles, ks[slot]->as<int8_t>(), mean[slot]->as<double>());
-      gp->stream = keep;
-      TB_TRY(rc);
-    }
-    TB_CUDA(cudaEventRecord(gp->evK[slot], sb));
-    // ---- stream A: digit GEMM, tail, reductions, results out ----
-    TB_CUDA(cudaStreamWaitEvent(sa, gp->evK[slot], 0));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (gp->profile) {
-      TB_CUDA(cudaEventCreate(&e0));
-      TB_CUDA(cudaEventCreate(&e1));
-      TB_CUDA(cudaEventRecord(e0, sa));
-    }
-    if (fast)
-      TB_TRY(oz5_launch_gemm(gp, sa, ks[slot]->as<int8_t>(), tiles, G, McPad, part[slot]->as<double>()));
-    else
-      TB_TRY(oz::launch_trigemm<oz::OZ_SUMSQ>(sa, tiles, gp->dAS.as<int8_t>(), ks[slot]->as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
-                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 0, part[slot]->as<double>(), nullptr, 0));
-    if (!fast) TB_LAUNCHED();
-    if (gp->profile) {
-      TB_CUDA(cudaEventRecord(e1, sa));
-      gp->prof_events.emplace_back(e0, e1);
-      gp->prof_event_flops.push_back((double)McPad * (double)gp->N * (double)gp->N);
-    }
-    TB_CUDA(cudaGetLastError());
-    double* d_vals = rq.out_vals ? (vals_dev ? rq.out_vals + c0 : gp->sVals.as<double>()) : nullptr;
-    double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;
-    double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
-    const int tb_blocks = (int)((mc + 255) / 256);
-    TB_TRY(launch_tail(gp, sa, rq, part[slot]->as<double>(), G, McPad, mean[slot]->as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk,
-                       nullptr));
-    if (rq.want_argmax) {
-      argmax_fold_kernel<<<1, 256, 0, sa>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks,
-                                            gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
-      TB_LAUNCHED();
-    }
-    if (rq.out_vals && !vals_dev)
-      TB_CUDA(cudaMemcpyAsync(rq.out_vals + c0, gp->sVals.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, sa));
-    if (rq.out_mean && !mean_dev)
-      TB_CUDA(cudaMemcpyAsync(rq.out_mean + c0, mean[slot]->p, sizeof(double) * mc, cudaMemcpyDeviceToHost, sa));
-    if (rq.out_var && !var_dev)
-      TB_CUDA(cudaMemcpyAsync(rq.out_var + c0, gp->sVar.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, sa));
-    TB_CUDA(cudaEventRecord(gp->evDone[slot], sa));
+    const int G = cp.G ? cp.G : eng_groups(gp, e, (int)((mc + cp.nt - 1) / cp.nt));
+    const EvalOut o = dev.chunk(gp, rq, c0);
+    TB_TRY(eval_chunk(gp, rq, e, xc, mc, c0, G, o));
+    TB_TRY(dev.copy_back(gp, rq, c0, mc, o));
   }
-  if (rq.want_argmax) {
-    TB_CUDA(cudaMemcpyAsync(&rq.best_value, gp->sRun.p, 8, cudaMemcpyDeviceToHost, sa));
-    TB_CUDA(cudaMemcpyAsync(&rq.best_index, (char*)gp->sRun.p + 8, 8, cudaMemcpyDeviceToHost, sa));
-  }
-  TB_CUDA(cudaStreamSynchronize(sb));
-  TB_CUDA(cudaStreamSynchronize(sa));
-  TB_CUDA(cudaGetLastError());
-  if (gp->profile) {
-    for (size_t i = 0; i < gp->prof_events.size(); ++i) {
-      float ms = 0.f;
-      TB_CUDA(cudaEventElapsedTime(&ms, gp->prof_events[i].first, gp->prof_events[i].second));
-      gp->prof_ms += ms;
-      gp->prof_flops += gp->prof_event_flops[i];
-      gp->prof_launches += 1;
-      cudaEventDestroy(gp->prof_events[i].first);
-      cudaEventDestroy(gp->prof_events[i].second);
-    }
-    gp->prof_events.clear();
-    gp->prof_event_flops.clear();
-  }
-  return 0;
-}
-
-// Can the joint / gradient paths of this handle run on the single-pass engine (ozaki5.cuh)?  Needs an admitted variance mode;
-// the gradient path also needs the V GEMM's own admission (oz5_ensure_kinv).
-static int oz5_store_ready(tb_gp* gp, bool need_kinv, bool* ok) {
-  *ok = false;
-  if (!(gp->engine == 1 && gp->N <= 16384)) return 0;
-  TB_TRY(oz5_ensure(gp));
-  if (gp->oz5_planes == 0) return 0;
-  if (need_kinv) {
-    TB_TRY(ensure_kinv_dense(gp));
-    TB_TRY(oz5_ensure_kinv(gp));
-    if (!gp->kinv5_ok) return 0;
-  }
-  *ok = true;
-  return 0;
-}
-static inline int oz5_groups(const tb_gp* gp, int tiles) {  // row-block groups per candidate tile: >= 2 items per SM
-  return std::max(std::max(1, (gp->NB + 3) / 4), std::min(gp->NB, (2 * NUM_SMS + tiles - 1) / tiles));
-}
-
-// value + gradient on the single-pass engine: K* digits -> variance GEMM (sum of squares) -> V = K^-1 k* (store GEMM over the
-// same K* digits, dense left factor) -> gradient assembly -> tail
-static int run_eval_grad_oz5(tb_gp* gp, EvalRequest& rq) {
-  TB_CUDA(cudaSetDevice(gp->device));
-  cudaStream_t st = gp->stream;
-  const int D = gp->D;
-  if (rq.want_argmax) {
-    TB_CHECK(rq.M > 0, "argmax over an empty candidate set");
-    TB_TRY(gp->sRun.reserve(16));
-    double init_v = -INFINITY;
-    int64_t init_i = INT64_MAX;
-    TB_CUDA(cudaMemcpyAsync(gp->sRun.p, &init_v, 8, cudaMemcpyHostToDevice, st));
-    TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, st));
-  }
-  if (rq.M == 0) return 0;
-  TB_CHECK(rq.acq >= 0, "gradients need an acquisition kind");
-  const int nt = oz5_tile_width(gp);
-  const size_t per_tile = oz5_tile_bytes(gp);
-  const int64_t ldv = (int64_t)gp->NB * BM;
-  // scratch per chunk: K* digits + V (ldv doubles per candidate): bound both at ~1.3 GB
-  int64_t max_tiles = std::max<int64_t>(1, (int64_t)(((size_t)1280 << 20) / std::max(per_tile, (size_t)nt * ldv * sizeof(double))));
-  if (max_tiles >= NUM_SMS) max_tiles = (max_tiles / NUM_SMS) * NUM_SMS;
-  const int64_t chunk_cap = std::min<int64_t>(max_tiles * nt, ((rq.M + nt - 1) / nt) * nt);
-  const int64_t tiles_cap = chunk_cap / nt;
-  const bool xc_dev = is_device_ptr(rq.Xc);
-  const bool vals_dev = is_device_ptr(rq.out_vals), mean_dev = is_device_ptr(rq.out_mean), var_dev = is_device_ptr(rq.out_var);
-  const bool gdev = is_device_ptr(rq.out_grad);
-  const int Gcap = gp->NB;
-  TB_TRY(gp->sKs.reserve((size_t)tiles_cap * per_tile));
-  TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)Gcap * chunk_cap));
-  TB_TRY(gp->sMean.reserve(sizeof(double) * chunk_cap));
-  TB_TRY(gp->sV.reserve((size_t)chunk_cap * ldv * sizeof(double)));
-  TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * chunk_cap));
-  if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * chunk_cap * D));
-  if (rq.out_vals && !vals_dev) TB_TRY(gp->sVals.reserve(sizeof(double) * chunk_cap));
-  if (rq.out_var && !var_dev) TB_TRY(gp->sVar.reserve(sizeof(double) * chunk_cap));
-  if (!gdev) TB_TRY(gp->sGrad.reserve(sizeof(double) * chunk_cap * D));
-  const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
-  if (rq.want_argmax) {
-    TB_TRY(gp->sBlkBest.reserve(sizeof(double) * tail_blocks_cap));
-    TB_TRY(gp->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
-  }
-  for (int64_t c0 = 0; c0 < rq.M; c0 += chunk_cap) {
-    const int64_t mc = std::min<int64_t>(chunk_cap, rq.M - c0);
-    const int tiles = (int)((mc + nt - 1) / nt);
-    const int64_t McPad = (int64_t)tiles * nt;
-    const int G = oz5_groups(gp, tiles);
-    const double* xc_chunk;
-    if (xc_dev) {
-      xc_chunk = rq.Xc + c0 * D;
-    } else {
-      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, rq.Xc + c0 * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
-      xc_chunk = gp->sXc.as<double>();
-    }
-    TB_TRY(oz5_launch_kstar(gp, st, xc_chunk, mc, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-    TB_TRY(oz5_launch_gemm(gp, st, gp->sKs.as<int8_t>(), tiles, G, McPad, gp->sPartial.as<double>()));
-    TB_TRY(launch_partials(gp, st, rq.acq, rq.param, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), xc_chunk, mc));
-    TB_TRY(oz5_launch_gemm_store(gp, st, 1, gp->sKs.as<int8_t>(), tiles, G, gp->sV.as<double>(), ldv));
-    double* gd = gdev ? rq.out_grad + c0 * D : gp->sGrad.as<double>();
-    switch (gp->kernel) {
-      case TB_RBF: launch_grad_dp<TB_RBF>(gp, xc_chunk, mc, gd); break;
-      case TB_MATERN12: launch_grad_dp<TB_MATERN12>(gp, xc_chunk, mc, gd); break;
-      case TB_MATERN32: launch_grad_dp<TB_MATERN32>(gp, xc_chunk, mc, gd); break;
-      default: launch_grad_dp<TB_MATERN52>(gp, xc_chunk, mc, gd); break;
-    }
-    TB_LAUNCHED();
-    TB_CUDA(cudaGetLastError());
-    double* d_vals = rq.out_vals ? (vals_dev ? rq.out_vals + c0 : gp->sVals.as<double>()) : nullptr;
-    double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;
-    double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
-    const int tb_blocks = (int)((mc + 255) / 256);
-    TB_TRY(launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd));
-    if (!gdev) TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
-    if (rq.want_argmax) {
-      argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks, gp->sRun.as<double>(),
-                                            reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
-      TB_LAUNCHED();
-    }
-    if (rq.out_vals && !vals_dev) TB_CUDA(cudaMemcpyAsync(rq.out_vals + c0, gp->sVals.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (rq.out_mean && !mean_dev) TB_CUDA(cudaMemcpyAsync(rq.out_mean + c0, gp->sMean.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (rq.out_var && !var_dev) TB_CUDA(cudaMemcpyAsync(rq.out_var + c0, gp->sVar.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (!xc_dev || (rq.out_vals && !vals_dev) || (rq.out_mean && !mean_dev) || (rq.out_var && !var_dev) || !gdev)
-      TB_CUDA(cudaStreamSynchronize(st));  // scratch is reused by the next chunk: host-staged copies must drain first
-  }
-  if (rq.want_argmax) {
-    TB_CUDA(cudaMemcpyAsync(&rq.best_value, gp->sRun.p, 8, cudaMemcpyDeviceToHost, st));
-    TB_CUDA(cudaMemcpyAsync(&rq.best_index, (char*)gp->sRun.p + 8, 8, cudaMemcpyDeviceToHost, st));
-  }
+  if (rq.want_argmax) TB_TRY(argmax_read(gp, rq));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
-  return 0;
-}
-
-static int run_eval(tb_gp* gp, EvalRequest& rq) {
-  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_CHECK(rq.M >= 0, "negative candidate count");
-  // int32 accumulators of the int8 engine are exact up to K = 16384; larger models use the native fp64 engine
-  if (gp->engine == 1 && !rq.out_grad && gp->N <= 16384) return run_eval_oz(gp, rq);
-  if (rq.out_grad && rq.acq >= 0) {
-    bool fast = false;
-    TB_CUDA(cudaSetDevice(gp->device));
-    TB_TRY(oz5_store_ready(gp, true, &fast));
-    if (fast) return run_eval_grad_oz5(gp, rq);
-  }
-  TB_CUDA(cudaSetDevice(gp->device));
-  cudaStream_t st = gp->stream;
-  const int D = gp->D;
-  if (rq.want_argmax) {
-    TB_CHECK(rq.M > 0, "argmax over an empty candidate set");
-    TB_TRY(gp->sRun.reserve(16));
-    double init_v = -INFINITY;  // a candidate worth -inf still beats "nothing seen" through the lower-index tie rule
-    int64_t init_i = INT64_MAX;
-    TB_CUDA(cudaMemcpyAsync(gp->sRun.p, &init_v, 8, cudaMemcpyHostToDevice, st));
-    TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, st));
-  }
-  if (rq.M == 0) return 0;
-
-  const bool xc_dev = is_device_ptr(rq.Xc);
-  const bool vals_dev = is_device_ptr(rq.out_vals), mean_dev = is_device_ptr(rq.out_mean),
-             var_dev = is_device_ptr(rq.out_var);
-  const int64_t max_tiles = chunk_tiles(gp);
-  const int64_t Mc_max = max_tiles * BT;
-  const int64_t chunk_cap = std::min<int64_t>(Mc_max, ((rq.M + BT - 1) / BT) * BT);
-  const int64_t tiles_cap = chunk_cap / BT;
-  const int Gmax = gp->NB;  // upper bound of every group choice below
-
-  const bool ozaki = gp->engine == 1 && gp->N <= 16384;  // here: only reached with a gradient request
-  if (ozaki) {
-    TB_TRY(ensure_ozaki(gp));
-    if (rq.out_grad) TB_TRY(ensure_kinv_digits(gp));
-  }
-  TB_TRY(gp->sKs.reserve(std::max((size_t)tiles_cap * gp->nkc * PANEL * sizeof(double),
-                                  (size_t)tiles_cap * gp->nst * oz::S * oz::TILE)));
-  TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)Gmax * chunk_cap));
-  TB_TRY(gp->sMean.reserve(sizeof(double) * chunk_cap));
-  if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * chunk_cap * D));
-  if (rq.out_vals && !vals_dev) TB_TRY(gp->sVals.reserve(sizeof(double) * chunk_cap));
-  if (rq.out_var && !var_dev) TB_TRY(gp->sVar.reserve(sizeof(double) * chunk_cap));
-  if (rq.out_grad) {
-    TB_CHECK(rq.acq >= 0, "gradients need an acquisition kind");
-    if (!ozaki) {
-      TB_TRY(ensure_upper_panels(gp));
-      TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));
-    }
-    TB_TRY(gp->sV.reserve((size_t)chunk_cap * gp->NB * BM * sizeof(double)));
-    TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * chunk_cap));
-    if (!is_device_ptr(rq.out_grad)) TB_TRY(gp->sGrad.reserve(sizeof(double) * chunk_cap * D));
-  }
-  const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
-  if (rq.want_argmax) {
-    TB_TRY(gp->sBlkBest.reserve(sizeof(double) * tail_blocks_cap));
-    TB_TRY(gp->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
-  }
-
-  for (int64_t c0 = 0; c0 < rq.M; c0 += chunk_cap) {
-    const int64_t mc = std::min<int64_t>(chunk_cap, rq.M - c0);
-    const int tiles = (int)((mc + BT - 1) / BT);
-    const int64_t McPad = (int64_t)tiles * BT;
-    // int8 engine: one serpentine PAIR of row-blocks per CTA, so the ~150 co-resident CTAs touch only ~9 candidate tiles
-    // and their K* digit tiles are re-read from L2 instead of HBM (ncu: 28 GB -> ~1 GB of DRAM reads per launch)
-    const int G = ozaki ? std::max(std::max(1, (gp->NB + 3) / 4), std::min(gp->NB, (2 * NUM_SMS + tiles - 1) / tiles)) : pick_groups(gp, tiles);
-
-    const double* xc_chunk;
-    if (xc_dev) {
-      xc_chunk = rq.Xc + c0 * D;
-    } else {
-      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, rq.Xc + c0 * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
-      xc_chunk = gp->sXc.as<double>();
-    }
-    const bool use_oz = ozaki;
-    if (use_oz)
-      TB_TRY(launch_kstar_digits(gp, xc_chunk, mc, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-    else
-      TB_TRY(launch_kstar(gp, xc_chunk, mc, tiles, gp->sKs.as<double>(), gp->sMean.as<double>()));
-
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (gp->profile) {
-      TB_CUDA(cudaEventCreate(&e0));
-      TB_CUDA(cudaEventCreate(&e1));
-      TB_CUDA(cudaEventRecord(e0, st));
-    }
-    if (use_oz)
-      TB_TRY(oz::launch_trigemm<oz::OZ_SUMSQ>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
-                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 0, gp->sPartial.as<double>(), nullptr,
-                                              0));
-    else if (rq.out_grad)
-      trigemm_kernel<false, EPI_SUMSQ_PACKED><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-          gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, gp->sPartial.as<double>(),
-          gp->sA.as<double>(), nullptr, 0);
-    else
-      trigemm_kernel<false, EPI_SUMSQ><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-          gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, gp->sPartial.as<double>(),
-          nullptr, nullptr, 0);
-    TB_LAUNCHED();
-    if (gp->profile) {
-      TB_CUDA(cudaEventRecord(e1, st));
-      gp->prof_events.emplace_back(e0, e1);
-      gp->prof_event_flops.push_back((double)McPad * (double)gp->N * (double)gp->N);
-    }
-    TB_CUDA(cudaGetLastError());
-
-    const bool gdev = rq.out_grad && is_device_ptr(rq.out_grad);
-    double* gd = rq.out_grad ? (gdev ? rq.out_grad + c0 * D : gp->sGrad.as<double>()) : nullptr;
-    if (rq.out_grad) {
-      if (use_oz)
-        TB_TRY(gradient_chunk_oz(gp, rq.acq, rq.param, xc_chunk, mc, tiles, G, McPad, gd));
-      else
-        TB_TRY(gradient_chunk(gp, rq.acq, rq.param, xc_chunk, mc, tiles, G, McPad, gd));
-    }
-
-    double* d_vals = rq.out_vals ? (vals_dev ? rq.out_vals + c0 : gp->sVals.as<double>()) : nullptr;
-    double* d_mean = rq.out_mean ? (mean_dev ? rq.out_mean + c0 : nullptr) : nullptr;  // sMean already holds it
-    double* d_var = rq.out_var ? (var_dev ? rq.out_var + c0 : gp->sVar.as<double>()) : nullptr;
-    const int tb_blocks = (int)((mc + 255) / 256);
-    TB_TRY(launch_tail(gp, st, rq, gp->sPartial.as<double>(), G, McPad, gp->sMean.as<double>(), mc, c0, d_vals, d_mean, d_var, xc_chunk, gd));
-    if (rq.out_grad && !gdev) TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
-    if (rq.want_argmax) {
-      argmax_fold_kernel<<<1, 256, 0, st>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), tb_blocks,
-                                            gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
-      TB_LAUNCHED();
-    }
-    if (rq.out_vals && !vals_dev)
-      TB_CUDA(cudaMemcpyAsync(rq.out_vals + c0, gp->sVals.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (rq.out_mean && !mean_dev)
-      TB_CUDA(cudaMemcpyAsync(rq.out_mean + c0, gp->sMean.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (rq.out_var && !var_dev)
-      TB_CUDA(cudaMemcpyAsync(rq.out_var + c0, gp->sVar.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    // scratch is reused by the next chunk: host-staged copies must drain first
-    if (!xc_dev || (rq.out_vals && !vals_dev) || (rq.out_mean && !mean_dev) || (rq.out_var && !var_dev) ||
-        (rq.out_grad && !is_device_ptr(rq.out_grad)))
-      TB_CUDA(cudaStreamSynchronize(st));
-  }
-  if (rq.want_argmax) {
-    TB_CUDA(cudaMemcpyAsync(&rq.best_value, gp->sRun.p, 8, cudaMemcpyDeviceToHost, st));
-    TB_CUDA(cudaMemcpyAsync(&rq.best_index, (char*)gp->sRun.p + 8, 8, cudaMemcpyDeviceToHost, st));
-  }
-  TB_CUDA(cudaStreamSynchronize(st));
-  TB_CUDA(cudaGetLastError());
-  if (gp->profile) {
-    for (size_t i = 0; i < gp->prof_events.size(); ++i) {
-      float ms = 0.f;
-      TB_CUDA(cudaEventElapsedTime(&ms, gp->prof_events[i].first, gp->prof_events[i].second));
-      gp->prof_ms += ms;
-      gp->prof_flops += gp->prof_event_flops[i];
-      gp->prof_launches += 1;
-      cudaEventDestroy(gp->prof_events[i].first);
-      cudaEventDestroy(gp->prof_events[i].second);
-    }
-    gp->prof_events.clear();
-    gp->prof_event_flops.clear();
-  }
-  return 0;
+  return profile_fold(gp);
 }
 
 // posterior mean and its gradient (no variance, no GEMM, no K^-1): one mean_grad_kernel launch per 65,536 points
@@ -1807,29 +1504,10 @@ static int run_mean_grad(tb_gp* gp, const double* Xc, int64_t M, double* mean, d
     double* md = mean_dev ? mean + c0 : gp->sMean.as<double>();
     double* gd = grad_dev ? grad + c0 * D : gp->sGrad.as<double>();
     const unsigned blocks = (unsigned)((mc + 7) / 8);
-#define TB_MG(KIND, DPV) \
-  mean_grad_kernel<KIND, DPV><<<blocks, 256, 0, st>>>(Xs, al, xc, il, (int)gp->N, D, mc, gp->variance, gp->mean_const, md, gd)
-#define TB_MG_DP(KIND)        \
-  switch (gp->DP) {           \
-    case 2: TB_MG(KIND, 2); break;   \
-    case 4: TB_MG(KIND, 4); break;   \
-    case 6: TB_MG(KIND, 6); break;   \
-    case 8: TB_MG(KIND, 8); break;   \
-    case 10: TB_MG(KIND, 10); break; \
-    case 12: TB_MG(KIND, 12); break; \
-    case 16: TB_MG(KIND, 16); break; \
-    case 20: TB_MG(KIND, 20); break; \
-    case 24: TB_MG(KIND, 24); break; \
-    default: TB_MG(KIND, 32); break; \
-  }
-    switch (gp->kernel) {
-      case TB_RBF: TB_MG_DP(TB_RBF); break;
-      case TB_MATERN12: TB_MG_DP(TB_MATERN12); break;
-      case TB_MATERN32: TB_MG_DP(TB_MATERN32); break;
-      default: TB_MG_DP(TB_MATERN52); break;
-    }
-#undef TB_MG_DP
-#undef TB_MG
+    with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+      mean_grad_kernel<decltype(K)::value, decltype(P)::value><<<blocks, 256, 0, st>>>(Xs, al, xc, il, (int)gp->N, D, mc, gp->variance,
+                                                                                       gp->mean_const, md, gd);
+    });
     TB_LAUNCHED();
     TB_CUDA(cudaGetLastError());
     if (!mean_dev) TB_CUDA(cudaMemcpyAsync(mean + c0, md, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
@@ -1872,24 +1550,14 @@ static int ensure_gibbon(tb_gp* gp) {
   const double* Psd = gp->dGibPs.as<double>();
   const double* Linv = gp->dLinv.as<double>();
   const dim3 cols((unsigned)((N + 127) / 128), (unsigned)m);
-  switch (gp->kernel) {
-    case TB_RBF: gibbon_kxp_kernel<TB_RBF><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
-    case TB_MATERN12: gibbon_kxp_kernel<TB_MATERN12><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
-    case TB_MATERN32: gibbon_kxp_kernel<TB_MATERN32><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
-    default: gibbon_kxp_kernel<TB_MATERN52><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); break;
-  }
+  with_kind(gp->kernel, [&](auto K) { gibbon_kxp_kernel<decltype(K)::value><<<cols, 128, 0, st>>>(Xs, Psd, N, DP, gp->variance, Kxp); });
   TB_LAUNCHED();
   trmv_lower_cols_kernel<<<cols, 128, 0, st>>>(Linv, N, N, Kxp, N, Y, N);
   TB_LAUNCHED();
   trmv_lower_t_cols_kernel<<<dim3((unsigned)((N + 7) / 8), (unsigned)m), 256, 0, st>>>(Linv, N, N, Y, N, W, N);
   TB_LAUNCHED();
   const dim3 pairs((unsigned)m, (unsigned)m);
-  switch (gp->kernel) {
-    case TB_RBF: gibbon_pcov_kernel<TB_RBF><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
-    case TB_MATERN12: gibbon_pcov_kernel<TB_MATERN12><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
-    case TB_MATERN32: gibbon_pcov_kernel<TB_MATERN32><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
-    default: gibbon_pcov_kernel<TB_MATERN52><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); break;
-  }
+  with_kind(gp->kernel, [&](auto K) { gibbon_pcov_kernel<decltype(K)::value><<<pairs, 256, 0, st>>>(Psd, Y, N, DP, m, gp->variance, B); });
   TB_LAUNCHED();
   std::vector<double> b((size_t)m * m);
   TB_CUDA(cudaMemcpyAsync(b.data(), B, sizeof(double) * b.size(), cudaMemcpyDeviceToHost, st));
@@ -2091,11 +1759,12 @@ int tb_gp_set_engine(tb_gp* gp, int engine) {
 int tb_gp_engine_info(tb_gp* gp, int* digit_products, double* error_estimate) {
   TB_CHECK(gp, "tb_gp_engine_info: null handle");
   TB_CHECK(gp->cache_valid, "tb_gp_engine_info: posterior cache is not built");
+  TB_CUDA(cudaSetDevice(gp->device));
+  tb::Engine e;
+  TB_TRY(tb::select_engine(gp, false, &e));
   int products = 0;
   double est = 0.0;
-  if (gp->engine == 1 && gp->N <= 16384) {
-    TB_CUDA(cudaSetDevice(gp->device));
-    TB_TRY(oz5_ensure(gp));
+  if (e != tb::Engine::F64) {
     if (gp->oz5_mode == 5) products = 15;
     else if (gp->oz5_mode == 3) products = 6;
     else products = gp->dtype == TB_F32 ? 10 : 21;
@@ -2222,17 +1891,11 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
   int64_t nbc_cap = std::max<int64_t>(1, (max_tiles * BT) / q);  // whole batches per chunk
   nbc_cap = std::min<int64_t>(nbc_cap, rq.B);
   const int64_t cand_cap = nbc_cap * q;
-  const bool oz_joint = gp->engine == 1 && gp->N <= 16384;
-  bool fast = false;  // single-pass engine (ozaki5.cuh) for A = Linv K*
-  TB_TRY(oz5_store_ready(gp, false, &fast));
-  const int nt = fast ? oz5_tile_width(gp) : BT;  // candidates per tile
+  Engine e;
+  TB_TRY(select_engine(gp, false, &e));
+  const int nt = eng_tile_width(gp, e);  // candidates per tile
   const int64_t tiles_cap = (cand_cap + nt - 1) / nt;
-  if (oz_joint && !fast) {
-    TB_TRY(ensure_ozaki(gp));
-    TB_CUDA(cudaStreamSynchronize(st));
-  }
-  TB_TRY(gp->sKs.reserve(fast ? (size_t)tiles_cap * oz5_tile_bytes(gp)
-                              : std::max((size_t)tiles_cap * gp->nkc * PANEL * sizeof(double), (size_t)tiles_cap * gp->nst * oz::S * oz::TILE)));
+  TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
   TB_TRY(gp->sV.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // A plain
   TB_TRY(gp->sMean.reserve(sizeof(double) * tiles_cap * nt));
   const bool xc_dev = is_device_ptr(rq.Xc);
@@ -2286,7 +1949,6 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
     const int64_t mc = nbc * q;
     const int tiles = (int)((mc + nt - 1) / nt);
     const int64_t McPad = (int64_t)tiles * nt;
-    const int G = pick_groups(gp, tiles);
     const double* xc_chunk;
     if (xc_dev) {
       xc_chunk = rq.Xc + b0 * q * D;
@@ -2294,25 +1956,9 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
       TB_CUDA(cudaMemcpyAsync(gp->sXc.p, rq.Xc + b0 * q * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
       xc_chunk = gp->sXc.as<double>();
     }
-    if (fast) {
-      // A = Linv K* as 15 (fp32 models: 10) exact digit products in one pass, stored for the per-batch Gram kernel
-      TB_TRY(oz5_launch_kstar(gp, st, xc_chunk, mc, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-      TB_TRY(oz5_launch_gemm_store(gp, st, 0, gp->sKs.as<int8_t>(), tiles, oz5_groups(gp, tiles), gp->sV.as<double>(), lda));
-    } else if (oz_joint) {
-      // A = Linv K* on the int8 tensor cores (fp64-accurate digit GEMM), stored for the per-batch Gram kernel
-      TB_TRY(launch_kstar_digits(gp, xc_chunk, mc, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-      const int Goz = std::max(std::max(1, (gp->NB + 3) / 4), std::min(gp->NB, (2 * NUM_SMS + tiles - 1) / tiles));
-      TB_TRY(oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
-                                              gp->nst, Goz, McPad, gp->oz_out_scale, oz_npass(gp), 0, nullptr, gp->sV.as<double>(),
-                                              lda));
-    } else {
-      TB_TRY(launch_kstar(gp, xc_chunk, mc, tiles, gp->sKs.as<double>(), gp->sMean.as<double>()));
-      trigemm_kernel<false, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-          gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, nullptr, nullptr,
-          gp->sV.as<double>(), lda);
-    }
-    TB_LAUNCHED();
-    TB_CUDA(cudaGetLastError());
+    // A = Linv K*, stored plain for the per-batch Gram kernel
+    TB_TRY(eng_kstar(gp, e, xc_chunk, mc, tiles));
+    TB_TRY(eng_store_a(gp, e, tiles, McPad, gp->sV.as<double>()));
     double* dptr[4];
     for (int i = 0; i < 4; ++i) {
       Out& o = outs[i];
@@ -2324,12 +1970,10 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
     double* om = bei ? bmu.as<double>() : dptr[0];
     double* oc = bei ? bcov.as<double>() : dptr[1];
     double* oq = bei ? nullptr : dptr[3];
-    switch (gp->kernel) {
-      case TB_RBF: TB_TRY(launch_joint<TB_RBF>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
-      case TB_MATERN12: TB_TRY(launch_joint<TB_MATERN12>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
-      case TB_MATERN32: TB_TRY(launch_joint<TB_MATERN32>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
-      default: TB_TRY(launch_joint<TB_MATERN52>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, eps_dev, om, oc, dptr[2], oq, err)); break;
-    }
+    TB_TRY(with_kind(gp->kernel, [&](auto K) {
+      return launch_joint<decltype(K)::value>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc,
+                                              jr, eps_dev, om, oc, dptr[2], oq, err);
+    }));
     if (bei) {
       bei_kernel<<<(unsigned)nbc, bei_warps * 32, smem_bei, st>>>(om, oc, q, eps_dev, rq.S, rq.eta, dptr[3], err);
       TB_LAUNCHED();
@@ -2353,38 +1997,16 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
 // A = Linv K(X, Xc) for M device-resident points, stored plain ([point][lda], lda = NB*128) in gp->sA; posterior means in
 // gp->sMean.  One launch over all M points (callers bound M).
 static int compute_a_plain(tb_gp* gp, const double* xc_dev, int64_t M) {
-  cudaStream_t st = gp->stream;
-  const int64_t lda = (int64_t)gp->NB * BM;
-  const bool oz_path = gp->engine == 1 && gp->N <= 16384;
-  bool fast = false;
-  TB_TRY(oz5_store_ready(gp, false, &fast));
-  const int nt = fast ? oz5_tile_width(gp) : BT;
+  Engine e;
+  TB_TRY(select_engine(gp, false, &e));
+  const int nt = eng_tile_width(gp, e);
   const int tiles = (int)((M + nt - 1) / nt);
   const int64_t McPad = (int64_t)tiles * nt;
-  if (oz_path && !fast) TB_TRY(ensure_ozaki(gp));
-  TB_TRY(gp->sKs.reserve(fast ? (size_t)tiles * oz5_tile_bytes(gp)
-                              : std::max((size_t)tiles * gp->nkc * PANEL * sizeof(double), (size_t)tiles * gp->nst * oz::S * oz::TILE)));
-  TB_TRY(gp->sA.reserve((size_t)McPad * lda * sizeof(double)));
+  TB_TRY(gp->sKs.reserve((size_t)tiles * eng_tile_bytes(gp, e)));
+  TB_TRY(gp->sA.reserve((size_t)McPad * gp->NB * BM * sizeof(double)));
   TB_TRY(gp->sMean.reserve(sizeof(double) * McPad));
-  if (fast) {
-    TB_TRY(oz5_launch_kstar(gp, st, xc_dev, M, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-    TB_TRY(oz5_launch_gemm_store(gp, st, 0, gp->sKs.as<int8_t>(), tiles, oz5_groups(gp, tiles), gp->sA.as<double>(), lda));
-    return 0;
-  }
-  if (oz_path) {
-    TB_TRY(launch_kstar_digits(gp, xc_dev, M, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-    const int Goz = std::max(std::max(1, (gp->NB + 3) / 4), std::min(gp->NB, (2 * NUM_SMS + tiles - 1) / tiles));
-    TB_TRY(oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
-                                            gp->nst, Goz, McPad, gp->oz_out_scale, oz_npass(gp), 0, nullptr, gp->sA.as<double>(), lda));
-  } else {
-    const int G = pick_groups(gp, tiles);
-    TB_TRY(launch_kstar(gp, xc_dev, M, tiles, gp->sKs.as<double>(), gp->sMean.as<double>()));
-    trigemm_kernel<false, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-        gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, nullptr, nullptr, gp->sA.as<double>(), lda);
-  }
-  TB_LAUNCHED();
-  TB_CUDA(cudaGetLastError());
-  return 0;
+  TB_TRY(eng_kstar(gp, e, xc_dev, M, tiles));
+  return eng_store_a(gp, e, tiles, McPad, gp->sA.as<double>());
 }
 
 // out[i][j] = k(x1_i, x2_j) - sum_k A1[i][k] A2[j][k]: posterior covariance between two point sets, row-major [M1, M2]
@@ -2440,16 +2062,12 @@ static int run_cross_cov(tb_gp* gp, const double* X1, int64_t M1, const double* 
   const double* x2 = x1 + M1 * D;
   const double* il = gp->dInvLs.as<double>();
   const dim3 grid((unsigned)((M2 + fac::FB - 1) / fac::FB), (unsigned)((M1 + fac::FB - 1) / fac::FB));
-#define TB_CCOV(KIND)                                                                                                        \
-  TB_CUDA(cudaFuncSetAttribute(cross_cov_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fac::GEMM_SMEM)); \
-  cross_cov_kernel<KIND><<<grid, fac::THREADS, fac::GEMM_SMEM, st>>>(A1, A2, lda, (int)lda, x1, x2, il, D, M1, M2, gp->variance, od)
-  switch (gp->kernel) {
-    case TB_RBF: TB_CCOV(TB_RBF); break;
-    case TB_MATERN12: TB_CCOV(TB_MATERN12); break;
-    case TB_MATERN32: TB_CCOV(TB_MATERN32); break;
-    default: TB_CCOV(TB_MATERN52); break;
-  }
-#undef TB_CCOV
+  TB_TRY(with_kind(gp->kernel, [&](auto K) {
+    constexpr int KIND = decltype(K)::value;
+    TB_CUDA(cudaFuncSetAttribute(cross_cov_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fac::GEMM_SMEM));
+    cross_cov_kernel<KIND><<<grid, fac::THREADS, fac::GEMM_SMEM, st>>>(A1, A2, lda, (int)lda, x1, x2, il, D, M1, M2, gp->variance, od);
+    return 0;
+  }));
   TB_LAUNCHED();
   if (!out_dev) TB_CUDA(cudaMemcpyAsync(out, od, sizeof(double) * (size_t)M1 * M2, cudaMemcpyDeviceToHost, st));
   TB_CUDA(cudaStreamSynchronize(st));
@@ -2525,16 +2143,12 @@ static int run_sample_joint(tb_gp* gp, const double* Xc, int64_t M, const double
     const double* A = gp->sA.as<double>();
     const double* il = gp->dInvLs.as<double>();
     double* cov = bcov.as<double>();
-#define TB_PCOV(KIND)                                                                                                            \
-  TB_CUDA(cudaFuncSetAttribute(posterior_cov_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fac::GEMM_SMEM)); \
-  posterior_cov_kernel<KIND><<<dim3(t, t), fac::THREADS, fac::GEMM_SMEM, st>>>(A, lda, (int)lda, xc, il, D, M, gp->variance, jitter, cov)
-    switch (gp->kernel) {
-      case TB_RBF: TB_PCOV(TB_RBF); break;
-      case TB_MATERN12: TB_PCOV(TB_MATERN12); break;
-      case TB_MATERN32: TB_PCOV(TB_MATERN32); break;
-      default: TB_PCOV(TB_MATERN52); break;
-    }
-#undef TB_PCOV
+    TB_TRY(with_kind(gp->kernel, [&](auto K) {
+      constexpr int KIND = decltype(K)::value;
+      TB_CUDA(cudaFuncSetAttribute(posterior_cov_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fac::GEMM_SMEM));
+      posterior_cov_kernel<KIND><<<dim3(t, t), fac::THREADS, fac::GEMM_SMEM, st>>>(A, lda, (int)lda, xc, il, D, M, gp->variance, jitter, cov);
+      return 0;
+    }));
     TB_LAUNCHED();
   }
   // blocked Cholesky of the covariance with the cache-build kernels (factor.cuh)
@@ -2594,10 +2208,14 @@ static int run_sample_joint(tb_gp* gp, const double* Xc, int64_t M, const double
 // -> grad_kernel (the training-point sums) -> qei_cross_kernel (the K(x_b, x_b) term).  Tails:
 //   QEI_TAIL_MC   qei_backward_kernel: batch Monte-Carlo EI (function.py:1181-1186), eps [q, S] normal base samples
 //   QEI_TAIL_GENZ bei_backward_kernel: batch EI (function.py:1747-1805), eps = the Sobol points w [q-1, S]
-template <int KIND>
-static void launch_qei_cross(tb_gp* gp, const double* xc, int64_t npts, int q, const double* sbar, double* grad) {
-  qei_cross_kernel<KIND><<<(unsigned)((npts + 127) / 128), 128, 0, gp->stream>>>(xc, gp->dInvLs.as<double>(), gp->D, npts, q, sbar,
-                                                                                 gp->variance, grad);
+static int launch_qei_cross(tb_gp* gp, const double* xc, int64_t npts, int q, const double* sbar, double* grad) {
+  with_kind(gp->kernel, [&](auto K) {
+    qei_cross_kernel<decltype(K)::value><<<(unsigned)((npts + 127) / 128), 128, 0, gp->stream>>>(xc, gp->dInvLs.as<double>(), gp->D, npts,
+                                                                                                 q, sbar, gp->variance, grad);
+  });
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 enum { QEI_TAIL_MC = 0, QEI_TAIL_GENZ = 1 };
@@ -2612,22 +2230,14 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
   TB_CHECK(S >= 1 && eps, "need S >= 1 base samples");
   TB_CHECK(jitter >= 0.0, "jitter must be non-negative");
   if (B == 0) return 0;
-  const bool oz_path = gp->engine == 1 && gp->N <= 16384;  // else: native fp64 DMMA kernels
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
   const int D = gp->D;
   const int QT = (q + 7) / 8, QP = QT * 8;
   const int64_t lda = (int64_t)gp->NB * BM;
-  bool fast = false;  // single-pass engine for both store GEMMs (A = Linv K*, V = K^-1 K*)
-  if (oz_path) TB_TRY(oz5_store_ready(gp, true, &fast));
-  const int nt = fast ? oz5_tile_width(gp) : BT;
-  if (fast) {
-  } else if (oz_path) {
-    TB_TRY(ensure_ozaki(gp));
-    TB_TRY(ensure_kinv_digits(gp));
-  } else {
-    TB_TRY(ensure_upper_panels(gp));
-  }
+  Engine e;
+  TB_TRY(select_engine(gp, true, &e));
+  const int nt = eng_tile_width(gp, e);
   const int64_t max_tiles = chunk_tiles(gp);
   int64_t nbc_cap = std::min<int64_t>(std::max<int64_t>(1, (max_tiles * BT) / q), B);
   const int64_t cand_cap = nbc_cap * q;
@@ -2637,11 +2247,10 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
     tb::DevBuf* b;
     ~ReleaseA() { b->release(); }
   } rel_a{&baplain};
-  if (oz_path) {
-    TB_TRY(gp->sKs.reserve(fast ? (size_t)tiles_cap * oz5_tile_bytes(gp) : (size_t)tiles_cap * gp->nst * oz::S * oz::TILE));
+  TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
+  if (e != Engine::F64) {
     TB_TRY(gp->sA.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // A plain
   } else {
-    TB_TRY(gp->sKs.reserve((size_t)tiles_cap * gp->nkc * PANEL * sizeof(double)));
     TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));  // A packed
     TB_TRY(baplain.reserve((size_t)tiles_cap * BT * lda * sizeof(double)));
     TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)gp->NB * tiles_cap * BT));
@@ -2699,54 +2308,20 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
       TB_CUDA(cudaMemcpyAsync(gp->sXc.p, Xc + b0 * q * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
       xc_chunk = gp->sXc.as<double>();
     }
-    const double* a_plain;
-    if (fast) {
-      TB_TRY(oz5_launch_kstar(gp, st, xc_chunk, mc, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-      const int Gs = oz5_groups(gp, tiles);
-      TB_TRY(oz5_launch_gemm_store(gp, st, 0, gp->sKs.as<int8_t>(), tiles, Gs, gp->sA.as<double>(), lda));
-      TB_TRY(oz5_launch_gemm_store(gp, st, 1, gp->sKs.as<int8_t>(), tiles, Gs, gp->sV.as<double>(), lda));
-      a_plain = gp->sA.as<double>();
-    } else if (oz_path) {
-      TB_TRY(launch_kstar_digits(gp, xc_chunk, mc, tiles, gp->sKs.as<int8_t>(), gp->sMean.as<double>()));
-      const int Goz = std::max(std::max(1, (gp->NB + 3) / 4), std::min(gp->NB, (2 * NUM_SMS + tiles - 1) / tiles));
-      TB_TRY(oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
-                                              gp->nst, Goz, McPad, gp->oz_out_scale, oz_npass(gp), 0, nullptr, gp->sA.as<double>(),
-                                              lda));
-      TB_LAUNCHED();
-      const int Gv = std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)));
-      TB_TRY(oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dKinvS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dKinvScale.as<double>(),
-                                              gp->NB, gp->nst, Gv, McPad, gp->oz_out_scale, oz_npass(gp), 1, nullptr,
-                                              gp->sV.as<double>(), lda));
-      TB_LAUNCHED();
-      a_plain = gp->sA.as<double>();
-    } else {
-      // native fp64 engine: A twice (plain for the Gram kernel, packed panels for the upper GEMM), then V = Linv^T A
-      const int G = pick_groups(gp, tiles);
-      TB_TRY(launch_kstar(gp, xc_chunk, mc, tiles, gp->sKs.as<double>(), gp->sMean.as<double>()));
-      trigemm_kernel<false, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-          gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, nullptr, nullptr, baplain.as<double>(), lda);
-      TB_LAUNCHED();
-      trigemm_kernel<false, EPI_SUMSQ_PACKED><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-          gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, gp->sPartial.as<double>(), gp->sA.as<double>(),
-          nullptr, 0);
-      TB_LAUNCHED();
-      const int nkB = gp->NB * (BM / BK);
-      trigemm_kernel<true, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-          gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB, nkB, G, McPad, nullptr, nullptr, gp->sV.as<double>(), lda);
-      TB_LAUNCHED();
-      a_plain = baplain.as<double>();
-    }
-    TB_CUDA(cudaGetLastError());
+    // fp64 engine: A twice (plain for the Gram kernel, packed panels for its V GEMM); int8 engines: A plain in sA
+    double* a_plain = e == Engine::F64 ? baplain.as<double>() : gp->sA.as<double>();
+    TB_TRY(eng_kstar(gp, e, xc_chunk, mc, tiles));
+    TB_TRY(eng_store_a(gp, e, tiles, McPad, a_plain));
+    if (e == Engine::F64) TB_TRY(eng_variance(gp, e, tiles, eng_groups(gp, e, tiles), McPad, true));
+    TB_TRY(eng_store_v(gp, e, tiles, McPad));
     const int jblocks = (int)((nbc + JOINT_WARPS - 1) / JOINT_WARPS);
     const int Nrows = (int)lda;
     double* dmu = bmu.as<double>();
     double* dcov = bcov.as<double>();
-    switch (gp->kernel) {
-      case TB_RBF: TB_TRY(launch_joint<TB_RBF>(gp, QT, jblocks, smem_joint, a_plain, lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, nullptr, dmu, dcov, nullptr, nullptr, err)); break;
-      case TB_MATERN12: TB_TRY(launch_joint<TB_MATERN12>(gp, QT, jblocks, smem_joint, a_plain, lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, nullptr, dmu, dcov, nullptr, nullptr, err)); break;
-      case TB_MATERN32: TB_TRY(launch_joint<TB_MATERN32>(gp, QT, jblocks, smem_joint, a_plain, lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, nullptr, dmu, dcov, nullptr, nullptr, err)); break;
-      default: TB_TRY(launch_joint<TB_MATERN52>(gp, QT, jblocks, smem_joint, a_plain, lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr, nullptr, dmu, dcov, nullptr, nullptr, err)); break;
-    }
+    TB_TRY(with_kind(gp->kernel, [&](auto K) {
+      return launch_joint<decltype(K)::value>(gp, QT, jblocks, smem_joint, a_plain, lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr,
+                                              nullptr, dmu, dcov, nullptr, nullptr, err);
+    }));
     double* cmu = gp->sMisc.as<double>();
     double* dval = val_dev ? out_val + b0 : bval.as<double>();
     if (genz) {
@@ -2761,21 +2336,8 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
                                                                                         bsbar.as<double>());
     TB_LAUNCHED();
     double* gd = grad_dev ? out_grad + b0 * q * D : gp->sGrad.as<double>();
-    switch (gp->kernel) {
-      case TB_RBF: launch_grad_dp<TB_RBF>(gp, xc_chunk, mc, gd); break;
-      case TB_MATERN12: launch_grad_dp<TB_MATERN12>(gp, xc_chunk, mc, gd); break;
-      case TB_MATERN32: launch_grad_dp<TB_MATERN32>(gp, xc_chunk, mc, gd); break;
-      default: launch_grad_dp<TB_MATERN52>(gp, xc_chunk, mc, gd); break;
-    }
-    TB_LAUNCHED();
-    switch (gp->kernel) {
-      case TB_RBF: launch_qei_cross<TB_RBF>(gp, xc_chunk, mc, q, bsbar.as<double>(), gd); break;
-      case TB_MATERN12: launch_qei_cross<TB_MATERN12>(gp, xc_chunk, mc, q, bsbar.as<double>(), gd); break;
-      case TB_MATERN32: launch_qei_cross<TB_MATERN32>(gp, xc_chunk, mc, q, bsbar.as<double>(), gd); break;
-      default: launch_qei_cross<TB_MATERN52>(gp, xc_chunk, mc, q, bsbar.as<double>(), gd); break;
-    }
-    TB_LAUNCHED();
-    TB_CUDA(cudaGetLastError());
+    TB_TRY(launch_grad(gp, xc_chunk, mc, gd));
+    TB_TRY(launch_qei_cross(gp, xc_chunk, mc, q, bsbar.as<double>(), gd));
     if (!val_dev) TB_CUDA(cudaMemcpyAsync(out_val + b0, bval.p, sizeof(double) * nbc, cudaMemcpyDeviceToHost, st));
     if (!grad_dev) TB_CUDA(cudaMemcpyAsync(out_grad + b0 * q * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
     if (!xc_dev || !val_dev || !grad_dev) TB_CUDA(cudaStreamSynchronize(st));
@@ -3018,28 +2580,8 @@ static void launch_kdot_nbt(tb_rff* r, const double* xc, int64_t mc, double* out
     TB_LAUNCHED();
   }
 }
-template <int KIND>
-static void launch_kdot_dp(tb_rff* r, const double* xc, int64_t mc, double* out) {
-  switch (r->DP) {
-    case 2: launch_kdot_nbt<KIND, 2>(r, xc, mc, out); break;
-    case 4: launch_kdot_nbt<KIND, 4>(r, xc, mc, out); break;
-    case 6: launch_kdot_nbt<KIND, 6>(r, xc, mc, out); break;
-    case 8: launch_kdot_nbt<KIND, 8>(r, xc, mc, out); break;
-    case 10: launch_kdot_nbt<KIND, 10>(r, xc, mc, out); break;
-    case 12: launch_kdot_nbt<KIND, 12>(r, xc, mc, out); break;
-    case 16: launch_kdot_nbt<KIND, 16>(r, xc, mc, out); break;
-    case 20: launch_kdot_nbt<KIND, 20>(r, xc, mc, out); break;
-    case 24: launch_kdot_nbt<KIND, 24>(r, xc, mc, out); break;
-    default: launch_kdot_nbt<KIND, 32>(r, xc, mc, out); break;
-  }
-}
 static int launch_kdot(tb_rff* r, const double* xc, int64_t mc, double* out) {
-  switch (r->kernel) {
-    case TB_RBF: launch_kdot_dp<TB_RBF>(r, xc, mc, out); break;
-    case TB_MATERN12: launch_kdot_dp<TB_MATERN12>(r, xc, mc, out); break;
-    case TB_MATERN32: launch_kdot_dp<TB_MATERN32>(r, xc, mc, out); break;
-    default: launch_kdot_dp<TB_MATERN52>(r, xc, mc, out); break;
-  }
+  with_kind_dp(r->kernel, r->DP, [&](auto K, auto P) { launch_kdot_nbt<decltype(K)::value, decltype(P)::value>(r, xc, mc, out); });
   TB_CUDA(cudaGetLastError());
   return 0;
 }
@@ -3126,20 +2668,7 @@ int tb_rff_eval(tb_rff* r, const void* Xc, int64_t M, void* out, double* min_val
       nbt = rem >= 5 ? 8 : rem >= 3 ? 4 : rem;  // trajectories per pass: the cosine of a feature is shared by all of them
       double* bb = want_min ? r->sBlkBest.as<double>() : nullptr;
       int64_t* bi = want_min ? r->sBlkIdx.as<int64_t>() : nullptr;
-#define TB_RFF_DP(DPV) TB_TRY((tb::launch_rff<DPV>(r, nbt, blocks, xc, b0, mc, c0, scale, addend, od, bb, bi)))
-      switch (r->DP) {
-        case 2: TB_RFF_DP(2); break;
-        case 4: TB_RFF_DP(4); break;
-        case 6: TB_RFF_DP(6); break;
-        case 8: TB_RFF_DP(8); break;
-        case 10: TB_RFF_DP(10); break;
-        case 12: TB_RFF_DP(12); break;
-        case 16: TB_RFF_DP(16); break;
-        case 20: TB_RFF_DP(20); break;
-        case 24: TB_RFF_DP(24); break;
-        default: TB_RFF_DP(32); break;
-      }
-#undef TB_RFF_DP
+      TB_TRY(tb::with_dp(r->DP, [&](auto P) { return tb::launch_rff<decltype(P)::value>(r, nbt, blocks, xc, b0, mc, c0, scale, addend, od, bb, bi); }));
     }
     if (want_min) {
       // blk arrays are laid out [nb][blocks of this launch]
