@@ -13,9 +13,27 @@
 
 namespace tb {
 
+// A device allocation that grows on demand and is freed with its owner.  None may have static storage duration: its cudaFree
+// would run after the CUDA runtime has been torn down at process exit.
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) {
+    o.p = nullptr;
+    o.cap = 0;
+  }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) {
+      release();
+      std::swap(p, o.p);
+      std::swap(cap, o.cap);
+    }
+    return *this;
+  }
+  ~DevBuf() { release(); }
   int reserve(size_t bytes) {
     if (bytes <= cap) return 0;
     if (p) cudaFree(p);
@@ -43,6 +61,41 @@ inline bool is_device_ptr(const void* p) {
   }
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
+
+// A caller's array of items of `width` elements each, on the device or on the host.  A device array is read and written in
+// place; a host array goes through `scratch` one chunk of items at a time.  Every copy goes on the call's stream `st`, and
+// the host waits once, at the end of the call: a copy from pageable memory to the device has consumed its source when it
+// returns, a copy from the device to pageable memory returns only once it has completed, and each copy is ordered with the
+// kernels on `st`, so stream order protects the scratch that the next chunk reuses.  (Pinned host arrays are read and
+// written by the stream alone until that final wait.)
+template <class T>
+struct Staged {
+  T* user;
+  int64_t width;
+  DevBuf* scratch;
+  cudaStream_t st;
+  bool dev;
+  Staged(T* user, int64_t width, DevBuf& scratch, cudaStream_t st)
+      : user(user), width(width), scratch(&scratch), st(st), dev(is_device_ptr(user)) {}
+  bool host() const { return user && !dev; }
+  int reserve(int64_t n) const { return host() ? scratch->reserve(sizeof(T) * width * n) : 0; }
+  // items [c0, c0 + n) of an input, on the device (null for a null array)
+  int in(int64_t c0, int64_t n, T** d) const {
+    if (!host()) {
+      *d = user ? user + c0 * width : nullptr;
+      return 0;
+    }
+    TB_CUDA(cudaMemcpyAsync(scratch->p, user + c0 * width, sizeof(T) * width * n, cudaMemcpyHostToDevice, st));
+    *d = scratch->as<T>();
+    return 0;
+  }
+  // where the items of an output from c0 on are written (null for a null array); back() brings a host array's home
+  T* out(int64_t c0) const { return host() ? scratch->as<T>() : user ? user + c0 * width : nullptr; }
+  int back(int64_t c0, int64_t n) const {
+    if (host()) TB_CUDA(cudaMemcpyAsync(user + c0 * width, scratch->p, sizeof(T) * width * n, cudaMemcpyDeviceToHost, st));
+    return 0;
+  }
+};
 
 // supported padded input dimensions of the distance loop (even, so rows load as double2), ascending
 template <int... V>

@@ -221,6 +221,88 @@ __global__ void colmajor_lower_to_rowmajor_kernel(const double* __restrict__ A, 
   if (i < N) out[i * N + j] = (j <= i) ? A[i + j * N] : 0.0;
 }
 
+// =================================================================================================
+// dtype bridge.  TB_F32 handles (fp32 models, e.g. BASELINE config 5) take and return float arrays: whole inputs are widened
+// to device doubles and outputs narrowed back.  Their posterior cache is fp64.  select_engine runs their candidate GEMMs on
+// the int8 engines with fewer digits than an fp64 handle gets: the single-pass engine with the fewest digits oz5_ensure
+// admits (3 digits / 6 products, 4 / 10 or 5 / 15), else the leading pass (10 products) of the 21-product engine.
+// Above N = 16384 and on engine 0 they run the fp64 DMMA kernels, as fp64 handles do.
+// =================================================================================================
+__global__ void widen_kernel(const float* __restrict__ in, int64_t n, double* __restrict__ out) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = (double)in[i];
+}
+__global__ void narrow_kernel(const double* __restrict__ in, int64_t n, float* __restrict__ out) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = (float)in[i];
+}
+
+// The arrays of one call in the handle's dtype, as device doubles.  TB_F64 handles: the caller's pointers, with no CUDA call.
+// TB_F32 handles: one device buffer per staged array, one widen / narrow launch per array, and finish() waits once.
+struct DtypeBridge {
+  tb_gp* gp;
+  bool f32;
+  std::vector<DevBuf> allocs;
+  struct Pending { double* dev; void* user; int64_t n; };
+  std::vector<Pending> outs;
+  explicit DtypeBridge(tb_gp* g) : gp(g), f32(g->dtype == TB_F32) {}
+  int alloc(void** p, size_t bytes) {
+    if (allocs.empty()) TB_CUDA(cudaSetDevice(gp->device));
+    allocs.emplace_back();
+    TB_TRY(allocs.back().reserve(std::max<size_t>(bytes, 16)));
+    *p = allocs.back().p;
+    return 0;
+  }
+  int in(const void* user, int64_t n, const double** out) {  // float (host or device) -> device double
+    *out = (const double*)user;
+    if (!f32) return 0;
+    *out = nullptr;
+    if (!user || n == 0) return 0;
+    const float* src = (const float*)user;
+    if (!is_device_ptr(user)) {
+      void* tmp;
+      TB_TRY(alloc(&tmp, sizeof(float) * n));
+      TB_CUDA(cudaMemcpyAsync(tmp, user, sizeof(float) * n, cudaMemcpyHostToDevice, gp->stream));
+      src = (const float*)tmp;
+    }
+    void* d;
+    TB_TRY(alloc(&d, sizeof(double) * n));
+    widen_kernel<<<(unsigned)((n + 255) / 256), 256, 0, gp->stream>>>(src, n, (double*)d);
+    TB_LAUNCHED();
+    *out = (const double*)d;
+    return 0;
+  }
+  int out(void* user, int64_t n, double** dev) {  // device double scratch, narrowed into `user` by finish()
+    *dev = (double*)user;
+    if (!f32) return 0;
+    *dev = nullptr;
+    if (!user || n == 0) return 0;
+    void* d;
+    TB_TRY(alloc(&d, sizeof(double) * n));
+    *dev = (double*)d;
+    outs.push_back({(double*)d, user, n});
+    return 0;
+  }
+  int finish() {
+    if (!f32) return 0;
+    for (auto& o : outs) {
+      float* dst = (float*)o.user;
+      void* tmp = nullptr;
+      const bool dev = is_device_ptr(o.user);
+      if (!dev) {
+        TB_TRY(alloc(&tmp, sizeof(float) * o.n));
+        dst = (float*)tmp;
+      }
+      narrow_kernel<<<(unsigned)((o.n + 255) / 256), 256, 0, gp->stream>>>(o.dev, o.n, dst);
+      TB_LAUNCHED();
+      if (!dev) TB_CUDA(cudaMemcpyAsync(o.user, tmp, sizeof(float) * o.n, cudaMemcpyDeviceToHost, gp->stream));
+    }
+    TB_CUDA(cudaStreamSynchronize(gp->stream));
+    TB_CUDA(cudaGetLastError());
+    return 0;
+  }
+};
+
 }  // namespace tb
 
 #define TB_CUSOLVER(expr)                                                                          \
@@ -287,14 +369,6 @@ int tb_gp_destroy(tb_gp* gp) {
   if (!gp) return 0;
   cudaSetDevice(gp->device);
   cudaStreamSynchronize(gp->stream);
-  for (tb::DevBuf* b : {&gp->dX, &gp->dy, &gp->dXs, &gp->dInvLs, &gp->dAlpha, &gp->dL, &gp->dLinv,
-                        &gp->dLinvP, &gp->dLinvTP, &gp->dAS, &gp->dRowScale, &gp->dKinv, &gp->dKinvS, &gp->dKinvScale, &gp->dDinv, &gp->dWork, &gp->dInfo, &gp->sKs, &gp->sPartial, &gp->sMean,
-                        &gp->sVals, &gp->sVar, &gp->sXc, &gp->sBlkBest, &gp->sBlkIdx, &gp->sRun,
-                        &gp->sA, &gp->sV, &gp->sGrad, &gp->sMisc, &gp->dMes, &gp->dXspare, &gp->dyspare, &gp->dLspare, &gp->dLinvSpare,
-                        &gp->dAS5, &gp->dRowScale5, &gp->dRowSum5, &gp->dX2, &gp->dKinvS5, &gp->dKinvScale5, &gp->dKinvSum5,
-                        &gp->dKinvSpare, &gp->sMeanPart, &gp->dPen, &gp->dGibPs, &gp->dGibLinv, &gp->dGibWhat,
-                        &gp->sGib, &gp->sScrUb, &gp->sScrX, &gp->sScrIdx, &gp->sScrBlk, &gp->dPreRows, &gp->dPreCentre})
-    b->release();
   for (auto& ev : gp->prof_events) {
     cudaEventDestroy(ev.first);
     cudaEventDestroy(ev.second);
@@ -302,15 +376,19 @@ int tb_gp_destroy(tb_gp* gp) {
   if (gp->cusolver) cusolverDnDestroy(gp->cusolver);
   if (gp->cublas) cublasDestroy(gp->cublas);
   if (gp->stream) cudaStreamDestroy(gp->stream);
-  delete gp;
+  delete gp;  // frees the device buffers
   return 0;
 }
 
-static int tb_gp_set_data_f64(tb_gp* gp, const void* X, const void* y, int64_t N, int D) {
-  TB_CHECK(gp && X && y, "tb_gp_set_data: null argument");
+int tb_gp_set_data(tb_gp* gp, const void* X_in, const void* y_in, int64_t N, int D) {
+  TB_CHECK(gp && X_in && y_in, "tb_gp_set_data: null argument");
   TB_CHECK(N > 0, "tb_gp_set_data: dataset must be populated (N > 0)");
   TB_CHECK(D > 0 && tb::pick_dp(D) > 0, "tb_gp_set_data: input dimension must be in [1, 32]");
   TB_CHECK(N <= 65535, "tb_gp_set_data: N > 65535 is not supported");  // grid.y of the per-column kernels
+  tb::DtypeBridge br(gp);
+  const double *X, *y;
+  TB_TRY(br.in(X_in, N * D, &X));
+  TB_TRY(br.in(y_in, N, &y));
   TB_CUDA(cudaSetDevice(gp->device));
   gp->N = N;
   gp->D = D;
@@ -538,12 +616,16 @@ int tb_gp_update_posterior_cache(tb_gp* gp) {
 // Rank-m append (SURVEY.md §8f-1): the reference refactorises from scratch whenever the data change
 // (models.py:171-186 -> interface.py:108-112); one BO step only appends rows, so L, Linv and alpha are extended in
 // O(m N^2) instead of O(N^3).  The hyper-parameters must be unchanged since the cache was built.
-static int tb_gp_append_data_f64(tb_gp* gp, const double* Xnew, const double* ynew, int64_t m) {
-  TB_CHECK(gp && Xnew && ynew, "tb_gp_append_data: null argument");
+int tb_gp_append_data(tb_gp* gp, const void* Xnew_in, const void* ynew_in, int64_t m) {
+  TB_CHECK(gp && Xnew_in && ynew_in, "tb_gp_append_data: null argument");
   TB_CHECK(gp->cache_valid, "tb_gp_append_data: posterior cache is not built: call tb_gp_update_posterior_cache first");
   TB_CHECK(m > 0 && m <= APPEND_MAX, "tb_gp_append_data: between 1 and " + std::to_string(APPEND_MAX) + " new points per call");
   const int64_t N0 = gp->N, N = N0 + m;
   TB_CHECK(N <= 65535, "tb_gp_append_data: N > 65535 is not supported");
+  tb::DtypeBridge br(gp);
+  const double *Xnew, *ynew;
+  TB_TRY(br.in(Xnew_in, m * gp->D, &Xnew));
+  TB_TRY(br.in(ynew_in, m, &ynew));
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
   const int D = gp->D, DP = gp->DP;
@@ -618,18 +700,21 @@ static int tb_gp_append_data_f64(tb_gp* gp, const double* Xnew, const double* yn
   return finish_cache(gp, N0);
 }
 
-static int tb_gp_get_cholesky_f64(tb_gp* gp, void* L_out) {
-  TB_CHECK(gp && L_out, "tb_gp_get_cholesky: null argument");
+int tb_gp_get_cholesky(tb_gp* gp, void* L_user) {
+  TB_CHECK(gp && L_user, "tb_gp_get_cholesky: null argument");
   TB_CHECK(gp->cache_valid, "tb_gp_get_cholesky: posterior cache is not built");
-  TB_CUDA(cudaSetDevice(gp->device));
   const int64_t N = gp->N;
+  tb::DtypeBridge br(gp);
+  double* L_out;
+  TB_TRY(br.out(L_user, N * N, &L_out));
+  TB_CUDA(cudaSetDevice(gp->device));
   TB_TRY(gp->sMisc.reserve(sizeof(double) * N * N));
   dim3 grid((unsigned)((N + 127) / 128), (unsigned)N);
   colmajor_lower_to_rowmajor_kernel<<<grid, 128, 0, gp->stream>>>(gp->dL.as<double>(), N, gp->sMisc.as<double>());
   TB_LAUNCHED();
   TB_CUDA(cudaMemcpyAsync(L_out, gp->sMisc.p, sizeof(double) * N * N, cudaMemcpyDefault, gp->stream));
   TB_CUDA(cudaStreamSynchronize(gp->stream));
-  return 0;
+  return br.finish();
 }
 
 }  // extern "C"
@@ -1255,31 +1340,6 @@ static int profile_fold(tb_gp* gp) {
 struct EvalOut {
   double *vals = nullptr, *mean = nullptr, *var = nullptr, *grad = nullptr;
 };
-// The caller's device arrays are written in place; host arrays go through the handle's staging buffers (the means through
-// gp->sMean, which the K* step fills anyway) and copy_back brings them home.
-struct EvalRoutes {
-  bool xc, vals, mean, var, grad;  // device pointers?
-  explicit EvalRoutes(const EvalRequest& rq)
-      : xc(is_device_ptr(rq.Xc)), vals(is_device_ptr(rq.out_vals)), mean(is_device_ptr(rq.out_mean)), var(is_device_ptr(rq.out_var)),
-        grad(is_device_ptr(rq.out_grad)) {}
-  EvalOut chunk(tb_gp* gp, const EvalRequest& rq, int64_t c0) const {
-    EvalOut o;
-    if (rq.out_vals) o.vals = vals ? rq.out_vals + c0 : gp->sVals.as<double>();
-    if (rq.out_mean && mean) o.mean = rq.out_mean + c0;
-    if (rq.out_var) o.var = var ? rq.out_var + c0 : gp->sVar.as<double>();
-    if (rq.out_grad) o.grad = grad ? rq.out_grad + c0 * gp->D : gp->sGrad.as<double>();
-    return o;
-  }
-  int copy_back(tb_gp* gp, const EvalRequest& rq, int64_t c0, int64_t mc, const EvalOut& o) const {
-    cudaStream_t st = gp->stream;
-    if (rq.out_grad && !grad)
-      TB_CUDA(cudaMemcpyAsync(rq.out_grad + c0 * gp->D, o.grad, sizeof(double) * mc * gp->D, cudaMemcpyDeviceToHost, st));
-    if (rq.out_vals && !vals) TB_CUDA(cudaMemcpyAsync(rq.out_vals + c0, o.vals, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (rq.out_mean && !mean) TB_CUDA(cudaMemcpyAsync(rq.out_mean + c0, gp->sMean.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (rq.out_var && !var) TB_CUDA(cudaMemcpyAsync(rq.out_var + c0, o.var, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    return 0;
-  }
-};
 
 // One chunk of n device candidates at xc: K* and the means, the variance GEMM over G row-block groups, the gradient when
 // o.grad is set, the acquisition tail and the argmax fold.  c0: global index of the first candidate.  The screened argmax's
@@ -1416,18 +1476,22 @@ static ChunkPlan plan_chunks(const tb_gp* gp, Engine e, bool grad, int64_t M) {
   return p;
 }
 
-// The driver behind predict, acquisition values and gradients and the fused argmax: the candidates in chunks (plan_chunks),
-// each through eval_chunk, all on the handle's stream.  Stream order protects the scratch that one chunk reuses from the
-// last, so the host waits once, at the end of the call.
-static int run_eval(tb_gp* gp, EvalRequest& rq) {
+// the argument checks of run_eval, made before anything is staged
+static int check_eval(const tb_gp* gp, const EvalRequest& rq) {
   TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
   TB_CHECK(rq.M >= 0, "negative candidate count");
+  if (rq.want_argmax) TB_CHECK(rq.M > 0, "argmax over an empty candidate set");
+  return 0;
+}
+
+// The driver behind predict, acquisition values and gradients and the fused argmax: the candidates in chunks (plan_chunks),
+// each through eval_chunk, all on the handle's stream, host arrays staged as Staged describes.
+static int run_eval(tb_gp* gp, EvalRequest& rq) {
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
   const int D = gp->D;
   const bool grad = rq.out_grad != nullptr;
   if (rq.want_argmax) {
-    TB_CHECK(rq.M > 0, "argmax over an empty candidate set");
     TB_TRY(gp->sRun.reserve(16));
     TB_TRY(argmax_reset(gp));
   }
@@ -1437,18 +1501,21 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
   TB_TRY(select_engine(gp, grad, &e));
   const ChunkPlan cp = plan_chunks(gp, e, grad, rq.M);
   const int64_t chunk_cap = cp.chunk_cap, tiles_cap = chunk_cap / cp.nt;
-  const EvalRoutes dev(rq);
+  // a host out_mean is copied from gp->sMean, which the K* step fills anyway
+  const Staged<const double> xin(rq.Xc, D, gp->sXc, st);
+  const Staged<double> vals(rq.out_vals, 1, gp->sVals, st), mean(rq.out_mean, 1, gp->sMean, st), var(rq.out_var, 1, gp->sVar, st),
+      grads(rq.out_grad, D, gp->sGrad, st);
   TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
   TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)(cp.G ? cp.G : gp->NB) * chunk_cap));
   TB_TRY(gp->sMean.reserve(sizeof(double) * chunk_cap));
-  if (!dev.xc) TB_TRY(gp->sXc.reserve(sizeof(double) * chunk_cap * D));
-  if (rq.out_vals && !dev.vals) TB_TRY(gp->sVals.reserve(sizeof(double) * chunk_cap));
-  if (rq.out_var && !dev.var) TB_TRY(gp->sVar.reserve(sizeof(double) * chunk_cap));
+  TB_TRY(xin.reserve(chunk_cap));
+  TB_TRY(vals.reserve(chunk_cap));
+  TB_TRY(var.reserve(chunk_cap));
   if (grad) {
     if (e == Engine::F64) TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));  // packed A
     TB_TRY(gp->sV.reserve((size_t)chunk_cap * gp->NB * BM * sizeof(double)));
     TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * chunk_cap));
-    if (!dev.grad) TB_TRY(gp->sGrad.reserve(sizeof(double) * chunk_cap * D));
+    TB_TRY(grads.reserve(chunk_cap));
   }
   if (rq.want_argmax) {
     const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
@@ -1457,19 +1524,23 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
   }
 
   bool screened = false;
-  if (e != Engine::F64 && argmax_screen_wanted(rq, dev.xc)) TB_TRY(argmax_screened(gp, rq, e, chunk_cap, cp.G, &screened));
+  if (e != Engine::F64 && argmax_screen_wanted(rq, xin.dev)) TB_TRY(argmax_screened(gp, rq, e, chunk_cap, cp.G, &screened));
   const int64_t m_loop = screened ? 0 : rq.M;  // the screened path has folded its survivors into gp->sRun already
   for (int64_t c0 = 0; c0 < m_loop; c0 += chunk_cap) {
     const int64_t mc = std::min<int64_t>(chunk_cap, rq.M - c0);
-    const double* xc = rq.Xc + c0 * D;
-    if (!dev.xc) {
-      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, xc, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
-      xc = gp->sXc.as<double>();
-    }
+    const double* xc;
+    TB_TRY(xin.in(c0, mc, &xc));
     const int G = cp.G ? cp.G : eng_groups(gp, e, (int)((mc + cp.nt - 1) / cp.nt));
-    const EvalOut o = dev.chunk(gp, rq, c0);
+    EvalOut o;
+    o.vals = vals.out(c0);
+    o.mean = mean.host() ? nullptr : mean.out(c0);
+    o.var = var.out(c0);
+    o.grad = grads.out(c0);
     TB_TRY(eval_chunk(gp, rq, e, xc, mc, c0, G, o));
-    TB_TRY(dev.copy_back(gp, rq, c0, mc, o));
+    TB_TRY(grads.back(c0, mc));
+    TB_TRY(vals.back(c0, mc));
+    TB_TRY(mean.back(c0, mc));
+    TB_TRY(var.back(c0, mc));
   }
   if (rq.want_argmax) TB_TRY(argmax_read(gp, rq));
   TB_CUDA(cudaStreamSynchronize(st));
@@ -1479,30 +1550,26 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
 
 // posterior mean and its gradient (no variance, no GEMM, no K^-1): one mean_grad_kernel launch per 65,536 points
 static int run_mean_grad(tb_gp* gp, const double* Xc, int64_t M, double* mean, double* grad) {
-  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_CHECK(M >= 0, "negative point count");
   if (M == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
   const int D = gp->D;
   constexpr int64_t CHUNK = 65536;
   const int64_t cap = std::min(M, CHUNK);
-  const bool xc_dev = is_device_ptr(Xc), mean_dev = is_device_ptr(mean), grad_dev = is_device_ptr(grad);
-  if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * cap * D));
-  if (!mean_dev) TB_TRY(gp->sMean.reserve(sizeof(double) * cap));
-  if (!grad_dev) TB_TRY(gp->sGrad.reserve(sizeof(double) * cap * D));
+  const Staged<const double> xin(Xc, D, gp->sXc, st);
+  const Staged<double> means(mean, 1, gp->sMean, st), grads(grad, D, gp->sGrad, st);
+  TB_TRY(xin.reserve(cap));
+  TB_TRY(means.reserve(cap));
+  TB_TRY(grads.reserve(cap));
   const double* Xs = gp->dXs.as<double>();
   const double* al = gp->dAlpha.as<double>();
   const double* il = gp->dInvLs.as<double>();
   for (int64_t c0 = 0; c0 < M; c0 += CHUNK) {
     const int64_t mc = std::min(CHUNK, M - c0);
-    const double* xc = Xc + c0 * D;
-    if (!xc_dev) {
-      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, xc, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
-      xc = gp->sXc.as<double>();
-    }
-    double* md = mean_dev ? mean + c0 : gp->sMean.as<double>();
-    double* gd = grad_dev ? grad + c0 * D : gp->sGrad.as<double>();
+    const double* xc;
+    TB_TRY(xin.in(c0, mc, &xc));
+    double* md = means.out(c0);
+    double* gd = grads.out(c0);
     const unsigned blocks = (unsigned)((mc + 7) / 8);
     with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
       mean_grad_kernel<decltype(K)::value, decltype(P)::value><<<blocks, 256, 0, st>>>(Xs, al, xc, il, (int)gp->N, D, mc, gp->variance,
@@ -1510,9 +1577,8 @@ static int run_mean_grad(tb_gp* gp, const double* Xc, int64_t M, double* mean, d
     });
     TB_LAUNCHED();
     TB_CUDA(cudaGetLastError());
-    if (!mean_dev) TB_CUDA(cudaMemcpyAsync(mean + c0, md, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-    if (!grad_dev) TB_CUDA(cudaMemcpyAsync(grad + c0 * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
-    if (!xc_dev || !mean_dev || !grad_dev) TB_CUDA(cudaStreamSynchronize(st));  // scratch is reused by the next chunk
+    TB_TRY(means.back(c0, mc));
+    TB_TRY(grads.back(c0, mc));
   }
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
@@ -1537,10 +1603,6 @@ static int ensure_gibbon(tb_gp* gp) {
   TB_TRY(gp->dGibPs.reserve(sizeof(double) * ps.size()));
   TB_CUDA(cudaMemcpyAsync(gp->dGibPs.p, ps.data(), sizeof(double) * ps.size(), cudaMemcpyHostToDevice, st));
   tb::DevBuf work;  // Kxp, Y, W [m][N] and B [m][m]
-  struct Release {
-    tb::DevBuf* b;
-    ~Release() { b->release(); }
-  } rel{&work};
   TB_TRY(work.reserve(sizeof(double) * (3 * (size_t)m * N + (size_t)m * m)));
   double* Kxp = work.as<double>();
   double* Y = Kxp + (size_t)m * N;
@@ -1605,14 +1667,31 @@ static int ensure_gibbon(tb_gp* gp) {
 
 extern "C" {
 
-static int tb_gp_predict_f64(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* var) {
+int tb_gp_predict(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* var) {
   TB_CHECK(gp && (M == 0 || (Xc && mean && var)), "tb_gp_predict: null argument");
   tb::EvalRequest rq;
-  rq.Xc = (const double*)Xc;
   rq.M = M;
-  rq.out_mean = (double*)mean;
-  rq.out_var = (double*)var;
-  return tb::run_eval(gp, rq);
+  TB_TRY(tb::check_eval(gp, rq));
+  tb::DtypeBridge br(gp);
+  TB_TRY(br.in(Xc, M * gp->D, &rq.Xc));
+  TB_TRY(br.out(mean, M, &rq.out_mean));
+  TB_TRY(br.out(var, M, &rq.out_var));
+  TB_TRY(tb::run_eval(gp, rq));
+  return br.finish();
+}
+
+int tb_gp_mean_gradient(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* grad) {
+  TB_CHECK(gp && (M == 0 || (Xc && mean && grad)), "tb_gp_mean_gradient: null argument");
+  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_CHECK(M >= 0, "negative point count");
+  tb::DtypeBridge br(gp);
+  const double* xd;
+  double *md, *gd;
+  TB_TRY(br.in(Xc, M * gp->D, &xd));
+  TB_TRY(br.out(mean, M, &md));
+  TB_TRY(br.out(grad, M * gp->D, &gd));
+  TB_TRY(tb::run_mean_grad(gp, xd, M, md, gd));
+  return br.finish();
 }
 
 // TB_ACQ_PENALIZED is stripped from acq here: every kernel and check below sees the plain kind
@@ -1642,7 +1721,7 @@ static int prepare_gibbon(tb_gp* gp, int acq, const char* who) {
   return 0;
 }
 
-static int tb_acq_eval_f64(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad) {
+int tb_acq_eval(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad) {
   TB_CHECK(gp && (M == 0 || (Xc && out)), "tb_acq_eval: null argument");
   bool pen = false;
   TB_TRY(split_penalized(gp, acq, pen, "tb_acq_eval"));
@@ -1654,14 +1733,17 @@ static int tb_acq_eval_f64(tb_gp* gp, int acq, double param, const void* Xc, int
   rq.acq = acq;
   rq.pen = pen;
   rq.param = param;
-  rq.Xc = (const double*)Xc;
   rq.M = M;
-  rq.out_vals = (double*)out;
-  rq.out_grad = (double*)grad;
-  return tb::run_eval(gp, rq);
+  TB_TRY(tb::check_eval(gp, rq));
+  tb::DtypeBridge br(gp);
+  TB_TRY(br.in(Xc, M * gp->D, &rq.Xc));
+  TB_TRY(br.out(out, M, &rq.out_vals));
+  TB_TRY(br.out(grad, M * gp->D, &rq.out_grad));
+  TB_TRY(tb::run_eval(gp, rq));
+  return br.finish();
 }
 
-static int tb_acq_argmax_f64(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* best_value,
+int tb_acq_argmax(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* best_value,
                   int64_t* best_index) {
   TB_CHECK(gp && Xc && best_value && best_index, "tb_acq_argmax: null argument");
   bool pen = false;
@@ -1674,18 +1756,21 @@ static int tb_acq_argmax_f64(tb_gp* gp, int acq, double param, const void* Xc, i
   rq.acq = acq;
   rq.pen = pen;
   rq.param = param;
-  rq.Xc = (const double*)Xc;
   rq.M = M;
-  rq.out_vals = (double*)out;
   rq.want_argmax = true;
+  TB_TRY(tb::check_eval(gp, rq));
+  tb::DtypeBridge br(gp);
+  TB_TRY(br.in(Xc, M * gp->D, &rq.Xc));
+  TB_TRY(br.out(out, M, &rq.out_vals));
   TB_TRY(tb::run_eval(gp, rq));
   if (rq.best_index == INT64_MAX) {  // every value was NaN: tf.math.argmax still returns a valid index (optimizer.py:149)
     rq.best_index = 0;
     rq.best_value = std::nan("");
   }
-  *(double*)best_value = rq.best_value;
+  if (gp->dtype == TB_F32) *(float*)best_value = (float)rq.best_value;
+  else *(double*)best_value = rq.best_value;
   *best_index = rq.best_index;
-  return 0;
+  return br.finish();
 }
 
 int tb_acq_set_min_value_samples(tb_gp* gp, const double* samples, int S) {
@@ -1872,14 +1957,19 @@ static int launch_joint(tb_gp* gp, int QT, int blocks, size_t smem, const double
   return 0;
 }
 
-static int run_joint(tb_gp* gp, JointRequest& rq) {
+// the argument checks of run_joint and run_qei_grad, made before anything is staged; sampled: the call takes base samples
+static int check_batch(const tb_gp* gp, int64_t B, int q, bool sampled, int S, const void* eps, double jitter) {
   TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_CHECK(rq.q >= 1 && rq.q <= 32, "batch size q must be in [1, 32]");
-  TB_CHECK(rq.B >= 0, "negative batch count");
-  if (rq.mode != JOINT_PREDICT) {
-    TB_CHECK(rq.S >= 1 && rq.eps, "need S >= 1 base samples");
-    TB_CHECK(rq.jitter >= 0.0, "jitter must be non-negative");
+  TB_CHECK(q >= 1 && q <= 32, "batch size q must be in [1, 32]");
+  TB_CHECK(B >= 0, "negative batch count");
+  if (sampled) {
+    TB_CHECK(S >= 1 && eps, "need S >= 1 base samples");
+    TB_CHECK(jitter >= 0.0, "jitter must be non-negative");
   }
+  return 0;
+}
+
+static int run_joint(tb_gp* gp, JointRequest& rq) {
   if (rq.B == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
@@ -1898,26 +1988,16 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
   TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
   TB_TRY(gp->sV.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // A plain
   TB_TRY(gp->sMean.reserve(sizeof(double) * tiles_cap * nt));
-  const bool xc_dev = is_device_ptr(rq.Xc);
-  if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * cand_cap * D));
+  const Staged<const double> xin(rq.Xc, (int64_t)q * D, gp->sXc, st);
+  TB_TRY(xin.reserve(nbc_cap));
   const bool bei = rq.mode == JOINT_BEI;
-  const int eps_rows = bei ? q - 1 : q;
-  const double* eps_dev = nullptr;
-  if (rq.mode != JOINT_PREDICT) {
-    if (is_device_ptr(rq.eps)) {
-      eps_dev = rq.eps;
-    } else {
-      TB_TRY(gp->sMisc.reserve(sizeof(double) * (size_t)eps_rows * rq.S + 64));
-      TB_CUDA(cudaMemcpyAsync(gp->sMisc.p, rq.eps, sizeof(double) * (size_t)eps_rows * rq.S, cudaMemcpyHostToDevice, st));
-      eps_dev = gp->sMisc.as<double>();
-    }
-  }
+  // eps is null for JOINT_PREDICT
+  const Staged<const double> eps(rq.eps, (int64_t)(bei ? q - 1 : q) * rq.S, gp->sMisc, st);
+  const double* eps_dev;
+  TB_TRY(eps.reserve(1));
+  TB_TRY(eps.in(0, 1, &eps_dev));
   // JOINT_BEI: the chunk's joint posterior stays on the device for bei_kernel
   tb::DevBuf bmu, bcov;
-  struct Release {
-    tb::DevBuf *a, *b;
-    ~Release() { a->release(); b->release(); }
-  } rel{&bmu, &bcov};
   JointRequest jpredict = rq;
   jpredict.mode = JOINT_PREDICT;
   size_t smem_bei = 0;
@@ -1932,16 +2012,9 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
   TB_TRY(gp->sRun.reserve(16));
   int* err = reinterpret_cast<int*>(gp->sRun.p);
   TB_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
-  // host-staged outputs
-  struct Out { double* user; size_t per_batch; tb::DevBuf* buf; };
-  Out outs[4] = {{rq.out_mean, (size_t)q, &gp->sVals}, {rq.out_cov, (size_t)q * q, &gp->sVar},
-                 {rq.out_samples, (size_t)rq.S * q, &gp->sGrad}, {rq.out_qei, 1, &gp->sBlkBest}};
-  bool any_host_out = false;
-  for (auto& o : outs)
-    if (o.user && !is_device_ptr(o.user)) {
-      TB_TRY(o.buf->reserve(sizeof(double) * o.per_batch * nbc_cap));
-      any_host_out = true;
-    }
+  const Staged<double> outs[4] = {{rq.out_mean, q, gp->sVals, st}, {rq.out_cov, (int64_t)q * q, gp->sVar, st},
+                                  {rq.out_samples, (int64_t)rq.S * q, gp->sGrad, st}, {rq.out_qei, 1, gp->sBlkBest, st}};
+  for (auto& o : outs) TB_TRY(o.reserve(nbc_cap));
   const size_t smem = (size_t)JOINT_WARPS * (QP * QP + QP * D + QP) * sizeof(double);
 
   for (int64_t b0 = 0; b0 < rq.B; b0 += nbc_cap) {
@@ -1950,20 +2023,12 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
     const int tiles = (int)((mc + nt - 1) / nt);
     const int64_t McPad = (int64_t)tiles * nt;
     const double* xc_chunk;
-    if (xc_dev) {
-      xc_chunk = rq.Xc + b0 * q * D;
-    } else {
-      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, rq.Xc + b0 * q * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
-      xc_chunk = gp->sXc.as<double>();
-    }
+    TB_TRY(xin.in(b0, nbc, &xc_chunk));
     // A = Linv K*, stored plain for the per-batch Gram kernel
     TB_TRY(eng_kstar(gp, e, xc_chunk, mc, tiles));
     TB_TRY(eng_store_a(gp, e, tiles, McPad, gp->sV.as<double>()));
     double* dptr[4];
-    for (int i = 0; i < 4; ++i) {
-      Out& o = outs[i];
-      dptr[i] = !o.user ? nullptr : (is_device_ptr(o.user) ? o.user + b0 * o.per_batch : o.buf->as<double>());
-    }
+    for (int i = 0; i < 4; ++i) dptr[i] = outs[i].out(b0);
     const int blocks = (int)((nbc + JOINT_WARPS - 1) / JOINT_WARPS);
     const int Nrows = (int)lda;
     const JointRequest& jr = bei ? jpredict : rq;
@@ -1979,11 +2044,7 @@ static int run_joint(tb_gp* gp, JointRequest& rq) {
       TB_LAUNCHED();
       TB_CUDA(cudaGetLastError());
     }
-    for (auto& o : outs)
-      if (o.user && !is_device_ptr(o.user))
-        TB_CUDA(cudaMemcpyAsync(o.user + b0 * o.per_batch, o.buf->p, sizeof(double) * o.per_batch * nbc,
-                                cudaMemcpyDeviceToHost, st));
-    if (!xc_dev || any_host_out) TB_CUDA(cudaStreamSynchronize(st));
+    for (auto& o : outs) TB_TRY(o.back(b0, nbc));
   }
   int herr = 0;
   TB_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2035,27 +2096,18 @@ cross_cov_kernel(const double* __restrict__ A1, const double* __restrict__ A2, i
 }
 
 static int run_cross_cov(tb_gp* gp, const double* X1, int64_t M1, const double* X2, int64_t M2, double* out) {
-  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_CHECK(M1 >= 1 && M2 >= 1 && M1 + M2 <= 16384, "tb_gp_covariance_between_points: between 1 and 16384 points in total");
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
   const int D = gp->D;
   const int64_t lda = (int64_t)gp->NB * BM, M = M1 + M2;
   tb::DevBuf bx, bout;
-  struct Release {
-    std::vector<tb::DevBuf*> v;
-    ~Release() { for (auto* b : v) b->release(); }
-  } rel{{&bx, &bout}};
   TB_TRY(bx.reserve(sizeof(double) * M * D));  // [X1; X2] contiguous on the device
   TB_CUDA(cudaMemcpyAsync(bx.p, X1, sizeof(double) * M1 * D, cudaMemcpyDefault, st));
   TB_CUDA(cudaMemcpyAsync(bx.as<double>() + M1 * D, X2, sizeof(double) * M2 * D, cudaMemcpyDefault, st));
   TB_TRY(compute_a_plain(gp, bx.as<double>(), M));
-  const bool out_dev = is_device_ptr(out);
-  double* od = out;
-  if (!out_dev) {
-    TB_TRY(bout.reserve(sizeof(double) * (size_t)M1 * M2));
-    od = bout.as<double>();
-  }
+  const Staged<double> outs(out, M1 * M2, bout, st);
+  TB_TRY(outs.reserve(1));
+  double* od = outs.out(0);
   const double* A1 = gp->sA.as<double>();
   const double* A2 = A1 + M1 * lda;
   const double* x1 = bx.as<double>();
@@ -2069,7 +2121,7 @@ static int run_cross_cov(tb_gp* gp, const double* X1, int64_t M1, const double* 
     return 0;
   }));
   TB_LAUNCHED();
-  if (!out_dev) TB_CUDA(cudaMemcpyAsync(out, od, sizeof(double) * (size_t)M1 * M2, cudaMemcpyDeviceToHost, st));
+  TB_TRY(outs.back(0, 1));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
   return 0;
@@ -2117,25 +2169,15 @@ __global__ void add_mean_rows_kernel(double* __restrict__ out, const double* __r
 }
 
 static int run_sample_joint(tb_gp* gp, const double* Xc, int64_t M, const double* z, int S, double jitter, double* out) {
-  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_CHECK(M >= 1 && M <= 16384, "tb_gp_sample_joint: between 1 and 16384 points");
-  TB_CHECK(S >= 1 && z && out && Xc, "tb_gp_sample_joint: need S >= 1 standard-normal draws per point");
-  TB_CHECK(jitter >= 0.0, "jitter must be non-negative");
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
   const int D = gp->D;
   const int64_t lda = (int64_t)gp->NB * BM;
   tb::DevBuf bx, bcov, bz, bout, bdinv;
-  struct Release {
-    std::vector<tb::DevBuf*> v;
-    ~Release() { for (auto* b : v) b->release(); }
-  } rel{{&bx, &bcov, &bz, &bout, &bdinv}};
-  const double* xc = Xc;
-  if (!is_device_ptr(Xc)) {
-    TB_TRY(bx.reserve(sizeof(double) * M * D));
-    TB_CUDA(cudaMemcpyAsync(bx.p, Xc, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
-    xc = bx.as<double>();
-  }
+  const Staged<const double> xin(Xc, D, bx, st);
+  const double* xc;
+  TB_TRY(xin.reserve(M));
+  TB_TRY(xin.in(0, M, &xc));
   TB_TRY(compute_a_plain(gp, xc, M));
   TB_TRY(bcov.reserve(sizeof(double) * M * M));
   {
@@ -2180,23 +2222,18 @@ static int run_sample_joint(tb_gp* gp, const double* Xc, int64_t M, const double
   TB_CHECK_CODE(info == 0, "Cholesky decomposition was not successful. The input might not be valid "
                       "(joint covariance + jitter*I is not positive definite at leading minor " + std::to_string(info) + ")", tb::ERR_NUMERIC);
   // samples = mean + L z
-  const double* zd = z;
-  if (!is_device_ptr(z)) {
-    TB_TRY(bz.reserve(sizeof(double) * (size_t)S * M));
-    TB_CUDA(cudaMemcpyAsync(bz.p, z, sizeof(double) * (size_t)S * M, cudaMemcpyHostToDevice, st));
-    zd = bz.as<double>();
-  }
-  const bool out_dev = is_device_ptr(out);
-  double* od = out;
-  if (!out_dev) {
-    TB_TRY(bout.reserve(sizeof(double) * (size_t)S * M));
-    od = bout.as<double>();
-  }
+  const Staged<const double> zin(z, (int64_t)S * M, bz, st);
+  const double* zd;
+  TB_TRY(zin.reserve(1));
+  TB_TRY(zin.in(0, 1, &zd));
+  const Staged<double> outs(out, (int64_t)S * M, bout, st);
+  TB_TRY(outs.reserve(1));
+  double* od = outs.out(0);
   trmv_lower_cols_kernel<<<dim3((unsigned)((M + 127) / 128), (unsigned)S), 128, 0, st>>>(bcov.as<double>(), M, M, zd, M, od, M);
   TB_LAUNCHED();
   add_mean_rows_kernel<<<(unsigned)(((int64_t)S * M + 255) / 256), 256, 0, st>>>(od, gp->sMean.as<double>(), M, (int64_t)S * M);
   TB_LAUNCHED();
-  if (!out_dev) TB_CUDA(cudaMemcpyAsync(out, od, sizeof(double) * (size_t)S * M, cudaMemcpyDeviceToHost, st));
+  TB_TRY(outs.back(0, 1));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
   return 0;
@@ -2222,13 +2259,8 @@ enum { QEI_TAIL_MC = 0, QEI_TAIL_GENZ = 1 };
 
 static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const double* eps, int S, double eta, double jitter,
                         double* out_val, double* out_grad, int tail = QEI_TAIL_MC) {
-  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_CHECK(q >= 1 && q <= 32, "batch size q must be in [1, 32]");
   const bool genz = tail == QEI_TAIL_GENZ;
   const int eps_rows = genz ? q - 1 : q;
-  TB_CHECK(B >= 0, "negative batch count");
-  TB_CHECK(S >= 1 && eps, "need S >= 1 base samples");
-  TB_CHECK(jitter >= 0.0, "jitter must be non-negative");
   if (B == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
@@ -2243,10 +2275,6 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
   const int64_t cand_cap = nbc_cap * q;
   const int64_t tiles_cap = (cand_cap + nt - 1) / nt;
   tb::DevBuf baplain;  // fp64 engine: plain copy of A for the Gram kernel (sA holds the packed panels the upper GEMM reads)
-  struct ReleaseA {
-    tb::DevBuf* b;
-    ~ReleaseA() { b->release(); }
-  } rel_a{&baplain};
   TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
   if (e != Engine::F64) {
     TB_TRY(gp->sA.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // A plain
@@ -2258,24 +2286,18 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
   TB_TRY(gp->sV.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // V plain
   TB_TRY(gp->sMean.reserve(sizeof(double) * tiles_cap * nt));
   TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * cand_cap));  // c_mu, c_var
-  const bool xc_dev = is_device_ptr(Xc), val_dev = is_device_ptr(out_val), grad_dev = is_device_ptr(out_grad);
-  if (!xc_dev) TB_TRY(gp->sXc.reserve(sizeof(double) * cand_cap * D));
-  if (!grad_dev) TB_TRY(gp->sGrad.reserve(sizeof(double) * cand_cap * D));
   tb::DevBuf beps, bcov, bmu, bsbar, bval;
-  struct Release {
-    std::vector<tb::DevBuf*> v;
-    ~Release() { for (auto* b : v) b->release(); }
-  } rel{{&beps, &bcov, &bmu, &bsbar, &bval}};
-  const double* eps_dev = eps;
-  if (!is_device_ptr(eps)) {
-    TB_TRY(beps.reserve(sizeof(double) * (size_t)eps_rows * S));
-    TB_CUDA(cudaMemcpyAsync(beps.p, eps, sizeof(double) * (size_t)eps_rows * S, cudaMemcpyHostToDevice, st));
-    eps_dev = beps.as<double>();
-  }
+  const Staged<const double> xin(Xc, (int64_t)q * D, gp->sXc, st), eps_in(eps, (int64_t)eps_rows * S, beps, st);
+  const Staged<double> vals(out_val, 1, bval, st), grads(out_grad, (int64_t)q * D, gp->sGrad, st);
+  TB_TRY(xin.reserve(nbc_cap));
+  TB_TRY(grads.reserve(nbc_cap));
+  const double* eps_dev;
+  TB_TRY(eps_in.reserve(1));
+  TB_TRY(eps_in.in(0, 1, &eps_dev));
   TB_TRY(bcov.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
   TB_TRY(bsbar.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
   TB_TRY(bmu.reserve(sizeof(double) * (size_t)cand_cap));
-  TB_TRY(bval.reserve(sizeof(double) * (size_t)nbc_cap));
+  TB_TRY(vals.reserve(nbc_cap));
   TB_TRY(gp->sRun.reserve(16));
   int* err = reinterpret_cast<int*>(gp->sRun.p);
   TB_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
@@ -2302,12 +2324,7 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
     const int tiles = (int)((mc + nt - 1) / nt);
     const int64_t McPad = (int64_t)tiles * nt;
     const double* xc_chunk;
-    if (xc_dev) {
-      xc_chunk = Xc + b0 * q * D;
-    } else {
-      TB_CUDA(cudaMemcpyAsync(gp->sXc.p, Xc + b0 * q * D, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
-      xc_chunk = gp->sXc.as<double>();
-    }
+    TB_TRY(xin.in(b0, nbc, &xc_chunk));
     // fp64 engine: A twice (plain for the Gram kernel, packed panels for its V GEMM); int8 engines: A plain in sA
     double* a_plain = e == Engine::F64 ? baplain.as<double>() : gp->sA.as<double>();
     TB_TRY(eng_kstar(gp, e, xc_chunk, mc, tiles));
@@ -2323,7 +2340,7 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
                                               nullptr, dmu, dcov, nullptr, nullptr, err);
     }));
     double* cmu = gp->sMisc.as<double>();
-    double* dval = val_dev ? out_val + b0 : bval.as<double>();
+    double* dval = vals.out(b0);
     if (genz) {
       bei_backward_kernel<<<(unsigned)nbc, bei_warps * 32, smem_back, st>>>(dmu, dcov, q, eps_dev, S, eta, dval, cmu, cmu + mc,
                                                                            bsbar.as<double>(), err);
@@ -2335,12 +2352,11 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
     qei_mix_kernel<<<dim3((unsigned)nbc, (unsigned)((gp->N + 255) / 256)), 256, 0, st>>>(gp->sV.as<double>(), lda, (int)gp->N, q,
                                                                                         bsbar.as<double>());
     TB_LAUNCHED();
-    double* gd = grad_dev ? out_grad + b0 * q * D : gp->sGrad.as<double>();
+    double* gd = grads.out(b0);
     TB_TRY(launch_grad(gp, xc_chunk, mc, gd));
     TB_TRY(launch_qei_cross(gp, xc_chunk, mc, q, bsbar.as<double>(), gd));
-    if (!val_dev) TB_CUDA(cudaMemcpyAsync(out_val + b0, bval.p, sizeof(double) * nbc, cudaMemcpyDeviceToHost, st));
-    if (!grad_dev) TB_CUDA(cudaMemcpyAsync(out_grad + b0 * q * D, gd, sizeof(double) * mc * D, cudaMemcpyDeviceToHost, st));
-    if (!xc_dev || !val_dev || !grad_dev) TB_CUDA(cudaStreamSynchronize(st));
+    TB_TRY(vals.back(b0, nbc));
+    TB_TRY(grads.back(b0, nbc));
   }
   int herr = 0;
   TB_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2355,47 +2371,55 @@ static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const dou
 
 extern "C" {
 
-static int tb_gp_predict_joint_f64(tb_gp* gp, const void* Xc, int64_t B, int q, void* mean, void* cov) {
+int tb_gp_predict_joint(tb_gp* gp, const void* Xc, int64_t B, int q, void* mean, void* cov) {
   TB_CHECK(gp && (B == 0 || (Xc && mean && cov)), "tb_gp_predict_joint: null argument");
+  TB_TRY(tb::check_batch(gp, B, q, false, 0, nullptr, 0.0));
   tb::JointRequest rq;
   rq.mode = JOINT_PREDICT;
-  rq.Xc = (const double*)Xc;
   rq.B = B;
   rq.q = q;
-  rq.out_mean = (double*)mean;
-  rq.out_cov = (double*)cov;
-  return tb::run_joint(gp, rq);
+  tb::DtypeBridge br(gp);
+  TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
+  TB_TRY(br.out(mean, B * q, &rq.out_mean));
+  TB_TRY(br.out(cov, B * q * q, &rq.out_cov));
+  TB_TRY(tb::run_joint(gp, rq));
+  return br.finish();
 }
 
-static int tb_acq_batch_mc_ei_f64(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double eta,
-                       double jitter, void* out) {
+int tb_acq_batch_mc_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double eta, double jitter,
+                       void* out) {
   TB_CHECK(gp && (B == 0 || (Xc && eps && out)), "tb_acq_batch_mc_ei: null argument");
+  TB_TRY(tb::check_batch(gp, B, q, true, S, eps, jitter));
   tb::JointRequest rq;
   rq.mode = JOINT_QEI;
-  rq.Xc = (const double*)Xc;
   rq.B = B;
   rq.q = q;
-  rq.eps = (const double*)eps;
   rq.S = S;
   rq.eta = eta;
   rq.jitter = jitter;
-  rq.out_qei = (double*)out;
-  return tb::run_joint(gp, rq);
+  tb::DtypeBridge br(gp);
+  TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
+  TB_TRY(br.in(eps, (int64_t)q * S, &rq.eps));
+  TB_TRY(br.out(out, B, &rq.out_qei));
+  TB_TRY(tb::run_joint(gp, rq));
+  return br.finish();
 }
 
-static int tb_gp_reparam_sample_f64(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double jitter,
-                         void* samples) {
+int tb_gp_reparam_sample(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double jitter, void* samples) {
   TB_CHECK(gp && (B == 0 || (Xc && eps && samples)), "tb_gp_reparam_sample: null argument");
+  TB_TRY(tb::check_batch(gp, B, q, true, S, eps, jitter));
   tb::JointRequest rq;
   rq.mode = JOINT_SAMPLE;
-  rq.Xc = (const double*)Xc;
   rq.B = B;
   rq.q = q;
-  rq.eps = (const double*)eps;
   rq.S = S;
   rq.jitter = jitter;
-  rq.out_samples = (double*)samples;
-  return tb::run_joint(gp, rq);
+  tb::DtypeBridge br(gp);
+  TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
+  TB_TRY(br.in(eps, (int64_t)q * S, &rq.eps));
+  TB_TRY(br.out(samples, B * S * q, &rq.out_samples));
+  TB_TRY(tb::run_joint(gp, rq));
+  return br.finish();
 }
 
 // ---- top-k ---------------------------------------------------------------------------------------
@@ -2406,45 +2430,36 @@ int tb_topk(int device, int dtype, const void* values, int64_t M, int k, void* t
   TB_CUDA(cudaSetDevice(device));
   int64_t P = BIT_TILE;
   while (P < M) P <<= 1;
-  const bool vdev = is_device_ptr(values), tvdev = is_device_ptr(top_values), tidev = is_device_ptr(top_indices);
-  tb::DevBuf a, vin, tv, ti;
-  int rc = 0;
-  auto body = [&]() -> int {
-    TB_TRY(a.reserve(sizeof(VI) * P));
-    const double* vd = (const double*)values;
-    if (!vdev) {
-      TB_TRY(vin.reserve(sizeof(double) * M));
-      TB_CUDA(cudaMemcpy(vin.p, values, sizeof(double) * M, cudaMemcpyHostToDevice));
-      vd = vin.as<double>();
-    }
-    topk_init_kernel<<<(unsigned)((P + 255) / 256), 256>>>(vd, M, P, a.as<VI>());
-    TB_LAUNCHED();
-    const unsigned nblk = (unsigned)(P / BIT_TILE);
-    bitonic_local_kernel<<<nblk, 1024>>>(a.as<VI>(), 2, BIT_TILE);
-    TB_LAUNCHED();
-    for (int64_t kk = (int64_t)BIT_TILE * 2; kk <= P; kk <<= 1) {
-      for (int64_t j = kk >> 1; j >= BIT_TILE; j >>= 1) {
-        bitonic_global_kernel<<<(unsigned)((P / 2 + 255) / 256), 256>>>(a.as<VI>(), P, kk, j);
-        TB_LAUNCHED();
-      }
-      bitonic_local_kernel<<<nblk, 1024>>>(a.as<VI>(), kk, kk);
+  tb::DevBuf a, vin, tv, ti;  // legacy default stream (0) throughout
+  const tb::Staged<const double> vals((const double*)values, M, vin, 0);
+  const tb::Staged<double> tvals((double*)top_values, k, tv, 0);
+  const tb::Staged<int64_t> tidx(top_indices, k, ti, 0);
+  TB_TRY(a.reserve(sizeof(VI) * P));
+  const double* vd;
+  TB_TRY(vals.reserve(1));
+  TB_TRY(vals.in(0, 1, &vd));
+  topk_init_kernel<<<(unsigned)((P + 255) / 256), 256>>>(vd, M, P, a.as<VI>());
+  TB_LAUNCHED();
+  const unsigned nblk = (unsigned)(P / BIT_TILE);
+  bitonic_local_kernel<<<nblk, 1024>>>(a.as<VI>(), 2, BIT_TILE);
+  TB_LAUNCHED();
+  for (int64_t kk = (int64_t)BIT_TILE * 2; kk <= P; kk <<= 1) {
+    for (int64_t j = kk >> 1; j >= BIT_TILE; j >>= 1) {
+      bitonic_global_kernel<<<(unsigned)((P / 2 + 255) / 256), 256>>>(a.as<VI>(), P, kk, j);
       TB_LAUNCHED();
     }
-    double* tvd = (double*)top_values;
-    int64_t* tid = top_indices;
-    if (!tvdev) { TB_TRY(tv.reserve(sizeof(double) * k)); tvd = tv.as<double>(); }
-    if (!tidev) { TB_TRY(ti.reserve(sizeof(int64_t) * k)); tid = ti.as<int64_t>(); }
-    topk_emit_kernel<<<(k + 255) / 256, 256>>>(a.as<VI>(), k, tvd, tid);
+    bitonic_local_kernel<<<nblk, 1024>>>(a.as<VI>(), kk, kk);
     TB_LAUNCHED();
-    TB_CUDA(cudaGetLastError());
-    if (!tvdev) TB_CUDA(cudaMemcpy(top_values, tvd, sizeof(double) * k, cudaMemcpyDeviceToHost));
-    if (!tidev) TB_CUDA(cudaMemcpy(top_indices, tid, sizeof(int64_t) * k, cudaMemcpyDeviceToHost));
-    TB_CUDA(cudaDeviceSynchronize());
-    return 0;
-  };
-  rc = body();
-  a.release(); vin.release(); tv.release(); ti.release();
-  return rc;
+  }
+  TB_TRY(tvals.reserve(1));
+  TB_TRY(tidx.reserve(1));
+  topk_emit_kernel<<<(k + 255) / 256, 256>>>(a.as<VI>(), k, tvals.out(0), tidx.out(0));
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  TB_TRY(tvals.back(0, 1));
+  TB_TRY(tidx.back(0, 1));
+  TB_CUDA(cudaDeviceSynchronize());
+  return 0;
 }
 
 }  // extern "C"
@@ -2484,11 +2499,8 @@ int tb_rff_destroy(tb_rff* r) {
   if (!r) return 0;
   cudaSetDevice(r->device);
   cudaStreamSynchronize(r->stream);
-  for (tb::DevBuf* b : {&r->dW, &r->dB, &r->dTheta, &r->dInvLs, &r->sXc, &r->sOut, &r->sBlkBest, &r->sBlkIdx,
-                        &r->sRunV, &r->sRunI, &r->dXs, &r->dV, &r->sCanon})
-    b->release();
   cudaStreamDestroy(r->stream);
-  delete r;
+  delete r;  // frees the device buffers
   return 0;
 }
 
@@ -2630,11 +2642,12 @@ int tb_rff_eval(tb_rff* r, const void* Xc, int64_t M, void* out, double* min_val
   cudaStream_t st = r->stream;
   const int D = r->D, nb = r->nb;
   const double scale = std::sqrt(2.0 * r->variance / (double)r->F);
-  const bool xdev = is_device_ptr(Xc), odev = is_device_ptr(out);
   const int64_t chunk = std::min<int64_t>(M, (int64_t)1 << 22);
   const int blocks_cap = (int)((chunk + RFF_THREADS - 1) / RFF_THREADS);
-  if (!xdev) TB_TRY(r->sXc.reserve(sizeof(double) * chunk * D));
-  if (out && !odev) TB_TRY(r->sOut.reserve(sizeof(double) * chunk * nb));
+  const tb::Staged<const double> xin((const double*)Xc, D, r->sXc, st);
+  const tb::Staged<double> outs((double*)out, nb, r->sOut, st);
+  TB_TRY(xin.reserve(chunk));
+  TB_TRY(outs.reserve(chunk));
   const bool want_min = min_value != nullptr;
   if (want_min) {
     TB_TRY(r->sBlkBest.reserve(sizeof(double) * (size_t)nb * blocks_cap));
@@ -2650,12 +2663,9 @@ int tb_rff_eval(tb_rff* r, const void* Xc, int64_t M, void* out, double* min_val
   for (int64_t c0 = 0; c0 < M; c0 += chunk) {
     const int64_t mc = std::min<int64_t>(chunk, M - c0);
     const int blocks = (int)((mc + RFF_THREADS - 1) / RFF_THREADS);
-    const double* xc = (const double*)Xc + c0 * D;
-    if (!xdev) {
-      TB_CUDA(cudaMemcpyAsync(r->sXc.p, xc, sizeof(double) * mc * D, cudaMemcpyHostToDevice, st));
-      xc = r->sXc.as<double>();
-    }
-    double* od = out ? (odev ? (double*)out + c0 * nb : r->sOut.as<double>()) : nullptr;
+    const double* xc;
+    TB_TRY(xin.in(c0, mc, &xc));
+    double* od = outs.out(c0);
     const double* addend = nullptr;
     if (r->N > 0) {
       TB_CHECK(r->nbc == nb, "tb_rff_eval: canonical weights and theta must have the same number of trajectories");
@@ -2676,9 +2686,7 @@ int tb_rff_eval(tb_rff* r, const void* Xc, int64_t M, void* out, double* min_val
                                           r->sRunV.as<double>(), r->sRunI.as<int64_t>());
       TB_LAUNCHED();
     }
-    if (out && !odev)
-      TB_CUDA(cudaMemcpyAsync((double*)out + c0 * nb, r->sOut.p, sizeof(double) * mc * nb, cudaMemcpyDeviceToHost, st));
-    if (!xdev || (out && !odev)) TB_CUDA(cudaStreamSynchronize(st));
+    TB_TRY(outs.back(c0, mc));
   }
   if (want_min) {
     std::vector<double> hv(nb);
@@ -2695,179 +2703,7 @@ int tb_rff_eval(tb_rff* r, const void* Xc, int64_t M, void* out, double* min_val
 }  // extern "C"
 
 
-// =================================================================================================
-// dtype dispatch.  TB_F32 handles (fp32 models, e.g. BASELINE config 5) take and return float arrays;
-// in this build the arithmetic still runs on the fp64 DMMA path (inputs widened on the device, outputs
-// narrowed), which exceeds the fp32 tolerance; an fp32-native tensor path is listed as next in DESIGN.md.
-// =================================================================================================
-namespace tb {
-
-__global__ void widen_kernel(const float* __restrict__ in, int64_t n, double* __restrict__ out) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (double)in[i];
-}
-__global__ void narrow_kernel(const double* __restrict__ in, int64_t n, float* __restrict__ out) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (float)in[i];
-}
-
-// per-call staging of float arrays as device doubles
-struct F32Bridge {
-  tb_gp* gp;
-  std::vector<void*> allocs;
-  struct Pending { double* dev; void* user; int64_t n; };
-  std::vector<Pending> outs;
-  explicit F32Bridge(tb_gp* g) : gp(g) {}
-  ~F32Bridge() { for (void* p : allocs) cudaFree(p); }
-  int alloc(void** p, size_t bytes) {
-    TB_CUDA(cudaMalloc(p, std::max<size_t>(bytes, 16)));
-    allocs.push_back(*p);
-    return 0;
-  }
-  int in(const void* user, int64_t n, const double** out) {  // float (host or device) -> device double
-    *out = nullptr;
-    if (!user || n == 0) return 0;
-    const float* src = (const float*)user;
-    if (!is_device_ptr(user)) {
-      void* tmp;
-      TB_TRY(alloc(&tmp, sizeof(float) * n));
-      TB_CUDA(cudaMemcpyAsync(tmp, user, sizeof(float) * n, cudaMemcpyHostToDevice, gp->stream));
-      src = (const float*)tmp;
-    }
-    void* d;
-    TB_TRY(alloc(&d, sizeof(double) * n));
-    widen_kernel<<<(unsigned)((n + 255) / 256), 256, 0, gp->stream>>>(src, n, (double*)d);
-    TB_LAUNCHED();
-    *out = (const double*)d;
-    return 0;
-  }
-  int out(void* user, int64_t n, double** dev) {  // device double scratch, narrowed into `user` by finish()
-    *dev = nullptr;
-    if (!user || n == 0) return 0;
-    void* d;
-    TB_TRY(alloc(&d, sizeof(double) * n));
-    *dev = (double*)d;
-    outs.push_back({(double*)d, user, n});
-    return 0;
-  }
-  int finish() {
-    for (auto& o : outs) {
-      float* dst = (float*)o.user;
-      void* tmp = nullptr;
-      const bool dev = is_device_ptr(o.user);
-      if (!dev) {
-        TB_TRY(alloc(&tmp, sizeof(float) * o.n));
-        dst = (float*)tmp;
-      }
-      narrow_kernel<<<(unsigned)((o.n + 255) / 256), 256, 0, gp->stream>>>(o.dev, o.n, dst);
-      TB_LAUNCHED();
-      if (!dev) TB_CUDA(cudaMemcpyAsync(o.user, tmp, sizeof(float) * o.n, cudaMemcpyDeviceToHost, gp->stream));
-    }
-    TB_CUDA(cudaStreamSynchronize(gp->stream));
-    TB_CUDA(cudaGetLastError());
-    return 0;
-  }
-};
-
-}  // namespace tb
-
 extern "C" {
-
-int tb_gp_set_data(tb_gp* gp, const void* X, const void* y, int64_t N, int D) {
-  TB_CHECK(gp && X && y, "tb_gp_set_data: null argument");
-  if (gp->dtype == TB_F64) return tb_gp_set_data_f64(gp, X, y, N, D);
-  TB_CHECK(N > 0 && D > 0, "tb_gp_set_data: dataset must be populated (N > 0)");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double *Xd, *yd;
-  TB_TRY(br.in(X, N * D, &Xd));
-  TB_TRY(br.in(y, N, &yd));
-  return tb_gp_set_data_f64(gp, Xd, yd, N, D);
-}
-
-int tb_gp_append_data(tb_gp* gp, const void* Xnew, const void* ynew, int64_t m) {
-  TB_CHECK(gp && Xnew && ynew, "tb_gp_append_data: null argument");
-  if (gp->dtype == TB_F64) return tb_gp_append_data_f64(gp, (const double*)Xnew, (const double*)ynew, m);
-  TB_CHECK(m > 0 && gp->have_data, "tb_gp_append_data: set the data first and append at least one point");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double *Xd, *yd;
-  TB_TRY(br.in(Xnew, m * gp->D, &Xd));
-  TB_TRY(br.in(ynew, m, &yd));
-  return tb_gp_append_data_f64(gp, Xd, yd, m);
-}
-
-int tb_gp_get_cholesky(tb_gp* gp, void* L_out) {
-  TB_CHECK(gp && L_out, "tb_gp_get_cholesky: null argument");
-  if (gp->dtype == TB_F64) return tb_gp_get_cholesky_f64(gp, L_out);
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  double* Ld;
-  TB_TRY(br.out(L_out, gp->N * gp->N, &Ld));
-  TB_TRY(tb_gp_get_cholesky_f64(gp, Ld));
-  return br.finish();
-}
-
-int tb_gp_predict(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* var) {
-  TB_CHECK(gp && (M == 0 || (Xc && mean && var)), "tb_gp_predict: null argument");
-  if (gp->dtype == TB_F64) return tb_gp_predict_f64(gp, Xc, M, mean, var);
-  if (M == 0) return 0;
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double* xd;
-  double *md, *vd;
-  TB_TRY(br.in(Xc, M * gp->D, &xd));
-  TB_TRY(br.out(mean, M, &md));
-  TB_TRY(br.out(var, M, &vd));
-  TB_TRY(tb_gp_predict_f64(gp, xd, M, md, vd));
-  return br.finish();
-}
-
-int tb_gp_mean_gradient(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* grad) {
-  TB_CHECK(gp && (M == 0 || (Xc && mean && grad)), "tb_gp_mean_gradient: null argument");
-  if (gp->dtype == TB_F64) return tb::run_mean_grad(gp, (const double*)Xc, M, (double*)mean, (double*)grad);
-  if (M == 0) return 0;
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double* xd;
-  double *md, *gd;
-  TB_TRY(br.in(Xc, M * gp->D, &xd));
-  TB_TRY(br.out(mean, M, &md));
-  TB_TRY(br.out(grad, M * gp->D, &gd));
-  TB_TRY(tb::run_mean_grad(gp, xd, M, md, gd));
-  return br.finish();
-}
-
-int tb_acq_eval(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad) {
-  TB_CHECK(gp && (M == 0 || (Xc && out)), "tb_acq_eval: null argument");
-  if (gp->dtype == TB_F64) return tb_acq_eval_f64(gp, acq, param, Xc, M, out, grad);
-  if (M == 0) return 0;
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double* xd;
-  double *od, *gd;
-  TB_TRY(br.in(Xc, M * gp->D, &xd));
-  TB_TRY(br.out(out, M, &od));
-  TB_TRY(br.out(grad, M * gp->D, &gd));
-  TB_TRY(tb_acq_eval_f64(gp, acq, param, xd, M, od, gd));
-  return br.finish();
-}
-
-int tb_acq_argmax(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* best_value,
-                  int64_t* best_index) {
-  TB_CHECK(gp && Xc && best_value && best_index, "tb_acq_argmax: null argument");
-  if (gp->dtype == TB_F64) return tb_acq_argmax_f64(gp, acq, param, Xc, M, out, best_value, best_index);
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double* xd;
-  double* od;
-  double best = 0.0;
-  TB_TRY(br.in(Xc, M * gp->D, &xd));
-  TB_TRY(br.out(out, M, &od));
-  TB_TRY(tb_acq_argmax_f64(gp, acq, param, xd, M, od, &best, best_index));
-  *(float*)best_value = (float)best;
-  return br.finish();
-}
 
 // ---- device-side multi-start L-BFGS (SURVEY.md §8f-3; acquisition/optimizer.py:566-745) ----
 __global__ void lbfgs_finish_kernel(tb::lb::State s, int64_t P, double* __restrict__ f_out, int32_t* __restrict__ success,
@@ -2902,10 +2738,6 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   const size_t PD = (size_t)P * D;
   // per-problem state + compact evaluation buffers (freed on return)
   tb::DevBuf bx, bf, bg, bd, bt, bS, bY, brho, bgam, bint, bnfev, btrial, bidx, bxt, bval, bgrad, bbox, bcount, bres;
-  struct Release {
-    std::vector<tb::DevBuf*> v;
-    ~Release() { for (auto* b : v) b->release(); }
-  } rel{{&bx, &bf, &bg, &bd, &bt, &bS, &bY, &brho, &bgam, &bint, &bnfev, &btrial, &bidx, &bxt, &bval, &bgrad, &bbox, &bcount, &bres}};
   TB_TRY(bx.reserve(8 * PD)); TB_TRY(bg.reserve(8 * PD)); TB_TRY(bd.reserve(8 * PD)); TB_TRY(btrial.reserve(8 * PD));
   TB_TRY(bf.reserve(8 * (size_t)P)); TB_TRY(bt.reserve(8 * (size_t)P)); TB_TRY(bgam.reserve(8 * (size_t)P));
   TB_TRY(bS.reserve(8 * PD * m)); TB_TRY(bY.reserve(8 * PD * m)); TB_TRY(brho.reserve(8 * (size_t)P * m));
@@ -2988,45 +2820,11 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   return 0;
 }
 
-int tb_gp_predict_joint(tb_gp* gp, const void* Xc, int64_t B, int q, void* mean, void* cov) {
-  TB_CHECK(gp && (B == 0 || (Xc && mean && cov)), "tb_gp_predict_joint: null argument");
-  if (gp->dtype == TB_F64) return tb_gp_predict_joint_f64(gp, Xc, B, q, mean, cov);
-  if (B == 0) return 0;
-  TB_CHECK(q >= 1 && q <= 32, "batch size q must be in [1, 32]");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double* xd;
-  double *md, *cd;
-  TB_TRY(br.in(Xc, B * q * gp->D, &xd));
-  TB_TRY(br.out(mean, B * q, &md));
-  TB_TRY(br.out(cov, B * q * q, &cd));
-  TB_TRY(tb_gp_predict_joint_f64(gp, xd, B, q, md, cd));
-  return br.finish();
-}
-
-int tb_acq_batch_mc_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double eta,
-                       double jitter, void* out) {
-  TB_CHECK(gp && (B == 0 || (Xc && eps && out)), "tb_acq_batch_mc_ei: null argument");
-  if (gp->dtype == TB_F64) return tb_acq_batch_mc_ei_f64(gp, Xc, B, q, eps, S, eta, jitter, out);
-  if (B == 0) return 0;
-  TB_CHECK(q >= 1 && q <= 32 && S >= 1, "batch size q must be in [1, 32] and S >= 1");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double *xd, *ed;
-  double* od;
-  TB_TRY(br.in(Xc, B * q * gp->D, &xd));
-  TB_TRY(br.in(eps, (int64_t)q * S, &ed));
-  TB_TRY(br.out(out, B, &od));
-  TB_TRY(tb_acq_batch_mc_ei_f64(gp, xd, B, q, ed, S, eta, jitter, od));
-  return br.finish();
-}
-
 int tb_gp_covariance_between_points(tb_gp* gp, const void* X1, int64_t M1, const void* X2, int64_t M2, void* out) {
   TB_CHECK(gp && X1 && X2 && out, "tb_gp_covariance_between_points: null argument");
-  if (gp->dtype == TB_F64) return tb::run_cross_cov(gp, (const double*)X1, M1, (const double*)X2, M2, (double*)out);
-  TB_CHECK(M1 >= 1 && M2 >= 1, "tb_gp_covariance_between_points: need at least one point in each set");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
+  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_CHECK(M1 >= 1 && M2 >= 1 && M1 + M2 <= 16384, "tb_gp_covariance_between_points: between 1 and 16384 points in total");
+  tb::DtypeBridge br(gp);
   const double *x1, *x2;
   double* od;
   TB_TRY(br.in(X1, M1 * gp->D, &x1));
@@ -3038,10 +2836,11 @@ int tb_gp_covariance_between_points(tb_gp* gp, const void* X1, int64_t M1, const
 
 int tb_gp_sample_joint(tb_gp* gp, const void* Xc, int64_t M, const double* z, int S, double jitter, void* out) {
   TB_CHECK(gp && Xc && z && out, "tb_gp_sample_joint: null argument");
-  if (gp->dtype == TB_F64) return tb::run_sample_joint(gp, (const double*)Xc, M, z, S, jitter, (double*)out);
-  TB_CHECK(M >= 1 && S >= 1, "tb_gp_sample_joint: need at least one point and one draw");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
+  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_CHECK(M >= 1 && M <= 16384, "tb_gp_sample_joint: between 1 and 16384 points");
+  TB_CHECK(S >= 1, "tb_gp_sample_joint: need S >= 1 standard-normal draws per point");
+  TB_CHECK(jitter >= 0.0, "jitter must be non-negative");
+  tb::DtypeBridge br(gp);
   const double* xd;
   double* od;
   TB_TRY(br.in(Xc, M * gp->D, &xd));
@@ -3053,12 +2852,8 @@ int tb_gp_sample_joint(tb_gp* gp, const void* Xc, int64_t M, const double* z, in
 int tb_acq_batch_mc_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double eta, double jitter,
                             void* out, void* grad) {
   TB_CHECK(gp && (B == 0 || (Xc && eps && out && grad)), "tb_acq_batch_mc_ei_grad: null argument");
-  if (gp->dtype == TB_F64)
-    return tb::run_qei_grad(gp, (const double*)Xc, B, q, (const double*)eps, S, eta, jitter, (double*)out, (double*)grad);
-  if (B == 0) return 0;
-  TB_CHECK(q >= 1 && q <= 32 && S >= 1, "batch size q must be in [1, 32] and S >= 1");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
+  TB_TRY(tb::check_batch(gp, B, q, true, S, eps, jitter));
+  tb::DtypeBridge br(gp);
   const double *xd, *ed;
   double *od, *gd;
   TB_TRY(br.in(Xc, B * q * gp->D, &xd));
@@ -3090,13 +2885,7 @@ int tb_acq_batch_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w
   rq.eps = w;
   rq.S = S;
   rq.eta = eta;
-  if (gp->dtype == TB_F64) {
-    rq.Xc = (const double*)Xc;
-    rq.out_qei = (double*)out;
-    return tb::run_joint(gp, rq);
-  }
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
+  tb::DtypeBridge br(gp);
   TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
   TB_TRY(br.out(out, B, &rq.out_qei));
   TB_TRY(tb::run_joint(gp, rq));
@@ -3107,10 +2896,7 @@ int tb_acq_batch_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const doub
                          void* grad) {
   TB_TRY(bei_args(gp, Xc, B, q, w, S, out, grad, true, "tb_acq_batch_ei_grad"));
   if (B == 0) return 0;
-  if (gp->dtype == TB_F64)
-    return tb::run_qei_grad(gp, (const double*)Xc, B, q, w, S, eta, 0.0, (double*)out, (double*)grad, tb::QEI_TAIL_GENZ);
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
+  tb::DtypeBridge br(gp);
   const double* xd;
   double *od, *gd;
   TB_TRY(br.in(Xc, B * q * gp->D, &xd));
@@ -3129,32 +2915,19 @@ int tb_mvn_cdf(int device, const double* x, const double* mean, const double* co
   TB_CHECK(S >= 1, "tb_mvn_cdf: need S >= 1 Sobol points");
   if (B == 0) return 0;
   TB_CUDA(cudaSetDevice(device));
-  tb::DevBuf bx, bm, bc, bw, bo, berr;
-  struct Release {
-    std::vector<tb::DevBuf*> v;
-    ~Release() { for (auto* b : v) b->release(); }
-  } rel{{&bx, &bm, &bc, &bw, &bo, &berr}};
-  auto stage = [](tb::DevBuf& buf, const double* p, size_t n, const double** dev) -> int {
-    if (!p || is_device_ptr(p)) {
-      *dev = p;
-      return 0;
-    }
-    TB_TRY(buf.reserve(sizeof(double) * n));
-    TB_CUDA(cudaMemcpy(buf.p, p, sizeof(double) * n, cudaMemcpyHostToDevice));
-    *dev = buf.as<double>();
-    return 0;
+  tb::DevBuf bx, bm, bc, bw, bo, berr;  // legacy default stream (0) throughout
+  auto stage = [](const tb::Staged<const double>& s, const double** dev) -> int {
+    TB_TRY(s.reserve(1));
+    return s.in(0, 1, dev);
   };
   const double *xd, *md, *cd, *wd;
-  TB_TRY(stage(bx, x, (size_t)B * Q, &xd));
-  TB_TRY(stage(bm, mean, (size_t)B * Q, &md));
-  TB_TRY(stage(bc, cov, (size_t)B * Q * Q, &cd));
-  TB_TRY(stage(bw, Q >= 2 ? w : nullptr, (size_t)(Q - 1) * S, &wd));
-  const bool odev = is_device_ptr(out);
-  double* od = out;
-  if (!odev) {
-    TB_TRY(bo.reserve(sizeof(double) * B));
-    od = bo.as<double>();
-  }
+  TB_TRY(stage({x, (int64_t)B * Q, bx, 0}, &xd));
+  TB_TRY(stage({mean, (int64_t)B * Q, bm, 0}, &md));
+  TB_TRY(stage({cov, (int64_t)B * Q * Q, bc, 0}, &cd));
+  TB_TRY(stage({Q >= 2 ? w : nullptr, (int64_t)(Q - 1) * S, bw, 0}, &wd));
+  const tb::Staged<double> outs(out, B, bo, 0);
+  TB_TRY(outs.reserve(1));
+  double* od = outs.out(0);
   TB_TRY(berr.reserve(sizeof(int)));
   TB_CUDA(cudaMemset(berr.p, 0, sizeof(int)));
   const size_t smem = (size_t)tb::BEI_MAX_WARPS * tb::bei_warp_doubles(Q) * sizeof(double);
@@ -3165,28 +2938,11 @@ int tb_mvn_cdf(int device, const double* x, const double* mean, const double* co
   TB_CUDA(cudaGetLastError());
   int herr = 0;
   TB_CUDA(cudaMemcpy(&herr, berr.p, sizeof(int), cudaMemcpyDeviceToHost));
-  if (!odev) TB_CUDA(cudaMemcpy(out, od, sizeof(double) * B, cudaMemcpyDeviceToHost));
+  TB_TRY(outs.back(0, 1));
   TB_CUDA(cudaDeviceSynchronize());
   TB_CHECK_CODE(herr == 0, "Cholesky decomposition was not successful. The input might not be valid "
                       "(cov + jitter*I of a row is not positive definite)", tb::ERR_NUMERIC);
   return 0;
-}
-
-int tb_gp_reparam_sample(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double jitter,
-                         void* samples) {
-  TB_CHECK(gp && (B == 0 || (Xc && eps && samples)), "tb_gp_reparam_sample: null argument");
-  if (gp->dtype == TB_F64) return tb_gp_reparam_sample_f64(gp, Xc, B, q, eps, S, jitter, samples);
-  if (B == 0) return 0;
-  TB_CHECK(q >= 1 && q <= 32 && S >= 1, "batch size q must be in [1, 32] and S >= 1");
-  TB_CUDA(cudaSetDevice(gp->device));
-  tb::F32Bridge br(gp);
-  const double *xd, *ed;
-  double* sd;
-  TB_TRY(br.in(Xc, B * q * gp->D, &xd));
-  TB_TRY(br.in(eps, (int64_t)q * S, &ed));
-  TB_TRY(br.out(samples, B * S * q, &sd));
-  TB_TRY(tb_gp_reparam_sample_f64(gp, xd, B, q, ed, S, jitter, sd));
-  return br.finish();
 }
 
 }  // extern "C"
