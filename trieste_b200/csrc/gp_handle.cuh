@@ -215,10 +215,14 @@ struct tb_gp {
   // screened argmax (tb_api.cu, argmax_screened): the screen bound ub of all M candidates, the survivors' coordinates / global
   // indices, and the bound pass's per-block winners + probe pair + survivor counts
   tb::DevBuf sScrUb, sScrX, sScrIdx, sScrBlk;
-  // fp32 mirrors of the posterior for the bound pass (prescreen.cuh), rebuilt when cache_gen moves: rows [nst*64][W] of
-  // (x', |x'|^2, σ_f² α, |σ_f² α|), the centre [DP] subtracted from scaled inputs, and the constants of the bound
+  // mirrors of the posterior for the bound pass (prescreen.cuh), rebuilt when cache_gen moves: pre_tc (tensor-core pass): its
+  // stages of fp16 B fragments and |σ_f² α| (pre_nsl n8 slices, the first pre_npos_sl with α > 0); otherwise (CUDA-core pass)
+  // fp32 rows [nst*64][W] of (x', |x'|^2, σ_f² α, |σ_f² α|); the centre [DP] subtracted from scaled inputs, and the constants
+  // of the bound
   tb::DevBuf dPreRows, dPreCentre;
   uint64_t pre_gen = ~(uint64_t)0;
+  bool pre_tc = false;
+  int pre_nsl = 0, pre_npos_sl = 0;
   double pre_scale = 1.0, pre_x2max = 0.0, pre_rel = 0.0, pre_lin = 0.0, pre_lin_max = 0.0, pre_abs = 0.0;
 
   // profiling of the dominant kernel

@@ -1017,7 +1017,51 @@ static bool argmax_screen_wanted(const EvalRequest& rq, bool xc_dev) {
   return rq.M >= SCREEN_MIN_M;
 }
 
-// fp32 mirrors of the posterior for the bound pass (prescreen.cuh) and the constants of its error bound (DESIGN.md §4d),
+// The tensor-core pass's training columns (tc_mean_bounds_kernel) from the fp32 mirror rows h (x', n = |x'|^2, a, |a|):
+// columns with a > 0 first, then the others, each class padded with zero columns to whole n8 slices; per slice, lane
+// (g, tg)'s B fragments of column g (k = 16 kk + 2 tg + {0, 1} and + 8) and then the slice's 8 weights |a|; zero stages up to
+// a whole one.  *f16_ok: every |X'_d| < 2^14 and n < 2^15, so the fp16 operands stay finite.
+static std::vector<unsigned char> prescreen_tc_columns(const std::vector<float>& h, int64_t N, int DP, int W, int* nsl,
+                                                       int* npos_sl, bool* f16_ok) {
+  const int NK = pre::tc_nk(DP), K = 16 * NK, SL = pre::tc_slices(DP), SLB = pre::tc_slice_bytes(DP);
+  std::vector<int64_t> cls[2];
+  for (int64_t j = 0; j < N; ++j) cls[h[(size_t)j * W + DP + 1] > 0.0f ? 0 : 1].push_back(j);
+  *npos_sl = (int)((cls[0].size() + 7) / 8);
+  *nsl = *npos_sl + (int)((cls[1].size() + 7) / 8);
+  std::vector<unsigned char> out((size_t)((*nsl + SL - 1) / SL) * SL * SLB, 0);
+  std::vector<__half> col((size_t)K);
+  *f16_ok = true;
+  auto split = [](float x, __half* lo) {
+    const __half hi = __float2half_rn(x);
+    *lo = __float2half_rn(x - __half2float(hi));
+    return hi;
+  };
+  for (int c = 0; c < 8 * *nsl; ++c) {
+    const int k = c < 8 * *npos_sl ? 0 : 1;
+    const int64_t i = k == 0 ? c : c - 8 * *npos_sl;
+    if (i >= (int64_t)cls[k].size()) continue;
+    const float* r = &h[(size_t)cls[k][i] * W];
+    std::fill(col.begin(), col.end(), __float2half_rn(0.0f));
+    for (int d = 0; d < DP; ++d) {
+      __half lo;
+      const __half hi = split(r[d], &lo);
+      col[d] = col[DP + d] = __float2half_rn(-2.0f * __half2float(hi));
+      col[2 * DP + d] = __float2half_rn(-2.0f * __half2float(lo));
+      *f16_ok = *f16_ok && std::fabs(r[d]) < 16384.0f;
+    }
+    col[3 * DP] = split(r[DP], &col[3 * DP + 1]);
+    *f16_ok = *f16_ok && r[DP] < 32768.0f;
+    unsigned char* sp = &out[(size_t)(c / 8) * SLB];
+    const int g = c % 8;
+    for (int tg = 0; tg < 4; ++tg)
+      for (int kk = 0; kk < NK; ++kk)
+        for (int hf = 0; hf < 2; ++hf) std::memcpy(sp + ((g * 4 + tg) * NK + kk) * 8 + 4 * hf, &col[kk * 16 + 8 * hf + 2 * tg], 4);
+    std::memcpy(sp + 256 * NK + 4 * g, &r[DP + 2], 4);
+  }
+  return out;
+}
+
+// Mirrors of the posterior for the bound pass (prescreen.cuh) and the constants of its error bound (DESIGN.md §4d),
 // rebuilt on the host whenever the posterior cache moves (cache_gen: refits and appends).  x' = (x / l - centre) * pre: the
 // centre is the midpoint of the training rows' bounding box (a shift leaves distances alone and shrinks the norms the
 // expansion form cancels), pre folds the kernel's distance scale and log2(e) into the coordinates.
@@ -1041,16 +1085,21 @@ static int prescreen_ensure(tb_gp* gp) {
     default: pre2 = 5.0 * LOG2E * LOG2E, cq = LN2 * LN2 / 6.0; break;
   }
   const double pre = std::sqrt(pre2);
-  std::vector<double> centre((size_t)DP, 0.0);
+  std::vector<double> centre((size_t)DP, 0.0), half_width((size_t)DP, 0.0);
   double unc2 = 0.0;  // max_j |x_j / l|^2, uncentred (the fp64 path's own cancellation)
   for (int d = 0; d < D; ++d) {
     double lo = INFINITY, hi = -INFINITY;
     for (int64_t j = 0; j < N; ++j) lo = std::min(lo, xs[j * DP + d]), hi = std::max(hi, xs[j * DP + d]);
     centre[d] = 0.5 * (lo + hi);
+    half_width[d] = 0.5 * (hi - lo);
   }
   std::vector<float> h((size_t)rows * W, 0.0f);
-  double x2max = 0.0, asum = 0.0, c2 = 0.0;
-  for (int d = 0; d < D; ++d) c2 += centre[d] * centre[d];
+  double x2max = 0.0, asum = 0.0, c2 = 0.0, box2 = 0.0;  // box2: |x'|^2 at a corner of the training rows' bounding box
+  for (int d = 0; d < D; ++d) {
+    c2 += centre[d] * centre[d];
+    const double hw = half_width[d] * pre;
+    box2 += hw * hw;
+  }
   for (int64_t j = 0; j < N; ++j) {
     float* r = &h[(size_t)j * W];
     double n2 = 0.0, u2 = 0.0;
@@ -1091,33 +1140,59 @@ static int prescreen_ensure(tb_gp* gp) {
                + kappa * s0                                 // s-proportional part up to s0
                + (double)(N + 64) * std::ldexp(1.0, -52)    // the fp64 path's own kernel values and sum, the fp64 folds
                + 1e-15;                                     // the clamp q >= 1e-30
+  const double lin_max = std::ldexp(1.0, -10);
   double lin;
+  std::vector<unsigned char> tc;
+  double terms = (double)rows;  // terms each candidate's sums add
+  gp->pre_tc = false;
   if (expand) {
-    lin = cq * (2 * DP + 10) * u;  // expansion-form cancellation and input rounding: |dq| <= (2 DP + 10) u (|x'|^2 + max|X'|^2)
     const double l64 = cq * (2 * DP + 10) * std::ldexp(1.0, -52);  // the fp64 path's expansion form on uncentred inputs
-    lin += l64;
     rel += l64 * pre2 * (c2 + unc2);
+    // FFMA dot product (mean_bounds_kernel): |dq| <= (2 DP + 10) u (|x'|^2 + max n_j)
+    lin = cq * (2 * DP + 10) * u + l64;
+    // tensor cores (tc_mean_bounds_kernel): |dq| <= lin_q (|x'|^2 + max n_j) + abs_q
+    const double rd = std::sqrt((double)DP);
+    const double lin_q = (4 + 1.01 * DP + 1) * u                      // input rounding of x' and X', the fp32 |x'|^2, n_j
+                         + 4.01 * std::ldexp(1.0, -22)                // dropped x_lo X_lo and the lo parts' rounding
+                         + 1.01 * rd * std::ldexp(1.0, -25)           // subnormal lo parts, via |x| + |X| <= 1 + (x2 + n) / 2
+                         + pre::tc_nk(DP) * 2.01 * 24 * std::ldexp(1.0, -23);  // accumulation, per k16 step
+    const double abs_q = 1.01 * rd * std::ldexp(1.0, -24) + std::ldexp(1.0, -25);
+    const double lin_tc = cq * lin_q + l64;
+    // The tensor-core pass's distance bound is ~7x wider.  It runs only where it still trusts, with a factor 2 to spare, every
+    // candidate inside the training rows' bounding box (|x'|^2 <= box2); elsewhere (short lengthscales: large pre-scaled norms)
+    // the FFMA pass keeps the screen pruning.
+    bool f16_ok = false;
+    if (1.01 * lin_tc * (box2 + 1.01 * x2max) <= 0.5 * lin_max) {
+      tc = prescreen_tc_columns(h, N, DP, W, &gp->pre_nsl, &gp->pre_npos_sl, &f16_ok);
+      gp->pre_tc = f16_ok;  // the fp16 operands of every training row are finite
+    }
+    if (gp->pre_tc) {
+      terms = 8.0 * gp->pre_nsl;
+      lin = lin_tc;
+      rel += cq * abs_q;
+    }
   } else {
     lin = LN2 * u;  // Matern12: |dr'| <= u (|x'| + max|X'|) from the input rounding
   }
   gp->pre_rel = 1.01 * rel;
   gp->pre_lin = 1.01 * lin;
-  gp->pre_lin_max = std::ldexp(1.0, -10);
-  gp->pre_abs = 1.01 * (asum * (2700.0 * std::ldexp(1.0, -126) + kappa * tail) + 2.0 * (double)rows * std::ldexp(1.0, -149));
+  gp->pre_lin_max = lin_max;
+  gp->pre_abs = 1.01 * (asum * (2700.0 * std::ldexp(1.0, -126) + kappa * tail) + 2.0 * terms * std::ldexp(1.0, -149));
   gp->pre_scale = pre;
   gp->pre_x2max = 1.01 * x2max;
-  TB_TRY(gp->dPreRows.reserve(sizeof(float) * h.size()));
+  const size_t bytes = gp->pre_tc ? tc.size() : sizeof(float) * h.size();
+  TB_TRY(gp->dPreRows.reserve(bytes));
   TB_TRY(gp->dPreCentre.reserve(sizeof(double) * DP));
-  TB_CUDA(cudaMemcpyAsync(gp->dPreRows.p, h.data(), sizeof(float) * h.size(), cudaMemcpyHostToDevice, st));
+  TB_CUDA(cudaMemcpyAsync(gp->dPreRows.p, gp->pre_tc ? (const void*)tc.data() : (const void*)h.data(), bytes, cudaMemcpyHostToDevice, st));
   TB_CUDA(cudaMemcpyAsync(gp->dPreCentre.p, centre.data(), sizeof(double) * DP, cudaMemcpyHostToDevice, st));
   TB_CUDA(cudaStreamSynchronize(st));
   gp->pre_gen = gp->cache_gen;
   return 0;
 }
 
-static int prescreen_cpt(int DP) { return DP <= 12 ? 4 : DP <= 20 ? 2 : 1; }
 static int prescreen_blocks(const tb_gp* gp, int64_t M) {
-  const int64_t per = (int64_t)pre::TH * prescreen_cpt(gp->DP);
+  const int DP = gp->DP;
+  const int64_t per = gp->pre_tc ? pre::tc_cands(DP) : (int64_t)pre::TH * (DP <= 12 ? 4 : DP <= 20 ? 2 : 1);
   return (int)((M + per - 1) / per);
 }
 
@@ -1135,14 +1210,21 @@ static int launch_mean_bounds(tb_gp* gp, cudaStream_t st, const double* Xc, int6
   b.x2max = gp->pre_x2max;
   b.mean_const = gp->mean_const;
   b.pre = gp->pre_scale;
-  const float* rows = gp->dPreRows.as<float>();
-  const int nst = (int)((gp->N + pre::KS - 1) / pre::KS), D = gp->D;
+  const int D = gp->D;
   const double* il = gp->dInvLs.as<double>();
   const double* cen = gp->dPreCentre.as<double>();
   const unsigned blocks = (unsigned)prescreen_blocks(gp, M);
   with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
-    pre::mean_bounds_kernel<decltype(K)::value, decltype(P)::value><<<blocks, pre::TH, 0, st>>>(rows, nst, Xc, il, cen, D, M, b, acq, param,
-                                                                                                 var_ub, out0, out1, blk_best, blk_idx);
+    constexpr int KIND = decltype(K)::value, DP = decltype(P)::value;
+    if (!gp->pre_tc) {
+      const int nst = (int)((gp->N + pre::KS - 1) / pre::KS);
+      pre::mean_bounds_kernel<KIND, DP><<<blocks, pre::TH, 0, st>>>(gp->dPreRows.as<float>(), nst, Xc, il, cen, D, M, b, acq, param,
+                                                                    var_ub, out0, out1, blk_best, blk_idx);
+    } else if constexpr (KIND != TB_MATERN12) {
+      pre::tc_mean_bounds_kernel<KIND, DP><<<blocks, pre::TH, 0, st>>>(gp->dPreRows.as<unsigned char>(), gp->pre_nsl, gp->pre_npos_sl,
+                                                                       Xc, il, cen, D, M, b, acq, param, var_ub, out0, out1, blk_best,
+                                                                       blk_idx);
+    }
   });
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
@@ -1380,6 +1462,7 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, Engine e, int64_t c
   const int D = gp->D, nt = eng_tile_width(gp, e);
   const int64_t M = rq.M;
   const int64_t cap = std::max<int64_t>(1, M / 4);
+  TB_TRY(prescreen_ensure(gp));  // it picks the bound-pass kernel, and with it the CTA count
   const int sblocks = (int)((M + 255) / 256), bblocks = prescreen_blocks(gp, M);
   TB_TRY(gp->sScrUb.reserve(sizeof(double) * (size_t)M));
   TB_TRY(gp->sScrX.reserve(sizeof(double) * (size_t)cap * D));
