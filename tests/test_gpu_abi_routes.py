@@ -220,6 +220,7 @@ def test_host_calls_spanning_several_chunks_match_device_calls():
         X = rng.uniform(size=(M, D))
         B = 25_001  # q-batches; one chunk of the joint drivers at N = 4096 holds fewer
         Xb = rng.uniform(size=(B, q, D))
+        w = rng.uniform(size=(q - 1, S))
         cases = {
             "eval values": (lib.tb_acq_eval, lambda m: [h, EI, 0.5, In(X[:m]), m, Out(m, np.float64), None], M_eval),
             "eval gradients": (lib.tb_acq_eval, lambda m: [h, EI, 0.5, In(X[:m]), m, Out(m, np.float64), Out((m, D), np.float64)],
@@ -228,6 +229,12 @@ def test_host_calls_spanning_several_chunks_match_device_calls():
             "joint": (lib.tb_gp_predict_joint, lambda b: [h, In(Xb[:b]), b, q, Out((b, q), np.float64), Out((b, q, q), np.float64)], B),
             "qei grad": (lib.tb_acq_batch_mc_ei_grad,
                          lambda b: [h, In(Xb[:b]), b, q, In(eps), S, 0.5, 1e-6, Out(b, np.float64), Out((b, q, D), np.float64)], B),
+            "batch mc ei": (lib.tb_acq_batch_mc_ei, lambda b: [h, In(Xb[:b]), b, q, In(eps), S, 0.5, 1e-6, Out(b, np.float64)], B),
+            "reparam samples": (lib.tb_gp_reparam_sample,
+                                lambda b: [h, In(Xb[:b]), b, q, In(eps), S, 1e-6, Out((b, S, q), np.float64)], B),
+            "batch ei": (lib.tb_acq_batch_ei, lambda b: [h, In(Xb[:b]), b, q, In(w), S, 0.5, Out(b, np.float64)], B),
+            "batch ei grad": (lib.tb_acq_batch_ei_grad,
+                              lambda b: [h, In(Xb[:b]), b, q, In(w), S, 0.5, Out(b, np.float64), Out((b, q, D), np.float64)], B),
         }
         for name, (fn, args, n) in cases.items():
             _call(fn, args(1000), (True, True))  # lazy builds

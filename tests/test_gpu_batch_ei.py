@@ -157,7 +157,7 @@ def test_agrees_with_device_batch_monte_carlo_ei():
         np.testing.assert_allclose(bei(X), mc(X), rtol=2e-2)
 
 
-@pytest.mark.parametrize("engine", ["int8", "fp64"])
+@pytest.mark.parametrize("engine", ["int8", "int8x21", "fp64"])
 @pytest.mark.parametrize("kind", ["rbf", "matern52"])
 @pytest.mark.parametrize("q,S", [(2, 64), (3, 100), (5, 33)])
 def test_value_and_gradient_match_oracle_and_finite_differences(q, S, kind, engine):

@@ -157,7 +157,7 @@ def test_monte_carlo_expected_improvement_single_point():
         MonteCarloExpectedImprovement(0)
 
 
-@pytest.mark.parametrize("engine", ["int8", "fp64"])
+@pytest.mark.parametrize("engine", ["int8", "int8x21", "fp64"])
 @pytest.mark.parametrize("kind", ["rbf", "matern32", "matern52"])
 @pytest.mark.parametrize("N,D,q,S", [(200, 6, 4, 64), (300, 6, 8, 512), (150, 3, 1, 32), (260, 10, 11, 100)])
 def test_batch_mc_ei_value_and_gradient_matches_oracle(N, D, q, S, kind, engine):

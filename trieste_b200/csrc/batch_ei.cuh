@@ -24,7 +24,6 @@ constexpr double GENZ_CLAMP = 1e-6;    // utils.py:177: y = Phi^-1(1e-6 + (1 - 2
 constexpr double GENZ_PIVOT = 1e-12;   // utils.py:168, 183: added to every pivot of the factor
 constexpr double BEI_JITTER = 1e-6;    // function.py:1776-1783 and the CDF's jitter (utils.py:114); hard-coded there too
 constexpr int BEI_MAX_WARPS = 4;
-constexpr int JOINT_BEI = 3;  // run_joint mode: JOINT_PREDICT into device scratch, then bei_kernel
 
 __device__ __forceinline__ double std_normal_pdf(double z) { return 0.3989422804014327 * exp(-0.5 * z * z); }
 

@@ -474,6 +474,35 @@ static int alpha_from_linv(tb_gp* gp) {
   return 0;
 }
 
+// Blocked Cholesky (factor.cuh) of the n x n column-major matrix A in place on gp->stream: L in the lower triangle, the
+// inverses of L's diagonal 128-blocks in dinv [ceil(n/128)][128][128].  *minor: the first leading minor that is not positive
+// definite (1-based), 0 if none.  Waits for the stream.
+static int blocked_cholesky(tb_gp* gp, double* A, int64_t n, double* dinv, int* minor) {
+  cudaStream_t st = gp->stream;
+  TB_TRY(gp->dInfo.reserve(sizeof(int)));
+  TB_CUDA(cudaMemsetAsync(gp->dInfo.p, 0, sizeof(int), st));
+  const int nbk = (int)((n + fac::FB - 1) / fac::FB);
+  const size_t diag_smem = sizeof(double) * fac::FB * (fac::FB + 1);
+  for (int jb = 0; jb < nbk; ++jb) {
+    const int j0 = jb * fac::FB;
+    fac::chol_diag_kernel<<<1, fac::THREADS, diag_smem, st>>>(A, n, j0, dinv, gp->dInfo.as<int>());
+    TB_LAUNCHED();
+    const int64_t below = n - (int64_t)(j0 + fac::FB);
+    if (below > 0) {
+      const unsigned t = (unsigned)((below + fac::FB - 1) / fac::FB);
+      fac::chol_panel_kernel<<<t, fac::THREADS, fac::GEMM_SMEM, st>>>(A, n, j0, dinv);
+      TB_LAUNCHED();
+      fac::chol_syrk_kernel<<<dim3(t, t), fac::THREADS, fac::GEMM_SMEM, st>>>(A, n, j0);
+      TB_LAUNCHED();
+    }
+  }
+  *minor = 0;
+  TB_CUDA(cudaMemcpyAsync(minor, gp->dInfo.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // pack the lower triangle of Linv into DMMA-fragment-ordered panels and mark the derived operand sets stale
 // appended_from > 0: the cache was extended from that many rows by tb_gp_append_data (the dense K^-1, when it exists, is grown
 // by the same rank instead of being invalidated)
@@ -536,26 +565,9 @@ int tb_gp_update_posterior_cache(tb_gp* gp) {
     // ---- hand-written path (factor.cuh): blocked Cholesky, Linv, alpha on the DMMA pipe; no library call ----
     const int nbk = (int)((N + fac::FB - 1) / fac::FB);
     TB_TRY(gp->dDinv.reserve(sizeof(double) * (size_t)nbk * fac::FB * fac::FB));
-    TB_CUDA(cudaMemsetAsync(gp->dInfo.p, 0, sizeof(int), st));
     double* A = gp->dL.as<double>();
-    const size_t diag_smem = sizeof(double) * fac::FB * (fac::FB + 1);
-    for (int jb = 0; jb < nbk; ++jb) {
-      const int j0 = jb * fac::FB;
-      fac::chol_diag_kernel<<<1, fac::THREADS, diag_smem, st>>>(A, N, j0, gp->dDinv.as<double>(), gp->dInfo.as<int>());
-      TB_LAUNCHED();
-      const int64_t below = N - (int64_t)(j0 + fac::FB);
-      if (below > 0) {
-        const unsigned t = (unsigned)((below + fac::FB - 1) / fac::FB);
-        fac::chol_panel_kernel<<<t, fac::THREADS, fac::GEMM_SMEM, st>>>(A, N, j0, gp->dDinv.as<double>());
-        TB_LAUNCHED();
-        fac::chol_syrk_kernel<<<dim3(t, t), fac::THREADS, fac::GEMM_SMEM, st>>>(A, N, j0);
-        TB_LAUNCHED();
-      }
-    }
-    int info = 0;
-    TB_CUDA(cudaMemcpyAsync(&info, gp->dInfo.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    TB_CUDA(cudaStreamSynchronize(st));
-    TB_CUDA(cudaGetLastError());
+    int info;
+    TB_TRY(blocked_cholesky(gp, A, N, gp->dDinv.as<double>(), &info));
     TB_CHECK_CODE(info == 0, "tb_gp_update_posterior_cache: Cholesky decomposition was not successful "
                         "(K + noise*I not positive definite at leading minor " + std::to_string(info) + ")", tb::ERR_NUMERIC);
     {
@@ -1999,34 +2011,50 @@ int tb_gp_profile_read(tb_gp* gp, double* trigemm_ms, int64_t* trigemm_launches,
 }  // extern "C"
 
 // =================================================================================================
-// joint posterior of q-batches: predict_joint / reparam samples / MC-qEI
+// q-batches of the joint posterior: predict_joint, reparam samples, MC-qEI and batch EI, values and gradients
 // =================================================================================================
 namespace tb {
 
-struct JointRequest {
-  int mode = JOINT_PREDICT;  // or JOINT_BEI: mean / cov into scratch, then bei_kernel into out_qei
+// what a q-batch call makes of each batch's joint posterior (mean [q], cov [q, q])
+enum class BatchTail {
+  Predict,  // mean and cov
+  Samples,  // mean + chol(cov + jitter I) eps, eps [q, S] normal base samples (sampler.py:277-278)
+  McEi,     // batch Monte-Carlo EI (function.py:1181-1186) over eps [q, S] normal base samples
+  BatchEi,  // batch EI of Chevalier & Ginsbourger (function.py:1747-1805) over the Sobol points w [q-1, S]
+};
+
+struct BatchRequest {
+  BatchTail tail;
+  bool grad = false;  // also d out_val / d Xc (McEi, BatchEi)
   const double* Xc = nullptr;  // [B, q, D]
-  int64_t B = 0;
-  int q = 0;
-  const double* eps = nullptr;  // [q, S] host or device (JOINT_BEI: the Sobol points w [q-1, S])
-  int S = 0;
-  double eta = 0.0, jitter = 0.0;
+  int64_t B;
+  int q;
+  const double* eps = nullptr;  // host or device: eps [q, S], or w [q-1, S] for BatchEi
+  int S;
+  double eta, jitter;
   double* out_mean = nullptr;     // [B, q]
   double* out_cov = nullptr;      // [B, q, q]
   double* out_samples = nullptr;  // [B, S, q]
-  double* out_qei = nullptr;      // [B]
+  double* out_val = nullptr;      // [B]
+  double* out_grad = nullptr;     // [B, q, D]
+  BatchRequest(BatchTail tail, int64_t B, int q, int S = 0, double eta = 0.0, double jitter = 0.0)
+      : tail(tail), B(B), q(q), S(S), eta(eta), jitter(jitter) {}
 };
 
+// joint_kernel over nb batches of the chunk whose A = Linv K* (plain) is in A and whose means are in gp->sMean
 template <int KIND>
-static int launch_joint(tb_gp* gp, int QT, int blocks, size_t smem, const double* A, int64_t lda, int Nrows,
-                        const double* mean, const double* xc, int64_t nb, const JointRequest& rq, const double* eps_dev,
-                        double* om, double* oc, double* os, double* oq, int* err) {
+static int launch_joint(tb_gp* gp, const BatchRequest& rq, int mode, const double* A, const double* xc, int64_t nb,
+                        const double* eps_dev, double* om, double* oc, double* os, double* oq, int* err) {
+  const int QT = (rq.q + 7) / 8, QP = QT * 8;
+  const int blocks = (int)((nb + JOINT_WARPS - 1) / JOINT_WARPS);
+  const size_t smem = (size_t)JOINT_WARPS * (QP * QP + QP * gp->D + QP) * sizeof(double);
+  const int64_t lda = (int64_t)gp->NB * BM;
   const double* il = gp->dInvLs.as<double>();
 #define TB_JOINT(QTV)                                                                                              \
   {                                                                                                                \
     TB_CUDA(cudaFuncSetAttribute(joint_kernel<KIND, QTV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    joint_kernel<KIND, QTV><<<blocks, JOINT_WARPS * 32, smem, gp->stream>>>(A, lda, Nrows, mean, xc, il, gp->D, nb, rq.q, \
-        gp->variance, rq.mode, eps_dev, rq.S, rq.eta, rq.jitter, om, oc, os, oq, err);                               \
+    joint_kernel<KIND, QTV><<<blocks, JOINT_WARPS * 32, smem, gp->stream>>>(A, lda, (int)lda, gp->sMean.as<double>(), xc, il, \
+        gp->D, nb, rq.q, gp->variance, mode, eps_dev, rq.S, rq.eta, rq.jitter, om, oc, os, oq, err);              \
   }
   switch (QT) {
     case 1: TB_JOINT(1); break;
@@ -2040,7 +2068,8 @@ static int launch_joint(tb_gp* gp, int QT, int blocks, size_t smem, const double
   return 0;
 }
 
-// the argument checks of run_joint and run_qei_grad, made before anything is staged; sampled: the call takes base samples
+// the argument checks of the q-batch calls other than batch EI (bei_args), made before anything is staged; sampled: the
+// call takes base samples
 static int check_batch(const tb_gp* gp, int64_t B, int q, bool sampled, int S, const void* eps, double jitter) {
   TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
   TB_CHECK(q >= 1 && q <= 32, "batch size q must be in [1, 32]");
@@ -2052,82 +2081,135 @@ static int check_batch(const tb_gp* gp, int64_t B, int q, bool sampled, int S, c
   return 0;
 }
 
-static int run_joint(tb_gp* gp, JointRequest& rq) {
+static int launch_qei_cross(tb_gp* gp, const double* xc, int64_t npts, int q, const double* sbar, double* grad) {
+  with_kind(gp->kernel, [&](auto K) {
+    qei_cross_kernel<decltype(K)::value><<<(unsigned)((npts + 127) / 128), 128, 0, gp->stream>>>(xc, gp->dInvLs.as<double>(), gp->D, npts,
+                                                                                                 q, sbar, gp->variance, grad);
+  });
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Every q-batch call, chunk by chunk of whole batches: K* -> A = Linv K* (stored plain) -> with a gradient, V = K^-1 K*
+// -> per-batch mean / cov (joint_kernel, which also computes the Samples tail and the McEi value) -> the other tails:
+// bei_kernel for the BatchEi value; for a gradient the tail's reverse kernel (value, G_mu, Sigma_bar: qei_backward_kernel
+// or bei_backward_kernel) -> per-batch mix V~ = Sigma_bar V (qei_mix_kernel) -> grad_kernel (the training-point sums) ->
+// qei_cross_kernel (the K(x_b, x_b) term).
+static int run_batch(tb_gp* gp, const BatchRequest& rq) {
   if (rq.B == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
-  const int D = gp->D, q = rq.q;
-  const int QT = (q + 7) / 8, QP = QT * 8;
+  const int D = gp->D, q = rq.q, S = rq.S;
   const int64_t lda = (int64_t)gp->NB * BM;
-
-  const int64_t max_tiles = chunk_tiles(gp);
-  int64_t nbc_cap = std::max<int64_t>(1, (max_tiles * BT) / q);  // whole batches per chunk
-  nbc_cap = std::min<int64_t>(nbc_cap, rq.B);
-  const int64_t cand_cap = nbc_cap * q;
+  const bool bei = rq.tail == BatchTail::BatchEi;
+  const int mode = rq.tail == BatchTail::Samples ? JOINT_SAMPLE : rq.tail == BatchTail::McEi && !rq.grad ? JOINT_QEI : JOINT_PREDICT;
+  const bool post_dev = bei || rq.grad;  // joint_kernel leaves mean / cov in bmu / bcov for a tail kernel
   Engine e;
-  TB_TRY(select_engine(gp, false, &e));
+  TB_TRY(select_engine(gp, rq.grad, &e));
   const int nt = eng_tile_width(gp, e);  // candidates per tile
+  const int64_t nbc_cap = std::min<int64_t>(std::max<int64_t>(1, (chunk_tiles(gp) * BT) / q), rq.B);  // whole batches per chunk
+  const int64_t cand_cap = nbc_cap * q;
   const int64_t tiles_cap = (cand_cap + nt - 1) / nt;
+  const size_t plain_bytes = (size_t)tiles_cap * nt * lda * sizeof(double);
+  // A plain, joint_kernel's operand, is in gp->sA, except on the fp64 engine with a gradient: there gp->sA holds A as the
+  // packed panels that the V GEMM reads, and A plain has the call's own buffer baplain
+  const bool packed_a = rq.grad && e == Engine::F64;
+  tb::DevBuf baplain, beps, bval, bmu, bcov, bsbar;
   TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
-  TB_TRY(gp->sV.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // A plain
+  if (packed_a) {
+    TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));
+    TB_TRY(baplain.reserve(plain_bytes));
+    TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)gp->NB * tiles_cap * BT));
+  } else {
+    TB_TRY(gp->sA.reserve(plain_bytes));
+  }
+  double* A = packed_a ? baplain.as<double>() : gp->sA.as<double>();
   TB_TRY(gp->sMean.reserve(sizeof(double) * tiles_cap * nt));
-  const Staged<const double> xin(rq.Xc, (int64_t)q * D, gp->sXc, st);
-  TB_TRY(xin.reserve(nbc_cap));
-  const bool bei = rq.mode == JOINT_BEI;
-  // eps is null for JOINT_PREDICT
-  const Staged<const double> eps(rq.eps, (int64_t)(bei ? q - 1 : q) * rq.S, gp->sMisc, st);
-  const double* eps_dev;
-  TB_TRY(eps.reserve(1));
-  TB_TRY(eps.in(0, 1, &eps_dev));
-  // JOINT_BEI: the chunk's joint posterior stays on the device for bei_kernel
-  tb::DevBuf bmu, bcov;
-  JointRequest jpredict = rq;
-  jpredict.mode = JOINT_PREDICT;
-  size_t smem_bei = 0;
-  int bei_warps = 0;
-  if (bei) {
+  if (rq.grad) {
+    TB_TRY(gp->sV.reserve(plain_bytes));                        // V plain
+    TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * cand_cap));  // c_mu, c_var
+    TB_TRY(bsbar.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
+  }
+  if (post_dev) {
     TB_TRY(bmu.reserve(sizeof(double) * (size_t)cand_cap));
     TB_TRY(bcov.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
-    bei_warps = std::min(BEI_MAX_WARPS, q + q * q);
-    smem_bei = (bei_cta_doubles(q) + (size_t)bei_warps * bei_warp_doubles(q)) * sizeof(double);
-    TB_CUDA(cudaFuncSetAttribute(bei_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bei));
   }
+  // with a gradient, gp->sMisc holds c_mu / c_var: the base samples and the values of host arrays go to the call's own buffers
+  const Staged<const double> xin(rq.Xc, (int64_t)q * D, gp->sXc, st);
+  const Staged<const double> eps(rq.eps, (int64_t)(bei ? q - 1 : q) * S, rq.grad ? beps : gp->sMisc, st);
+  const Staged<double> mean(rq.out_mean, q, gp->sVals, st), cov(rq.out_cov, (int64_t)q * q, gp->sVar, st);
+  const Staged<double> samples(rq.out_samples, (int64_t)S * q, gp->sGrad, st), grad(rq.out_grad, (int64_t)q * D, gp->sGrad, st);
+  const Staged<double> val(rq.out_val, 1, rq.grad ? bval : gp->sBlkBest, st);
+  const Staged<double>* outs[] = {&mean, &cov, &samples, &val, &grad};
+  TB_TRY(xin.reserve(nbc_cap));
+  for (auto* o : outs) TB_TRY(o->reserve(nbc_cap));
+  const double* eps_dev;  // null for Predict
+  TB_TRY(eps.reserve(1));
+  TB_TRY(eps.in(0, 1, &eps_dev));
   TB_TRY(gp->sRun.reserve(16));
   int* err = reinterpret_cast<int*>(gp->sRun.p);
   TB_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
-  const Staged<double> outs[4] = {{rq.out_mean, q, gp->sVals, st}, {rq.out_cov, (int64_t)q * q, gp->sVar, st},
-                                  {rq.out_samples, (int64_t)rq.S * q, gp->sGrad, st}, {rq.out_qei, 1, gp->sBlkBest, st}};
-  for (auto& o : outs) TB_TRY(o.reserve(nbc_cap));
-  const size_t smem = (size_t)JOINT_WARPS * (QP * QP + QP * D + QP) * sizeof(double);
+  // shared memory of the tail kernel, and warps per CTA of the batch EI kernels
+  int bei_warps = 0;
+  size_t tail_smem = 0;
+  if (bei) {
+    // as many warps (up to 4) as fit: one per unit CDF in flight, each with its per-sample state in shared memory
+    const size_t cta = bei_cta_doubles(q) * sizeof(double);
+    const size_t per_warp = (rq.grad ? bei_back_warp_doubles(q) : bei_warp_doubles(q)) * sizeof(double);
+    bei_warps = (int)std::min<size_t>(std::min<size_t>(BEI_MAX_WARPS, q + q * q), (227 * 1024 - cta) / per_warp);
+    tail_smem = cta + bei_warps * per_warp;
+    if (rq.grad)
+      TB_CUDA(cudaFuncSetAttribute(bei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
+    else
+      TB_CUDA(cudaFuncSetAttribute(bei_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
+  } else if (rq.grad) {
+    tail_smem = (size_t)QEIG_WARPS * (3 * q * q + 2 * q) * sizeof(double);
+    TB_CUDA(cudaFuncSetAttribute(qei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
+  }
 
   for (int64_t b0 = 0; b0 < rq.B; b0 += nbc_cap) {
     const int64_t nbc = std::min<int64_t>(nbc_cap, rq.B - b0);
     const int64_t mc = nbc * q;
     const int tiles = (int)((mc + nt - 1) / nt);
     const int64_t McPad = (int64_t)tiles * nt;
-    const double* xc_chunk;
-    TB_TRY(xin.in(b0, nbc, &xc_chunk));
-    // A = Linv K*, stored plain for the per-batch Gram kernel
-    TB_TRY(eng_kstar(gp, e, xc_chunk, mc, tiles));
-    TB_TRY(eng_store_a(gp, e, tiles, McPad, gp->sV.as<double>()));
-    double* dptr[4];
-    for (int i = 0; i < 4; ++i) dptr[i] = outs[i].out(b0);
-    const int blocks = (int)((nbc + JOINT_WARPS - 1) / JOINT_WARPS);
-    const int Nrows = (int)lda;
-    const JointRequest& jr = bei ? jpredict : rq;
-    double* om = bei ? bmu.as<double>() : dptr[0];
-    double* oc = bei ? bcov.as<double>() : dptr[1];
-    double* oq = bei ? nullptr : dptr[3];
+    const double* xc;
+    TB_TRY(xin.in(b0, nbc, &xc));
+    TB_TRY(eng_kstar(gp, e, xc, mc, tiles));
+    TB_TRY(eng_store_a(gp, e, tiles, McPad, A));
+    if (rq.grad) {
+      if (packed_a) TB_TRY(eng_variance(gp, e, tiles, eng_groups(gp, e, tiles), McPad, true));
+      TB_TRY(eng_store_v(gp, e, tiles, McPad));
+    }
+    double* mu = post_dev ? bmu.as<double>() : mean.out(b0);
+    double* cv = post_dev ? bcov.as<double>() : cov.out(b0);
+    double* dval = val.out(b0);
     TB_TRY(with_kind(gp->kernel, [&](auto K) {
-      return launch_joint<decltype(K)::value>(gp, QT, blocks, smem, gp->sV.as<double>(), lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc,
-                                              jr, eps_dev, om, oc, dptr[2], oq, err);
+      return launch_joint<decltype(K)::value>(gp, rq, mode, A, xc, nbc, eps_dev, mu, cv, samples.out(b0), post_dev ? nullptr : dval,
+                                              err);
     }));
-    if (bei) {
-      bei_kernel<<<(unsigned)nbc, bei_warps * 32, smem_bei, st>>>(om, oc, q, eps_dev, rq.S, rq.eta, dptr[3], err);
+    if (bei && !rq.grad) {
+      bei_kernel<<<(unsigned)nbc, bei_warps * 32, tail_smem, st>>>(mu, cv, q, eps_dev, S, rq.eta, dval, err);
       TB_LAUNCHED();
       TB_CUDA(cudaGetLastError());
     }
-    for (auto& o : outs) TB_TRY(o.back(b0, nbc));
+    if (rq.grad) {
+      double* cmu = gp->sMisc.as<double>();
+      if (bei)
+        bei_backward_kernel<<<(unsigned)nbc, bei_warps * 32, tail_smem, st>>>(mu, cv, q, eps_dev, S, rq.eta, dval, cmu, cmu + mc,
+                                                                              bsbar.as<double>(), err);
+      else
+        qei_backward_kernel<<<(unsigned)((nbc + QEIG_WARPS - 1) / QEIG_WARPS), QEIG_WARPS * 32, tail_smem, st>>>(
+            mu, cv, nbc, q, eps_dev, S, rq.eta, rq.jitter, dval, cmu, cmu + mc, bsbar.as<double>(), err);
+      TB_LAUNCHED();
+      qei_mix_kernel<<<dim3((unsigned)nbc, (unsigned)((gp->N + 255) / 256)), 256, 0, st>>>(gp->sV.as<double>(), lda, (int)gp->N, q,
+                                                                                          bsbar.as<double>());
+      TB_LAUNCHED();
+      double* gd = grad.out(b0);
+      TB_TRY(launch_grad(gp, xc, mc, gd));
+      TB_TRY(launch_qei_cross(gp, xc, mc, q, bsbar.as<double>(), gd));
+    }
+    for (auto* o : outs) TB_TRY(o->back(b0, nbc));
   }
   int herr = 0;
   TB_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2279,29 +2361,8 @@ static int run_sample_joint(tb_gp* gp, const double* Xc, int64_t M, const double
   // blocked Cholesky of the covariance with the cache-build kernels (factor.cuh)
   const int nbk = (int)((M + fac::FB - 1) / fac::FB);
   TB_TRY(bdinv.reserve(sizeof(double) * (size_t)nbk * fac::FB * fac::FB));
-  TB_TRY(gp->dInfo.reserve(sizeof(int)));
-  TB_CUDA(cudaMemsetAsync(gp->dInfo.p, 0, sizeof(int), st));
-  {
-    double* C = bcov.as<double>();
-    const size_t diag_smem = sizeof(double) * fac::FB * (fac::FB + 1);
-    for (int jb = 0; jb < nbk; ++jb) {
-      const int j0 = jb * fac::FB;
-      fac::chol_diag_kernel<<<1, fac::THREADS, diag_smem, st>>>(C, M, j0, bdinv.as<double>(), gp->dInfo.as<int>());
-      TB_LAUNCHED();
-      const int64_t below = M - (int64_t)(j0 + fac::FB);
-      if (below > 0) {
-        const unsigned t = (unsigned)((below + fac::FB - 1) / fac::FB);
-        fac::chol_panel_kernel<<<t, fac::THREADS, fac::GEMM_SMEM, st>>>(C, M, j0, bdinv.as<double>());
-        TB_LAUNCHED();
-        fac::chol_syrk_kernel<<<dim3(t, t), fac::THREADS, fac::GEMM_SMEM, st>>>(C, M, j0);
-        TB_LAUNCHED();
-      }
-    }
-  }
-  int info = 0;
-  TB_CUDA(cudaMemcpyAsync(&info, gp->dInfo.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  TB_CUDA(cudaStreamSynchronize(st));
-  TB_CUDA(cudaGetLastError());
+  int info;
+  TB_TRY(blocked_cholesky(gp, bcov.as<double>(), M, bdinv.as<double>(), &info));
   TB_CHECK_CODE(info == 0, "Cholesky decomposition was not successful. The input might not be valid "
                       "(joint covariance + jitter*I is not positive definite at leading minor " + std::to_string(info) + ")", tb::ERR_NUMERIC);
   // samples = mean + L z
@@ -2322,134 +2383,6 @@ static int run_sample_joint(tb_gp* gp, const double* Xc, int64_t M, const double
   return 0;
 }
 
-// ---- value AND gradient of a batch acquisition of the joint posterior ----
-// chunk pipeline: K* digits -> A = Linv K* (stored) -> per-batch mean / cov (joint_kernel) -> the tail's reverse kernel
-// (value, G_mu, Sigma_bar) -> V = K^-1 K* (dense digit GEMM over the same K* digits) -> per-batch mix V~ = Sigma_bar V
-// -> grad_kernel (the training-point sums) -> qei_cross_kernel (the K(x_b, x_b) term).  Tails:
-//   QEI_TAIL_MC   qei_backward_kernel: batch Monte-Carlo EI (function.py:1181-1186), eps [q, S] normal base samples
-//   QEI_TAIL_GENZ bei_backward_kernel: batch EI (function.py:1747-1805), eps = the Sobol points w [q-1, S]
-static int launch_qei_cross(tb_gp* gp, const double* xc, int64_t npts, int q, const double* sbar, double* grad) {
-  with_kind(gp->kernel, [&](auto K) {
-    qei_cross_kernel<decltype(K)::value><<<(unsigned)((npts + 127) / 128), 128, 0, gp->stream>>>(xc, gp->dInvLs.as<double>(), gp->D, npts,
-                                                                                                 q, sbar, gp->variance, grad);
-  });
-  TB_LAUNCHED();
-  TB_CUDA(cudaGetLastError());
-  return 0;
-}
-
-enum { QEI_TAIL_MC = 0, QEI_TAIL_GENZ = 1 };
-
-static int run_qei_grad(tb_gp* gp, const double* Xc, int64_t B, int q, const double* eps, int S, double eta, double jitter,
-                        double* out_val, double* out_grad, int tail = QEI_TAIL_MC) {
-  const bool genz = tail == QEI_TAIL_GENZ;
-  const int eps_rows = genz ? q - 1 : q;
-  if (B == 0) return 0;
-  TB_CUDA(cudaSetDevice(gp->device));
-  cudaStream_t st = gp->stream;
-  const int D = gp->D;
-  const int QT = (q + 7) / 8, QP = QT * 8;
-  const int64_t lda = (int64_t)gp->NB * BM;
-  Engine e;
-  TB_TRY(select_engine(gp, true, &e));
-  const int nt = eng_tile_width(gp, e);
-  const int64_t max_tiles = chunk_tiles(gp);
-  int64_t nbc_cap = std::min<int64_t>(std::max<int64_t>(1, (max_tiles * BT) / q), B);
-  const int64_t cand_cap = nbc_cap * q;
-  const int64_t tiles_cap = (cand_cap + nt - 1) / nt;
-  tb::DevBuf baplain;  // fp64 engine: plain copy of A for the Gram kernel (sA holds the packed panels the upper GEMM reads)
-  TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
-  if (e != Engine::F64) {
-    TB_TRY(gp->sA.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // A plain
-  } else {
-    TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));  // A packed
-    TB_TRY(baplain.reserve((size_t)tiles_cap * BT * lda * sizeof(double)));
-    TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)gp->NB * tiles_cap * BT));
-  }
-  TB_TRY(gp->sV.reserve((size_t)tiles_cap * nt * lda * sizeof(double)));  // V plain
-  TB_TRY(gp->sMean.reserve(sizeof(double) * tiles_cap * nt));
-  TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * cand_cap));  // c_mu, c_var
-  tb::DevBuf beps, bcov, bmu, bsbar, bval;
-  const Staged<const double> xin(Xc, (int64_t)q * D, gp->sXc, st), eps_in(eps, (int64_t)eps_rows * S, beps, st);
-  const Staged<double> vals(out_val, 1, bval, st), grads(out_grad, (int64_t)q * D, gp->sGrad, st);
-  TB_TRY(xin.reserve(nbc_cap));
-  TB_TRY(grads.reserve(nbc_cap));
-  const double* eps_dev;
-  TB_TRY(eps_in.reserve(1));
-  TB_TRY(eps_in.in(0, 1, &eps_dev));
-  TB_TRY(bcov.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
-  TB_TRY(bsbar.reserve(sizeof(double) * (size_t)nbc_cap * q * q));
-  TB_TRY(bmu.reserve(sizeof(double) * (size_t)cand_cap));
-  TB_TRY(vals.reserve(nbc_cap));
-  TB_TRY(gp->sRun.reserve(16));
-  int* err = reinterpret_cast<int*>(gp->sRun.p);
-  TB_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
-  const size_t smem_joint = (size_t)JOINT_WARPS * (QP * QP + QP * D + QP) * sizeof(double);
-  size_t smem_back;
-  int bei_warps = 0;
-  if (genz) {
-    // as many warps (up to 4) as fit: one per unit CDF in flight, each with its per-sample state in shared memory
-    const size_t cta = bei_cta_doubles(q) * sizeof(double), per_warp = bei_back_warp_doubles(q) * sizeof(double);
-    bei_warps = (int)std::min<size_t>(std::min<size_t>(BEI_MAX_WARPS, q + q * q), (227 * 1024 - cta) / per_warp);
-    smem_back = cta + bei_warps * per_warp;
-    TB_CUDA(cudaFuncSetAttribute(bei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_back));
-  } else {
-    smem_back = (size_t)QEIG_WARPS * (3 * q * q + 2 * q) * sizeof(double);
-    TB_CUDA(cudaFuncSetAttribute(qei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_back));
-  }
-  JointRequest jr;
-  jr.mode = JOINT_PREDICT;
-  jr.q = q;
-
-  for (int64_t b0 = 0; b0 < B; b0 += nbc_cap) {
-    const int64_t nbc = std::min<int64_t>(nbc_cap, B - b0);
-    const int64_t mc = nbc * q;
-    const int tiles = (int)((mc + nt - 1) / nt);
-    const int64_t McPad = (int64_t)tiles * nt;
-    const double* xc_chunk;
-    TB_TRY(xin.in(b0, nbc, &xc_chunk));
-    // fp64 engine: A twice (plain for the Gram kernel, packed panels for its V GEMM); int8 engines: A plain in sA
-    double* a_plain = e == Engine::F64 ? baplain.as<double>() : gp->sA.as<double>();
-    TB_TRY(eng_kstar(gp, e, xc_chunk, mc, tiles));
-    TB_TRY(eng_store_a(gp, e, tiles, McPad, a_plain));
-    if (e == Engine::F64) TB_TRY(eng_variance(gp, e, tiles, eng_groups(gp, e, tiles), McPad, true));
-    TB_TRY(eng_store_v(gp, e, tiles, McPad));
-    const int jblocks = (int)((nbc + JOINT_WARPS - 1) / JOINT_WARPS);
-    const int Nrows = (int)lda;
-    double* dmu = bmu.as<double>();
-    double* dcov = bcov.as<double>();
-    TB_TRY(with_kind(gp->kernel, [&](auto K) {
-      return launch_joint<decltype(K)::value>(gp, QT, jblocks, smem_joint, a_plain, lda, Nrows, gp->sMean.as<double>(), xc_chunk, nbc, jr,
-                                              nullptr, dmu, dcov, nullptr, nullptr, err);
-    }));
-    double* cmu = gp->sMisc.as<double>();
-    double* dval = vals.out(b0);
-    if (genz) {
-      bei_backward_kernel<<<(unsigned)nbc, bei_warps * 32, smem_back, st>>>(dmu, dcov, q, eps_dev, S, eta, dval, cmu, cmu + mc,
-                                                                           bsbar.as<double>(), err);
-    } else {
-      qei_backward_kernel<<<(unsigned)((nbc + QEIG_WARPS - 1) / QEIG_WARPS), QEIG_WARPS * 32, smem_back, st>>>(
-          dmu, dcov, nbc, q, eps_dev, S, eta, jitter, dval, cmu, cmu + mc, bsbar.as<double>(), err);
-    }
-    TB_LAUNCHED();
-    qei_mix_kernel<<<dim3((unsigned)nbc, (unsigned)((gp->N + 255) / 256)), 256, 0, st>>>(gp->sV.as<double>(), lda, (int)gp->N, q,
-                                                                                        bsbar.as<double>());
-    TB_LAUNCHED();
-    double* gd = grads.out(b0);
-    TB_TRY(launch_grad(gp, xc_chunk, mc, gd));
-    TB_TRY(launch_qei_cross(gp, xc_chunk, mc, q, bsbar.as<double>(), gd));
-    TB_TRY(vals.back(b0, nbc));
-    TB_TRY(grads.back(b0, nbc));
-  }
-  int herr = 0;
-  TB_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
-  TB_CUDA(cudaStreamSynchronize(st));
-  TB_CUDA(cudaGetLastError());
-  TB_CHECK_CODE(herr == 0, "Cholesky decomposition was not successful. The input might not be valid "
-                      "(covariance + jitter*I of a query batch is not positive definite)", tb::ERR_NUMERIC);
-  return 0;
-}
-
 }  // namespace tb
 
 extern "C" {
@@ -2457,15 +2390,12 @@ extern "C" {
 int tb_gp_predict_joint(tb_gp* gp, const void* Xc, int64_t B, int q, void* mean, void* cov) {
   TB_CHECK(gp && (B == 0 || (Xc && mean && cov)), "tb_gp_predict_joint: null argument");
   TB_TRY(tb::check_batch(gp, B, q, false, 0, nullptr, 0.0));
-  tb::JointRequest rq;
-  rq.mode = JOINT_PREDICT;
-  rq.B = B;
-  rq.q = q;
+  tb::BatchRequest rq(tb::BatchTail::Predict, B, q);
   tb::DtypeBridge br(gp);
   TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
   TB_TRY(br.out(mean, B * q, &rq.out_mean));
   TB_TRY(br.out(cov, B * q * q, &rq.out_cov));
-  TB_TRY(tb::run_joint(gp, rq));
+  TB_TRY(tb::run_batch(gp, rq));
   return br.finish();
 }
 
@@ -2473,35 +2403,24 @@ int tb_acq_batch_mc_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const void* 
                        void* out) {
   TB_CHECK(gp && (B == 0 || (Xc && eps && out)), "tb_acq_batch_mc_ei: null argument");
   TB_TRY(tb::check_batch(gp, B, q, true, S, eps, jitter));
-  tb::JointRequest rq;
-  rq.mode = JOINT_QEI;
-  rq.B = B;
-  rq.q = q;
-  rq.S = S;
-  rq.eta = eta;
-  rq.jitter = jitter;
+  tb::BatchRequest rq(tb::BatchTail::McEi, B, q, S, eta, jitter);
   tb::DtypeBridge br(gp);
   TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
   TB_TRY(br.in(eps, (int64_t)q * S, &rq.eps));
-  TB_TRY(br.out(out, B, &rq.out_qei));
-  TB_TRY(tb::run_joint(gp, rq));
+  TB_TRY(br.out(out, B, &rq.out_val));
+  TB_TRY(tb::run_batch(gp, rq));
   return br.finish();
 }
 
 int tb_gp_reparam_sample(tb_gp* gp, const void* Xc, int64_t B, int q, const void* eps, int S, double jitter, void* samples) {
   TB_CHECK(gp && (B == 0 || (Xc && eps && samples)), "tb_gp_reparam_sample: null argument");
   TB_TRY(tb::check_batch(gp, B, q, true, S, eps, jitter));
-  tb::JointRequest rq;
-  rq.mode = JOINT_SAMPLE;
-  rq.B = B;
-  rq.q = q;
-  rq.S = S;
-  rq.jitter = jitter;
+  tb::BatchRequest rq(tb::BatchTail::Samples, B, q, S, 0.0, jitter);
   tb::DtypeBridge br(gp);
   TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
   TB_TRY(br.in(eps, (int64_t)q * S, &rq.eps));
   TB_TRY(br.out(samples, B * S * q, &rq.out_samples));
-  TB_TRY(tb::run_joint(gp, rq));
+  TB_TRY(tb::run_batch(gp, rq));
   return br.finish();
 }
 
@@ -2936,14 +2855,14 @@ int tb_acq_batch_mc_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const v
                             void* out, void* grad) {
   TB_CHECK(gp && (B == 0 || (Xc && eps && out && grad)), "tb_acq_batch_mc_ei_grad: null argument");
   TB_TRY(tb::check_batch(gp, B, q, true, S, eps, jitter));
+  tb::BatchRequest rq(tb::BatchTail::McEi, B, q, S, eta, jitter);
+  rq.grad = true;
   tb::DtypeBridge br(gp);
-  const double *xd, *ed;
-  double *od, *gd;
-  TB_TRY(br.in(Xc, B * q * gp->D, &xd));
-  TB_TRY(br.in(eps, (int64_t)q * S, &ed));
-  TB_TRY(br.out(out, B, &od));
-  TB_TRY(br.out(grad, B * q * gp->D, &gd));
-  TB_TRY(tb::run_qei_grad(gp, xd, B, q, ed, S, eta, jitter, od, gd));
+  TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
+  TB_TRY(br.in(eps, (int64_t)q * S, &rq.eps));
+  TB_TRY(br.out(out, B, &rq.out_val));
+  TB_TRY(br.out(grad, B * q * gp->D, &rq.out_grad));
+  TB_TRY(tb::run_batch(gp, rq));
   return br.finish();
 }
 
@@ -2961,17 +2880,12 @@ static int bei_args(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w
 int tb_acq_batch_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w, int S, double eta, void* out) {
   TB_TRY(bei_args(gp, Xc, B, q, w, S, out, nullptr, false, "tb_acq_batch_ei"));
   if (B == 0) return 0;
-  tb::JointRequest rq;
-  rq.mode = tb::JOINT_BEI;
-  rq.B = B;
-  rq.q = q;
+  tb::BatchRequest rq(tb::BatchTail::BatchEi, B, q, S, eta);
   rq.eps = w;
-  rq.S = S;
-  rq.eta = eta;
   tb::DtypeBridge br(gp);
   TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
-  TB_TRY(br.out(out, B, &rq.out_qei));
-  TB_TRY(tb::run_joint(gp, rq));
+  TB_TRY(br.out(out, B, &rq.out_val));
+  TB_TRY(tb::run_batch(gp, rq));
   return br.finish();
 }
 
@@ -2979,13 +2893,14 @@ int tb_acq_batch_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const doub
                          void* grad) {
   TB_TRY(bei_args(gp, Xc, B, q, w, S, out, grad, true, "tb_acq_batch_ei_grad"));
   if (B == 0) return 0;
+  tb::BatchRequest rq(tb::BatchTail::BatchEi, B, q, S, eta);
+  rq.grad = true;
+  rq.eps = w;
   tb::DtypeBridge br(gp);
-  const double* xd;
-  double *od, *gd;
-  TB_TRY(br.in(Xc, B * q * gp->D, &xd));
-  TB_TRY(br.out(out, B, &od));
-  TB_TRY(br.out(grad, B * q * gp->D, &gd));
-  TB_TRY(tb::run_qei_grad(gp, xd, B, q, w, S, eta, 0.0, od, gd, tb::QEI_TAIL_GENZ));
+  TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
+  TB_TRY(br.out(out, B, &rq.out_val));
+  TB_TRY(br.out(grad, B * q * gp->D, &rq.out_grad));
+  TB_TRY(tb::run_batch(gp, rq));
   return br.finish();
 }
 
