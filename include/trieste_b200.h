@@ -247,7 +247,7 @@ void tb_launch_count_reset(void);
 /* engine of the variance GEMM: 0 = native fp64 (DMMA), 1 = fp64-accurate emulation on the INT8 tensor cores
  * (Ozaki splitting, wgmma s8; same stated tolerances; N <= 16384, larger models fall back to engine 0), 2 = engine 1
  * with the number of digit products pinned to the full 21 (engine 1 drops to 15 — fp32 handles: 6 — when the a-priori error
- * estimate of the cache allows it; csrc/ozaki5.cuh).  The
+ * estimate of the cache allows it; csrc/int8_engines.cu, csrc/ozaki5.cuh).  The
  * engine serves every path: predict / acquisition values, gradients (V = K^-1 k* as a dense digit GEMM) and the joint
  * paths (predict_joint / reparam samples / MC-qEI through the store-A epilogue). */
 int tb_gp_set_engine(tb_gp* gp, int engine);

@@ -1,16 +1,16 @@
-"""CPU emulation of the single-pass digit engine (trieste_b200/csrc/ozaki5.cuh, oz5_api.cu) — TEST INFRASTRUCTURE.
+"""CPU emulation of the single-pass digit engine (trieste_b200/csrc/ozaki5.cuh, ozaki.cuh, int8_engines.cu) — TEST INFRASTRUCTURE.
 
 The int8 tensor-core engine evaluates the fp64 product ``A = Linv · K*`` as exact integer digit GEMMs.  Everything it does is
 integer arithmetic on balanced base-256 digits plus a handful of fp64 operations in the epilogue, so NumPy can replay it
 exactly on the CPU (digit products of K <= 16384 terms stay below 2^31, far inside fp64's 2^53 exact-integer range):
 
-  * ``tight_row_scales``      ozaki5.cuh ``linv_rowstats_kernel``: rowscale[n] = max_k |Linv[n,k]| / FILL, rowsum[n]
-  * ``balanced_digits``       ozaki5.cuh ``digit_bytes`` / ``linv_digits_kernel``: v = rint(x / scale · 2^(8S)) = Σ_p d_p 256^(S-p)
+  * ``tight_row_scales``      ozaki.cuh ``rowstats_kernel`` (tight split): rowscale[n] = max_k |Linv[n,k]| / FILL, rowsum[n]
+  * ``balanced_digits``       ozaki.cuh ``digit_bytes`` / ``digits_kernel``: v = rint(x / scale · 2^(8S)) = Σ_p d_p 256^(S-p)
   * ``digit_bytes``           the carry-free byte trick ``(v + 0x80..80) ^ 0x80..80`` the kernels use to cut the digits
-  * ``centred_kstar_digits``  ozaki5.cuh ``kstar_digits_kernel`` + oz5_api.cu ``oz5_centre_int / oz5_h_eff``: integer centre
-  * ``digit_gemm``            ozaki5.cuh ``issue_stage`` (pairs p + q <= R share the level accumulator T_{p+q}) and the
-                              epilogue of ``trigemm_kernel`` (Horner over the levels, row scale, row-sum term)
-  * ``apriori_estimate``      oz5_api.cu ``oz5_estimate``: the admission test of the 15-product mode
+  * ``centred_kstar_digits``  ozaki5.cuh ``kstar_digits_kernel`` + int8_engines.cu ``centre_int / h_eff``: integer centre
+  * ``digit_gemm``            digit_gemm.cuh ``digit_gemm_kernel`` (pairs p + q <= R share the level accumulator T_{p+q}) and
+                              its epilogue (Horner over the levels, row scale, row-sum term)
+  * ``apriori_estimate``      int8_engines.cu ``single_pass_estimate``: the admission test of the 15-product mode
 
 It is how the error budget of DESIGN.md §4c was established (tools/digit_error_study.py regenerates that table) and it lets the
 CPU suite pin the budget without a GPU (tests/test_digit_emulation.py).  Nothing in the product imports this module."""
@@ -20,7 +20,7 @@ import math
 
 import numpy as np
 
-FILL = 0.4975  # ozaki5.cuh: |x̂| bound (the largest 5-digit balanced value is 0.49804)
+FILL = 0.4975  # ozaki.cuh: |x̂| bound (the largest 5-digit balanced value is 0.49804)
 
 
 def tight_row_scales(Linv: np.ndarray):
@@ -97,7 +97,7 @@ def digit_gemm(Linv: np.ndarray, Ks: np.ndarray, variance: float, SA: int = 5, S
 
 
 def apriori_estimate(variance: float, max_rowscale: float, N: int, S: int) -> float:
-    """oz5_api.cu ``oz5_estimate``: max |Δvar| / σ_f² when the levels r > S + 1 are dropped."""
+    """int8_engines.cu ``single_pass_estimate``: max |Δvar| / σ_f² when the levels r > S + 1 are dropped."""
     sB = 0.5 * variance / FILL
     return 1.6 * math.sqrt(variance) * max_rowscale * sB * math.sqrt(6.0 * N) * (65536.0 / 12.0) * 2.0 ** (-8 * (S + 2)) / variance
 

@@ -15,7 +15,7 @@ def _grown(objective, N0, m, D, kind="matern52", dtype=np.float64):
     return head, full
 
 
-@pytest.mark.parametrize("engine", ["int8", "fp64"])
+@pytest.mark.parametrize("engine", ["int8", "int8x21", "fp64"])
 @pytest.mark.parametrize("N0,m", [(1, 1), (127, 1), (127, 2), (128, 1), (300, 5), (250, 64), (1000, 8)])
 def test_append_matches_from_scratch_cache(N0, m, engine):
     import trieste_b200 as tb
@@ -57,7 +57,7 @@ def test_repeated_single_appends_track_the_oracle_and_gradients_follow():
     np.testing.assert_allclose(cj, ocj, rtol=0, atol=1e-9 * full.variance)
 
 
-@pytest.mark.parametrize("engine", ["int8", "fp64"])
+@pytest.mark.parametrize("engine", ["int8", "int8x21", "fp64"])
 def test_gradients_between_appends_use_the_rank_m_update_of_the_inverse(engine):
     """A BO loop with a gradient-based optimiser asks for gradients after EVERY append: the dense K^-1 behind the int8
     engine's gradient GEMM is grown by rank m with the factor (O(m N^2)) instead of being rebuilt (O(N^3))."""
@@ -78,6 +78,39 @@ def test_gradients_between_appends_use_the_rank_m_update_of_the_inverse(engine):
         oval, ograd = o.ei_gradient(ref, Xq, eta)
         np.testing.assert_allclose(val.reshape(-1), oval.reshape(-1), rtol=1e-6, atol=1e-15)
         np.testing.assert_allclose(grad.reshape(-1, 6), ograd, rtol=1e-6, atol=1e-12)
+
+
+def test_engine_toggles_between_appends_keep_every_result_bit_for_bit():
+    """Every operand derived from the posterior cache records the cache generation it was built from.  A handle that toggles
+    between the int8 engines around appends gives bit for bit what handles that never toggle give."""
+    import trieste_b200 as tb
+    from trieste_b200.acquisition import expected_improvement
+
+    head, full = _grown(o.hartmann_6, 250, 9, 6)
+    eta = o.ei_eta(head)
+    Xq = candidates(300, 6)
+
+    def run(nm):
+        val, grad = expected_improvement(nm, eta).value_and_gradient(Xq[:, None, :])
+        return np.concatenate([a.reshape(-1) for a in (val, grad, *nm.predict(Xq))])
+
+    toggled, single, full21 = (native_from_oracle(head) for _ in range(3))
+    full21.set_engine("int8x21")
+    first = run(toggled)
+    toggled.set_engine("int8x21")
+    np.testing.assert_array_equal(run(toggled), run(full21))
+    toggled.set_engine("int8")
+    np.testing.assert_array_equal(run(toggled), first)
+    for n in (251, 255, 259):  # appends of 1, 4 and 4 rows
+        for nm in (toggled, single, full21):
+            nm.update(tb.Dataset(full.X[:n], full.y[:n]))
+            assert nm.last_update_appended
+        ref = run(single)
+        np.testing.assert_array_equal(run(toggled), ref)
+        toggled.set_engine("int8x21")
+        np.testing.assert_array_equal(run(toggled), run(full21))
+        toggled.set_engine("int8")
+        np.testing.assert_array_equal(run(toggled), ref)
 
 
 def test_update_falls_back_to_a_full_refresh_when_it_is_not_an_append():

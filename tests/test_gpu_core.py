@@ -256,6 +256,14 @@ def test_single_candidate_and_single_training_point():
     assert idx == 0 and best == o.expected_improvement(omean, ovar, o.ei_eta(om))[0, 0] or abs(best - o.expected_improvement(omean, ovar, o.ei_eta(om))[0, 0]) < 1e-12
 
 
+def test_engine_reports_the_handle_default_until_set_engine(monkeypatch):
+    monkeypatch.setenv("TB_ENGINE", "fp64")  # not a knob of the library: it must not change what is reported
+    om, nm = model_pair(o.branin, 20, 2)
+    assert nm.engine == "int8" and nm.engine_info()[0] > 0
+    nm.set_engine("fp64")
+    assert nm.engine == "fp64" and nm.engine_info()[0] == 0
+
+
 def test_large_model_falls_back_to_fp64_engine():
     # the int8 engine's int32 accumulators are exact up to N = 16384; beyond that the native fp64 engine takes over
     om, nm = model_pair(o.hartmann_6, 16500, 6)

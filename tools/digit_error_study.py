@@ -42,4 +42,4 @@ for name, kw in rows:
     mx, rms, n = de.variance_error(Linv, Ks, var, **kw)
     print(f"| {name} | {n} | {mx:.2e} | {rms:.2e} |")
 for S in (5, 4, 3):
-    print(f"a-priori estimate (oz5_estimate) for S = {S}: {de.apriori_estimate(var, de.tight_row_scales(Linv)[0].max(), N, S):.2e}")
+    print(f"a-priori estimate (single_pass_estimate) for S = {S}: {de.apriori_estimate(var, de.tight_row_scales(Linv)[0].max(), N, S):.2e}")

@@ -52,6 +52,29 @@ struct DevBuf {
   T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+// State derived from the posterior cache records the cache_gen it was built from (tb_gp::cache_gen); it is current when the
+// two are equal.
+constexpr uint64_t STALE = ~(uint64_t)0;
+
+// One left operand of the digit GEMM (Linv or the dense K^-1): digit planes in the GEMM's stage layout, per-row scales, and
+// per-row sums (the single-pass engine's centring term; empty for the 21-product engine).
+struct DigitOperand {
+  DevBuf digits, scale, sum;
+  int planes = 0;        // digit planes stored per stage; 0: the single-pass engine was not admitted for this operand
+  uint64_t gen = STALE;  // cache_gen the operand was built from
+};
+
+// The int8 engines' state (int8_engines.cu owns it): both engines' Linv and K^-1 operands stay alive together, so one handle
+// can run single-pass values and 21-product gradients when the V estimate refuses the single-pass split.
+struct DigitState {
+  DigitOperand linv21, kinv21;  // 21-product engine: 6 planes, power-of-two row scales
+  DigitOperand linv, kinv;      // single-pass engine: tight row scales and row sums; linv.gen also stamps the admission below
+  DevBuf X2;                    // squared row norms of the scaled training inputs (centred K* generation)
+  bool full = false;            // tb_gp_set_engine(2): always the 21-product engine
+  int mode = 0;                 // digits the single-pass variance GEMM computes with (0: not admitted)
+  double est = 0.0;             // a-priori estimate of max |Δvar| / σ_f² in that mode
+};
+
 inline bool is_device_ptr(const void* p) {
   if (!p) return false;
   cudaPointerAttributes a;
@@ -167,30 +190,14 @@ struct tb_gp {
   tb::DevBuf dLinv;             // [N,N] column-major Linv (kept: predict_joint / gradients reuse it)
   tb::DevBuf dLinvP;            // packed lower panels
   tb::DevBuf dLinvTP;           // packed upper panels of Linv^T (lazy; gradient path)
-  bool upper_valid = false;
-  // int8 (Ozaki) engine: digit tiles of Linv, per-row scales, K* scale
+  uint64_t upper_gen = tb::STALE;
   int engine = 1;  // 0 = fp64 DMMA, 1 = int8 tensor cores (default; same stated tolerances, ~3x faster)
-  tb::DevBuf dAS, dRowScale;
-  tb::DevBuf dKinv, dKinvS, dKinvScale;  // gradient path of the int8 engine: digit tiles of K^-1 (full rows)
-  bool kinv_valid = false;       // digit tiles of K^-1 current
-  bool kinv_dense_valid = false; // dense K^-1 (dKinv, lower triangle, ld = kinv_dense_N) current: kept so that an append can
-  int64_t kinv_dense_N = 0;      // update it by rank m (tb_gp_append_data) instead of rebuilding it in O(N^3)
-  tb::DevBuf dKinvSpare;
-  tb::DevBuf sMeanPart;                // per-split mean partials of the k-split K* generation (few candidate tiles)
-  bool oz_valid = false;
-  int nst = 0, oz_bscale_exp = 0;
-  double oz_out_scale = 1.0;
-  // single-pass digit engine (ozaki5.cuh): tight row scales + row sums + S-digit tiles of Linv; mode = digits per operand
-  // (5: fp64 handles, 15 products; 3: fp32 handles, 6 products; 0: not eligible -> the 6-digit / 21-product kernels)
-  tb::DevBuf dAS5, dRowScale5, dRowSum5, dX2;
-  bool oz5_valid = false;
-  bool oz_full = false;  // tb_gp_set_engine(2): always the 6-digit / 21-product kernels
-  int oz5_mode = 0;
-  int oz5_planes = 0;    // digit planes stored per operand stage (5: fp64 handles; 4: fp32 handles, whose variance GEMM computes
-                         // with the 3 leading planes and whose store-A / V GEMMs use all 4)
-  double oz5_est = 0.0;  // a-priori estimate of max |Δvar| / σ_f² in the chosen mode
-  tb::DevBuf dKinvS5, dKinvScale5, dKinvSum5;  // tight digit tiles / row scales / row sums of the dense K^-1 (gradient path)
-  bool kinv5_valid = false, kinv5_ok = false;  // kinv5_ok: the V GEMM's own error estimate admits the single-pass engine
+  // dense K^-1 (lower triangle, ld = N) of the int8 engines' gradient path: an append grows it by rank m (tb_gp_append_data)
+  // instead of rebuilding it in O(N^3)
+  tb::DevBuf dKinv, dKinvSpare;
+  uint64_t kinv_gen = tb::STALE;
+  tb::DigitState digits;       // the int8 engines' digit operands (int8_engines.cu)
+  tb::DevBuf sMeanPart;        // per-split mean partials of the k-split K* generation (few candidate tiles)
   tb::DevBuf dWork, dInfo;      // cusolver workspace / info flag
   tb::DevBuf dDinv;             // inverses of the diagonal blocks of L (hand-written factorisation)
   bool factor_own = true;       // false (TB_FACTOR=cusolver): cuSOLVER / cuBLAS cross-check path
@@ -209,7 +216,7 @@ struct tb_gp {
   int gibM = 0, gibMp = 0, gibD = 0;
   double gibW = 0.0;
   uint64_t cache_gen = 0;               // bumped whenever the posterior cache is (re)built
-  uint64_t gib_gen = ~(uint64_t)0;      // cache_gen the derived GIBBON state was built for
+  uint64_t gib_gen = tb::STALE;         // cache_gen the derived GIBBON state was built for
   tb::DevBuf dGibPs, dGibLinv, dGibWhat;
   tb::DevBuf sGib;                      // per chunk: |u|^2 [mc], -w / V_det [mc], u [mp][mc] (gradient path)
   // screened argmax (tb_api.cu, argmax_screened): the screen bound ub of all M candidates, the survivors' coordinates / global
@@ -220,7 +227,7 @@ struct tb_gp {
   // fp32 rows [nst*64][W] of (x', |x'|^2, σ_f² α, |σ_f² α|); the centre [DP] subtracted from scaled inputs, and the constants
   // of the bound
   tb::DevBuf dPreRows, dPreCentre;
-  uint64_t pre_gen = ~(uint64_t)0;
+  uint64_t pre_gen = tb::STALE;
   bool pre_tc = false;
   int pre_nsl = 0, pre_npos_sl = 0;
   double pre_scale = 1.0, pre_x2max = 0.0, pre_rel = 0.0, pre_lin = 0.0, pre_lin_max = 0.0, pre_abs = 0.0;

@@ -1,6 +1,6 @@
 // Single-pass digit GEMM of the INT8 engine: fewer digit products, one pass.
 //
-// Same error-free splitting as ozaki.cuh, re-budgeted against the 1e-9·σ_f² variance bar:
+// Same error-free splitting and digit cutters as ozaki.cuh, re-budgeted against the 1e-9·σ_f² variance bar:
 //   * operands are scaled TIGHTLY (|x̂| <= 0.4975, arbitrary fp64 scale per row of Linv instead of a power of two with two
 //     spare bits) and K* is CENTRED: K* = h + K̃ with h = σ_f²/2, |K̃| <= h, so the sign bit of the top digit carries
 //     information;  A = Linv·K̃ + h·rowsum(Linv), the second term is a per-row constant added in the epilogue;
@@ -12,113 +12,19 @@
 // The K* digit tiles are NT candidates wide (192 for S = 5, 128 otherwise); the GEMM (digit_gemm.cuh) works on them in
 // column chunks of 64 candidates, whose S levels of int32 accumulators fit the registers of two consumer warpgroups.
 #pragma once
-#include "digit_gemm.cuh"
-#include "kernel_fn.cuh"
+#include "ozaki.cuh"
 
 namespace tb {
 namespace oz5 {
 
-using oz::ATILE;
+using oz::FILL;
+using oz::Geo;
 using oz::KST;
 using oz::LBO;
 using oz::SBO;
-constexpr double FILL = 0.4975;   // |x̂| bound: the largest 5-digit balanced value is 0.49804
+using oz::two_pow_8S;
 
-template <int S> struct Geo;
-template <> struct Geo<5> { static constexpr int NT = 192; };
-template <> struct Geo<4> { static constexpr int NT = 128; };
-template <> struct Geo<3> { static constexpr int NT = 128; };
-
-template <int S> __host__ __device__ constexpr int btile() { return Geo<S>::NT * KST; }
-template <int S> __host__ __device__ constexpr double two_pow_8S() { return S == 5 ? 1099511627776.0 : S == 4 ? 4294967296.0 : 16777216.0; }  // 2^40 / 2^32 / 2^24
-
-// v = Σ_{p=1..S} d_p 256^(S-p), d_p in [-128,127]: the int8 digits are the bytes of (v + 0x80..80) ^ 0x80..80 (no carry chain);
-// byte 0 = least significant digit d_S
-template <int S>
-__device__ __forceinline__ void digit_bytes(long long v, uint32_t& lo, uint32_t& hi) {
-  constexpr unsigned long long K = S == 5 ? 0x0000008080808080ULL : S == 4 ? 0x0000000080808080ULL : 0x0000000000808080ULL;
-  const unsigned long long w = ((unsigned long long)v + K) ^ K;
-  lo = (uint32_t)w;
-  hi = (uint32_t)(w >> 32);
-}
 template <int S> __host__ __device__ constexpr double dig_koff() { return S == 5 ? 551911719040.0 : S == 4 ? 2155905152.0 : 8421504.0; }  // 0x8080808080 / 0x80808080 / 0x808080
-// element JJ (0..15) of the lane's 16-byte rows: plane p (0 = most significant digit) takes byte S-1-p of the word
-template <int S, int JJ>
-__device__ __forceinline__ void scatter(uint32_t (&pk)[S][4], uint32_t lo, uint32_t hi) {
-#pragma unroll
-  for (int p = 0; p < S; ++p) {
-    const int b = S - 1 - p;
-    if (b >= 4) {
-      if (b == 4) pk[p][JJ >> 2] = oz::put_byte<JJ & 3, 0>(pk[p][JJ >> 2], hi);
-    } else if (b == 3) {
-      pk[p][JJ >> 2] = oz::put_byte<JJ & 3, 3>(pk[p][JJ >> 2], lo);
-    } else if (b == 2) {
-      pk[p][JJ >> 2] = oz::put_byte<JJ & 3, 2>(pk[p][JJ >> 2], lo);
-    } else if (b == 1) {
-      pk[p][JJ >> 2] = oz::put_byte<JJ & 3, 1>(pk[p][JJ >> 2], lo);
-    } else {
-      pk[p][JJ >> 2] = oz::put_byte<JJ & 3, 0>(pk[p][JJ >> 2], lo);
-    }
-  }
-}
-template <int S>
-__device__ __forceinline__ void scatter_rt(uint32_t (&pk)[S][4], int jj, uint32_t lo, uint32_t hi) {
-  switch (jj) {  // jj is a compile-time constant after unrolling
-    case 0: scatter<S, 0>(pk, lo, hi); break;
-    case 1: scatter<S, 1>(pk, lo, hi); break;
-    case 2: scatter<S, 2>(pk, lo, hi); break;
-    case 3: scatter<S, 3>(pk, lo, hi); break;
-    case 4: scatter<S, 4>(pk, lo, hi); break;
-    case 5: scatter<S, 5>(pk, lo, hi); break;
-    case 6: scatter<S, 6>(pk, lo, hi); break;
-    case 7: scatter<S, 7>(pk, lo, hi); break;
-    case 8: scatter<S, 8>(pk, lo, hi); break;
-    case 9: scatter<S, 9>(pk, lo, hi); break;
-    case 10: scatter<S, 10>(pk, lo, hi); break;
-    case 11: scatter<S, 11>(pk, lo, hi); break;
-    case 12: scatter<S, 12>(pk, lo, hi); break;
-    case 13: scatter<S, 13>(pk, lo, hi); break;
-    case 14: scatter<S, 14>(pk, lo, hi); break;
-    default: scatter<S, 15>(pk, lo, hi); break;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// once per BO step: tight row scales, row sums and digit tiles of Linv
-//   rowscale[n] = max_k |Linv[n,k]| / FILL   (1 for empty / padded rows),   rowsum[n] = Σ_k Linv[n,k]
-// ------------------------------------------------------------------------------------------------
-__global__ void linv_rowstats_kernel(const double* __restrict__ Linv, int64_t N, int64_t rows, double* __restrict__ rowscale,
-                                     double* __restrict__ rowsum) {
-  const int64_t n = blockIdx.x;
-  double mx = 0.0, sm = 0.0;
-  if (n < N)
-    for (int64_t k = threadIdx.x; k <= n; k += blockDim.x) {
-      const double v = Linv[n + k * N];
-      mx = fmax(mx, fabs(v));
-      sm += v;
-    }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    sm += __shfl_xor_sync(0xffffffffu, sm, o);
-  }
-  __shared__ double smx[8], ssm[8];
-  if ((threadIdx.x & 31) == 0) {
-    smx[threadIdx.x >> 5] = mx;
-    ssm[threadIdx.x >> 5] = sm;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
-      mx = fmax(mx, smx[w]);
-      sm += ssm[w];
-    }
-    if (n < rows) {
-      rowscale[n] = mx > 0.0 ? mx / FILL : 1.0;
-      rowsum[n] = sm;
-    }
-  }
-}
 
 // X2[k] = |Xs[k]|^2 for the rows that exist (Xs is [rows_have][DP], zero padded), 0 beyond
 __global__ void row_norms_kernel(const double* __restrict__ Xs, int64_t rows_have, int DP, int64_t rows, double* __restrict__ X2) {
@@ -128,82 +34,6 @@ __global__ void row_norms_kernel(const double* __restrict__ Xs, int64_t rows_hav
   if (k < rows_have)
     for (int d = 0; d < DP; ++d) s = fma(Xs[k * DP + d], Xs[k * DP + d], s);
   X2[k] = s;
-}
-
-template <int S>
-__global__ void linv_digits_kernel(const double* __restrict__ Linv, int64_t N, const double* __restrict__ rowscale,
-                                   int8_t* __restrict__ AS) {
-  const int I = blockIdx.y, kc = blockIdx.x;
-  if (kc >= 2 * (I + 1)) return;
-  int8_t* dst = AS + (oz::a_stage_offset(I) + kc) * (int64_t)(S * ATILE);
-  for (int e = threadIdx.x; e < 128 * KST; e += blockDim.x) {
-    const int r = e % 128, kin = e / 128;  // r fastest: column-major source is contiguous in n
-    const int64_t n = (int64_t)I * 128 + r, k = (int64_t)kc * KST + kin;
-    long long v = 0;
-    if (n < N && k <= n) v = __double2ll_rn(Linv[n + k * N] / rowscale[n] * two_pow_8S<S>());
-    uint32_t lo, hi;
-    digit_bytes<S>(v, lo, hi);
-    const unsigned long long w = ((unsigned long long)hi << 32) | lo;
-    const int off = (r >> 3) * SBO + (kin >> 4) * LBO + (r & 7) * 16 + (kin & 15);
-#pragma unroll
-    for (int p = 0; p < S; ++p) dst[p * ATILE + off] = (int8_t)((w >> (8 * (S - 1 - p))) & 0xff);
-  }
-}
-
-// K^-1 (gradient path): symmetric, given by its lower triangle (column-major, ld = N); full rows, same tight scaling and
-// row sums as for Linv:  V = K^-1 k* = K^-1 K~ + h rowsum(K^-1)
-__device__ __forceinline__ double sym_lower_at(const double* __restrict__ A, int64_t N, int64_t n, int64_t k) {
-  return n >= k ? A[n + k * N] : A[k + n * N];
-}
-__global__ void sym_rowstats_kernel(const double* __restrict__ A, int64_t N, int64_t rows, double* __restrict__ rowscale,
-                                    double* __restrict__ rowsum) {
-  const int64_t n = blockIdx.x;
-  double mx = 0.0, sm = 0.0;
-  if (n < N)
-    for (int64_t k = threadIdx.x; k < N; k += blockDim.x) {
-      const double v = sym_lower_at(A, N, n, k);
-      mx = fmax(mx, fabs(v));
-      sm += v;
-    }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    sm += __shfl_xor_sync(0xffffffffu, sm, o);
-  }
-  __shared__ double smx[8], ssm[8];
-  if ((threadIdx.x & 31) == 0) {
-    smx[threadIdx.x >> 5] = mx;
-    ssm[threadIdx.x >> 5] = sm;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
-      mx = fmax(mx, smx[w]);
-      sm += ssm[w];
-    }
-    if (n < rows) {
-      rowscale[n] = mx > 0.0 ? mx / FILL : 1.0;
-      rowsum[n] = sm;
-    }
-  }
-}
-template <int S>
-__global__ void sym_digits_kernel(const double* __restrict__ A, int64_t N, int nst, const double* __restrict__ rowscale,
-                                  int8_t* __restrict__ AS) {
-  const int I = blockIdx.y, kc = blockIdx.x;
-  int8_t* dst = AS + ((int64_t)I * nst + kc) * (int64_t)(S * ATILE);
-  for (int e = threadIdx.x; e < 128 * KST; e += blockDim.x) {
-    const int r = e % 128, kin = e / 128;
-    const int64_t n = (int64_t)I * 128 + r, k = (int64_t)kc * KST + kin;
-    long long v = 0;
-    if (n < N && k < N) v = __double2ll_rn(sym_lower_at(A, N, n, k) / rowscale[n] * two_pow_8S<S>());
-    uint32_t lo, hi;
-    digit_bytes<S>(v, lo, hi);
-    const unsigned long long w = ((unsigned long long)hi << 32) | lo;
-    const int off = (r >> 3) * SBO + (kin >> 4) * LBO + (r & 7) * 16 + (kin & 15);
-#pragma unroll
-    for (int p = 0; p < S; ++p) dst[p * ATILE + off] = (int8_t)((w >> (8 * (S - 1 - p))) & 0xff);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -322,7 +152,7 @@ kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2
       macc = fma(kval, al_s[buf][kv], macc);
       const double tb = fma(kval, inv_bscale_2p, dig_c);
       const uint32_t wl = (uint32_t)__double2loint(tb) ^ 0x80808080u, wh = (uint32_t)__double2hiint(tb) ^ 0x80u;
-      scatter_rt<S>(pk, j, wl, wh);
+      oz::scatter_rt<S>(pk, j, wl, wh);
     }
     if (tile_id < ntiles) {
 #pragma unroll
@@ -346,9 +176,6 @@ __global__ void mean_reduce_kernel(const double* __restrict__ part, int ksplit, 
   for (int i = 0; i < ksplit; ++i) s += part[(int64_t)i * stride + t];
   mean_out[t] = s + mean_const;
 }
-
-// the GEMM of this engine: the shared digit GEMM on NT-wide candidate tiles
-enum { EPI_SUMSQ = dg::EPI_SUMSQ, EPI_STORE = dg::EPI_STORE };
 
 }  // namespace oz5
 }  // namespace tb

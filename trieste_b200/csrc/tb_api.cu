@@ -4,8 +4,7 @@
 #include "kernels_extra.cuh"
 #include "prescreen.cuh"
 #include "batch_ei.cuh"
-#include "ozaki.cuh"
-#include "oz5_api.h"
+#include "int8_engines.h"
 #include <chrono>
 #include "factor.cuh"
 #include "lbfgs.cuh"
@@ -224,8 +223,8 @@ __global__ void colmajor_lower_to_rowmajor_kernel(const double* __restrict__ A, 
 // =================================================================================================
 // dtype bridge.  TB_F32 handles (fp32 models, e.g. BASELINE config 5) take and return float arrays: whole inputs are widened
 // to device doubles and outputs narrowed back.  Their posterior cache is fp64.  select_engine runs their candidate GEMMs on
-// the int8 engines with fewer digits than an fp64 handle gets: the single-pass engine with the fewest digits oz5_ensure
-// admits (3 digits / 6 products, 4 / 10 or 5 / 15), else the leading pass (10 products) of the 21-product engine.
+// the int8 engines with fewer digits than an fp64 handle gets: the single-pass engine with the fewest digits int8_select
+// admits (3 digits / 6 products, 4 / 10 or 5 / 15), else the 4 leading planes (10 products) of the 21-product engine.
 // Above N = 16384 and on engine 0 they run the fp64 DMMA kernels, as fp64 handles do.
 // =================================================================================================
 __global__ void widen_kernel(const float* __restrict__ in, int64_t n, double* __restrict__ out) {
@@ -503,9 +502,9 @@ static int blocked_cholesky(tb_gp* gp, double* A, int64_t n, double* dinv, int* 
   return 0;
 }
 
-// pack the lower triangle of Linv into DMMA-fragment-ordered panels and mark the derived operand sets stale
-// appended_from > 0: the cache was extended from that many rows by tb_gp_append_data (the dense K^-1, when it exists, is grown
-// by the same rank instead of being invalidated)
+// pack the lower triangle of Linv into DMMA-fragment-ordered panels and move to the next cache generation, which makes every
+// derived operand stale.  appended_from > 0: the cache was extended from that many rows by tb_gp_append_data; a dense K^-1 of
+// the previous generation is grown by the same rank instead.
 static int finish_cache(tb_gp* gp, int64_t appended_from = 0) {
   const int64_t N = gp->N;
   cudaStream_t st = gp->stream;
@@ -518,13 +517,9 @@ static int finish_cache(tb_gp* gp, int64_t appended_from = 0) {
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
   gp->cache_valid = true;
-  ++gp->cache_gen;  // state derived from the posterior (GIBBON repulsion) is rebuilt before its next use
-  gp->upper_valid = false;
-  gp->oz_valid = false;
-  gp->oz5_valid = false;
-  gp->kinv_valid = false;
-  gp->kinv5_valid = false;
-  if (appended_from > 0 && gp->kinv_dense_valid && gp->kinv_dense_N == appended_from) {
+  const bool grow_kinv = appended_from > 0 && gp->kinv_gen == gp->cache_gen;
+  ++gp->cache_gen;  // every operand derived from the posterior is rebuilt before its next use
+  if (grow_kinv) {
     TB_TRY(gp->dKinvSpare.reserve(sizeof(double) * N * N));
     fac::kinv_grow_kernel<<<dim3((unsigned)((N + 127) / 128), (unsigned)N), 128, 0, st>>>(gp->dKinv.as<double>(), appended_from,
                                                                                        gp->dLinv.as<double>(), N, gp->dKinvSpare.as<double>());
@@ -532,9 +527,7 @@ static int finish_cache(tb_gp* gp, int64_t appended_from = 0) {
     TB_CUDA(cudaStreamSynchronize(st));
     TB_CUDA(cudaGetLastError());
     std::swap(gp->dKinv, gp->dKinvSpare);
-    gp->kinv_dense_N = N;
-  } else {
-    gp->kinv_dense_valid = false;
+    gp->kinv_gen = gp->cache_gen;
   }
   return 0;
 }
@@ -784,8 +777,7 @@ int kernels_init() {
   TB_CUDA(cudaFuncSetAttribute(fac::trinv_level_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fac::GEMM_SMEM));
   TB_CUDA(cudaFuncSetAttribute(fac::trinv_level_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fac::GEMM_SMEM));
   TB_CUDA(cudaFuncSetAttribute(fac::kinv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fac::GEMM_SMEM));
-  TB_TRY(oz::trigemm_init());
-  TB_TRY(oz5_init());
+  TB_TRY(int8_init());
   TB_CUDA(cudaFuncSetAttribute(trigemm_kernel<false, EPI_SUMSQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM));
   TB_CUDA(cudaFuncSetAttribute(trigemm_kernel<false, EPI_SUMSQ_PACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM));
   TB_CUDA(cudaFuncSetAttribute(trigemm_kernel<false, EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM));
@@ -795,7 +787,7 @@ int kernels_init() {
 
 // Linv^T packed upper panels: built lazily, only the gradient path needs them
 static int ensure_upper_panels(tb_gp* gp) {
-  if (gp->upper_valid) return 0;
+  if (gp->upper_gen == gp->cache_gen) return 0;
   const int nkB = gp->NB * (BM / BK);
   const int64_t np = upper_panel_count(gp->NB, nkB);
   TB_TRY(gp->dLinvTP.reserve(sizeof(double) * np * PANEL));
@@ -804,7 +796,7 @@ static int ensure_upper_panels(tb_gp* gp) {
                                                          gp->dLinvTP.as<double>());
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
-  gp->upper_valid = true;
+  gp->upper_gen = gp->cache_gen;
   return 0;
 }
 
@@ -921,41 +913,12 @@ static int launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const 
   return 0;
 }
 
-// fp32 models (TB_F32 handles) run the HI pass only: 10 digit products, error ~1e-7 sigma_f^2 << the fp32 tolerance
-static inline int oz_npass(const tb_gp* gp) { return gp->dtype == TB_F32 ? 1 : 2; }
-
-// Ozaki engine state: digit tiles of Linv + row scales, built lazily after each cache refresh
-static int ensure_ozaki(tb_gp* gp) {
-  if (gp->oz_valid) return 0;
-  TB_CHECK(gp->N <= 16384, "the int8 engine supports N <= 16384 (int32 accumulator headroom)");
-  cudaStream_t st = gp->stream;
-  const int64_t rows = (int64_t)gp->NB * BM;
-  gp->nst = (int)((gp->N + oz::KST - 1) / oz::KST);
-  TB_TRY(gp->dRowScale.reserve(sizeof(double) * rows));
-  oz::linv_rowscale_kernel<<<(unsigned)rows, 256, 0, st>>>(gp->dLinv.as<double>(), gp->N, rows, gp->dRowScale.as<double>());
-  TB_LAUNCHED();
-  const int64_t nstages = oz::a_stage_offset(gp->NB);
-  TB_TRY(gp->dAS.reserve((size_t)nstages * oz::S * oz::TILE));
-  TB_CUDA(cudaMemsetAsync(gp->dAS.p, 0, (size_t)nstages * oz::S * oz::TILE, st));
-  oz::linv_digits_kernel<<<dim3(2 * gp->NB, gp->NB), 256, 0, st>>>(gp->dLinv.as<double>(), gp->N, gp->dRowScale.as<double>(),
-                                                                   gp->dAS.as<int8_t>());
-  TB_LAUNCHED();
-  TB_CUDA(cudaGetLastError());
-  int e = 0;
-  std::frexp(gp->variance, &e);  // variance = m 2^e, m in [0.5, 1)  ->  K* / 2^(e+2) < 1/4
-  gp->oz_bscale_exp = e + 2;
-  gp->oz_out_scale = std::ldexp(1.0, gp->oz_bscale_exp);
-  gp->oz_valid = true;
-  return 0;
-}
-
-// K^-1 digit tiles for the gradient path of the int8 engine: V = K^-1 k* as one dense digit GEMM (same K* digits as the
-// variance GEMM).  K^-1 from the cached factor with cuSOLVER potri (once per BO step, lazily).
-// dense K^-1 = Linv^T Linv (lower triangle, ld = N), O(N^3) on the DMMA pipe: once per full cache refresh; appends grow it in
-// O(m N^2) (finish_cache / fac::kinv_grow_kernel)
+// The dense K^-1 whose digit tiles the int8 engines' gradient path multiplies with the K* digits (V = K^-1 K*, one dense digit
+// GEMM): Linv^T Linv (lower triangle, ld = N), O(N^3) on the DMMA pipe (cuSOLVER potri on the cross-check path), lazily once
+// per full cache refresh; appends grow it in O(m N^2) (finish_cache / fac::kinv_grow_kernel)
 static int ensure_kinv_dense(tb_gp* gp) {
   const int64_t N = gp->N;
-  if (gp->kinv_dense_valid && gp->kinv_dense_N == N) return 0;
+  if (gp->kinv_gen == gp->cache_gen) return 0;
   cudaStream_t st = gp->stream;
   TB_TRY(gp->dKinv.reserve(sizeof(double) * N * N));
   if (gp->factor_own) {
@@ -973,46 +936,7 @@ static int ensure_kinv_dense(tb_gp* gp) {
                           gp->dInfo.as<int>());
     TB_CHECK_CODE(cs == CUSOLVER_STATUS_SUCCESS, "cusolverDnDpotri failed", tb::ERR_RUNTIME);
   }
-  gp->kinv_dense_valid = true;
-  gp->kinv_dense_N = N;
-  gp->kinv5_valid = false;
-  return 0;
-}
-
-static int ensure_kinv_digits(tb_gp* gp) {
-  if (gp->kinv_valid) return 0;
-  TB_TRY(ensure_ozaki(gp));
-  cudaStream_t st = gp->stream;
-  const int64_t N = gp->N, rows = (int64_t)gp->NB * BM;
-  TB_TRY(ensure_kinv_dense(gp));
-  TB_TRY(gp->dKinvScale.reserve(sizeof(double) * rows));
-  oz::sym_rowscale_kernel<<<(unsigned)rows, 256, 0, st>>>(gp->dKinv.as<double>(), N, rows, gp->dKinvScale.as<double>());
-  TB_LAUNCHED();
-  const size_t bytes = (size_t)gp->NB * gp->nst * oz::S * oz::TILE;
-  TB_TRY(gp->dKinvS.reserve(bytes));
-  oz::sym_digits_kernel<<<dim3(gp->nst, gp->NB), 256, 0, st>>>(gp->dKinv.as<double>(), N, gp->nst, gp->dKinvScale.as<double>(),
-                                                              gp->dKinvS.as<int8_t>());
-  TB_LAUNCHED();
-  TB_CUDA(cudaStreamSynchronize(st));
-  TB_CUDA(cudaGetLastError());
-  gp->kinv_valid = true;
-  return 0;
-}
-
-static int launch_kstar_digits(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean) {
-  const double* Xs = gp->dXs.as<double>();
-  const double* al = gp->dAlpha.as<double>();
-  const double* il = gp->dInvLs.as<double>();
-  const int N = (int)gp->N, nst = gp->nst, D = gp->D;
-  const double var = gp->variance, mc0 = gp->mean_const;
-  const double inv_b = std::ldexp(1.0, 48 - gp->oz_bscale_exp);
-  cudaStream_t st = gp->stream;
-  with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
-    oz::kstar_digits_kernel<decltype(K)::value, decltype(P)::value><<<tiles, 512, 0, st>>>(Xs, al, Xc_dev, il, N, nst, D, mc, var, inv_b,
-                                                                                            mc0, BS, mean);
-  });
-  TB_LAUNCHED();
-  TB_CUDA(cudaGetLastError());
+  gp->kinv_gen = gp->cache_gen;
   return 0;
 }
 
@@ -1249,45 +1173,31 @@ static int launch_mean_bounds(tb_gp* gp, cudaStream_t st, const double* Xc, int6
 // =================================================================================================
 enum class Engine {
   F64,   // native fp64 DMMA kernels (kernels_f64.cuh)
-  OZ21,  // two-pass 6-digit int8 engine, 21 digit products (ozaki.cuh)
-  OZ15,  // single-pass int8 engine (ozaki5.cuh): 15 digit products on fp64 handles, 6 or 10 on fp32 ones
+  OZ21,  // 6-digit int8 engine, 21 digit products (ozaki.cuh, int8_engines.cu)
+  OZ15,  // single-pass int8 engine (ozaki5.cuh, int8_engines.cu): 15 digit products on fp64 handles, 6 or 10 on fp32 ones
 };
 
 // The engine of a call, after the lazy builds it needs.  need_v: the call also needs V = K^-1 K* (gradients).  The int8
 // engines' int32 accumulators are exact up to K = N = 16384; larger models and engine 0 run the fp64 kernels.  The
-// single-pass engine runs when its a-priori error estimate admits the handle (oz5_ensure) and, for V, when the V GEMM's own
-// estimate does too (oz5_ensure_kinv); otherwise the 21-product engine does.
+// single-pass engine runs when its a-priori error estimates admit the handle (int8_select); otherwise the 21-product engine
+// does.
 static int select_engine(tb_gp* gp, bool need_v, Engine* eng) {
   if (!(gp->engine == 1 && gp->N <= 16384)) {
     if (need_v) TB_TRY(ensure_upper_panels(gp));
     *eng = Engine::F64;
     return 0;
   }
-  TB_TRY(oz5_ensure(gp));
-  // oz5_ensure sets oz5_mode (the digits the variance GEMM computes with) and oz5_planes (the digits stored) together, both
-  // zero or both non-zero, so either one says whether the single-pass engine is admitted
-  bool fast = gp->oz5_planes != 0;
-  if (fast && need_v) {
-    TB_TRY(ensure_kinv_dense(gp));
-    TB_TRY(oz5_ensure_kinv(gp));
-    fast = gp->kinv5_ok;
-  }
-  if (!fast) {
-    TB_TRY(ensure_ozaki(gp));
-    if (need_v) TB_TRY(ensure_kinv_digits(gp));
-  }
-  *eng = fast ? Engine::OZ15 : Engine::OZ21;
+  if (need_v) TB_TRY(ensure_kinv_dense(gp));
+  bool single_pass;
+  TB_TRY(int8_select(gp, need_v, &single_pass));
+  *eng = single_pass ? Engine::OZ15 : Engine::OZ21;
   return 0;
 }
 
 // candidates per K* tile, and the K* scratch bytes per tile
-static int eng_tile_width(const tb_gp* gp, Engine e) { return e == Engine::OZ15 ? oz5_tile_width(gp) : BT; }
+static int eng_tile_width(const tb_gp* gp, Engine e) { return e == Engine::F64 ? BT : int8_tile_width(gp, e == Engine::OZ15); }
 static size_t eng_tile_bytes(const tb_gp* gp, Engine e) {
-  switch (e) {
-    case Engine::F64: return (size_t)gp->nkc * PANEL * sizeof(double);
-    case Engine::OZ21: return (size_t)gp->nst * oz::S * oz::TILE;
-    default: return oz5_tile_bytes(gp);
-  }
+  return e == Engine::F64 ? (size_t)gp->nkc * PANEL * sizeof(double) : int8_tile_bytes(gp, e == Engine::OZ15);
 }
 
 // Row-block groups per candidate tile of the Linv GEMMs.  int8 engines: ~4 row-blocks per CTA amortise the CTA prologue
@@ -1300,14 +1210,11 @@ static int eng_groups(const tb_gp* gp, Engine e, int tiles) {
 }
 
 // K* of mc device candidates into gp->sKs (fp64 panels or digit tiles), their posterior means into gp->sMean.
-// split: the single-pass engine's k-split (nullptr: the one oz5_kstar_split gives for this many tiles)
+// split: the int8 engines' k-split (nullptr: the one int8_kstar_split gives for this many tiles)
 static int eng_kstar(tb_gp* gp, Engine e, const double* xc, int64_t mc, int tiles, const KSplit* split = nullptr) {
   double* mean = gp->sMean.as<double>();
-  switch (e) {
-    case Engine::F64: return launch_kstar(gp, xc, mc, tiles, gp->sKs.as<double>(), mean);
-    case Engine::OZ21: return launch_kstar_digits(gp, xc, mc, tiles, gp->sKs.as<int8_t>(), mean);
-    default: return oz5_launch_kstar(gp, gp->stream, xc, mc, tiles, gp->sKs.as<int8_t>(), mean, split);
-  }
+  if (e == Engine::F64) return launch_kstar(gp, xc, mc, tiles, gp->sKs.as<double>(), mean);
+  return int8_kstar(gp, e == Engine::OZ15, xc, mc, tiles, gp->sKs.as<int8_t>(), mean, split);
 }
 
 // Variance GEMM: sums of squares of A = Linv K* over G row-block groups into gp->sPartial.  fp64 engine with packed_a: A
@@ -1315,65 +1222,47 @@ static int eng_kstar(tb_gp* gp, Engine e, const double* xc, int64_t mc, int tile
 static int eng_variance(tb_gp* gp, Engine e, int tiles, int G, int64_t McPad, bool packed_a) {
   cudaStream_t st = gp->stream;
   double* partial = gp->sPartial.as<double>();
-  switch (e) {
-    case Engine::F64:
-      if (packed_a)
-        trigemm_kernel<false, EPI_SUMSQ_PACKED><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-            gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, gp->sA.as<double>(), nullptr, 0);
-      else
-        trigemm_kernel<false, EPI_SUMSQ><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
-            gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, nullptr, nullptr, 0);
-      TB_LAUNCHED();
-      TB_CUDA(cudaGetLastError());
-      return 0;
-    case Engine::OZ21:
-      return oz::launch_trigemm<oz::OZ_SUMSQ>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
-                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 0, partial, nullptr, 0);
-    default: return oz5_launch_gemm(gp, st, gp->sKs.as<int8_t>(), tiles, G, McPad, partial);
-  }
+  if (e != Engine::F64) return int8_variance(gp, e == Engine::OZ15, gp->sKs.as<int8_t>(), tiles, G, McPad, partial);
+  if (packed_a)
+    trigemm_kernel<false, EPI_SUMSQ_PACKED><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
+        gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, gp->sA.as<double>(), nullptr, 0);
+  else
+    trigemm_kernel<false, EPI_SUMSQ><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
+        gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, nullptr, nullptr, 0);
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 // A = Linv K* stored plain into out ([candidate][NB*128])
 static int eng_store_a(tb_gp* gp, Engine e, int tiles, int64_t McPad, double* out) {
-  cudaStream_t st = gp->stream;
   const int64_t lda = (int64_t)gp->NB * BM;
   const int G = eng_groups(gp, e, tiles);
-  switch (e) {
-    case Engine::F64:
-      trigemm_kernel<false, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB,
-                                                                                    gp->nkc, G, McPad, nullptr, nullptr, out, lda);
-      TB_LAUNCHED();
-      TB_CUDA(cudaGetLastError());
-      return 0;
-    case Engine::OZ21:
-      return oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dAS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dRowScale.as<double>(), gp->NB,
-                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 0, nullptr, out, lda);
-    default: return oz5_launch_gemm_store(gp, st, 0, gp->sKs.as<int8_t>(), tiles, G, out, lda);
-  }
+  if (e != Engine::F64) return int8_store(gp, e == Engine::OZ15, false, gp->sKs.as<int8_t>(), tiles, G, McPad, out, lda);
+  trigemm_kernel<false, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, gp->stream>>>(gp->dLinvP.as<double>(), gp->sKs.as<double>(),
+                                                                                        gp->NB, gp->nkc, G, McPad, nullptr, nullptr, out, lda);
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 // V = K^-1 K* stored plain into gp->sV ([candidate][NB*128]).  fp64 engine: Linv^T A over the packed A that eng_variance left
-// in gp->sA; int8 engines: the digit tiles of the dense K^-1 times the same K* digits.
+// in gp->sA; int8 engines: the digit tiles of the dense K^-1 times the same K* digits.  The 21-product engine's V GEMM has
+// its own row-block groups: at most ~8 row-blocks each.
 static int eng_store_v(tb_gp* gp, Engine e, int tiles, int64_t McPad) {
-  cudaStream_t st = gp->stream;
   const int64_t ldv = (int64_t)gp->NB * BM;
   double* V = gp->sV.as<double>();
-  switch (e) {
-    case Engine::F64: {
-      const int G = eng_groups(gp, e, tiles);
-      trigemm_kernel<true, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB,
-                                                                                   gp->NB * (BM / BK), G, McPad, nullptr, nullptr, V, ldv);
-      TB_LAUNCHED();
-      TB_CUDA(cudaGetLastError());
-      return 0;
-    }
-    case Engine::OZ21: {
-      const int G = std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)));
-      return oz::launch_trigemm<oz::OZ_STORE>(st, tiles, gp->dKinvS.as<int8_t>(), gp->sKs.as<int8_t>(), gp->dKinvScale.as<double>(), gp->NB,
-                                              gp->nst, G, McPad, gp->oz_out_scale, oz_npass(gp), 1, nullptr, V, ldv);
-    }
-    default: return oz5_launch_gemm_store(gp, st, 1, gp->sKs.as<int8_t>(), tiles, eng_groups(gp, e, tiles), V, ldv);
+  if (e == Engine::OZ21) {
+    const int G = std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)));
+    return int8_store(gp, false, true, gp->sKs.as<int8_t>(), tiles, G, McPad, V, ldv);
   }
+  const int G = eng_groups(gp, e, tiles);
+  if (e == Engine::OZ15) return int8_store(gp, true, true, gp->sKs.as<int8_t>(), tiles, G, McPad, V, ldv);
+  trigemm_kernel<true, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, gp->stream>>>(gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB,
+                                                                                       gp->NB * (BM / BK), G, McPad, nullptr, nullptr, V, ldv);
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 // =================================================================================================
@@ -1490,11 +1379,8 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, Engine e, int64_t c
   unsigned long long* count = reinterpret_cast<unsigned long long*>(probe_v + 2);
   // the unscreened loop's chunks: whole ones over [0, split), the last over [split, M); only the last can have another k-split
   const int64_t split = ((M - 1) / chunk_cap) * chunk_cap;
-  KSplit ks_full, ks_last;
-  if (e == Engine::OZ15) {
-    ks_full = oz5_kstar_split(gp, (int)(chunk_cap / nt));
-    ks_last = oz5_kstar_split(gp, (int)((M - split + nt - 1) / nt));
-  }
+  const KSplit ks_full = int8_kstar_split(gp, e == Engine::OZ15, (int)(chunk_cap / nt)),
+               ks_last = int8_kstar_split(gp, e == Engine::OZ15, (int)((M - split + nt - 1) / nt));
   const bool same_split = ks_full.ksplit == ks_last.ksplit && ks_full.kc_per == ks_last.kc_per;
   // 1. bound pass
   const double var_ub = std::fmax(gp->variance, 1e-12);
@@ -1914,7 +1800,7 @@ int tb_acq_set_gibbon_repulsion(tb_gp* gp, const double* pending, int m, double 
   gp->gibP.swap(p);
   gp->gibM = m;
   gp->gibD = gp->D;
-  gp->gib_gen = ~(uint64_t)0;
+  gp->gib_gen = STALE;
   const int rc = tb::ensure_gibbon(gp);
   if (rc) gp->gibM = 0;  // a pending set that cannot be factorised is not kept
   return rc;
@@ -1932,8 +1818,7 @@ int tb_gp_set_engine(tb_gp* gp, int engine) {
   TB_CHECK(gp, "tb_gp_set_engine: null handle");
   TB_CHECK(engine >= 0 && engine <= 2, "tb_gp_set_engine: engine must be 0 (fp64 DMMA), 1 (int8 Ozaki) or 2 (int8, full 21 products)");
   gp->engine = engine == 0 ? 0 : 1;
-  if (gp->oz_full != (engine == 2)) gp->oz5_valid = false;
-  gp->oz_full = engine == 2;
+  tb::int8_pin_full(gp, engine == 2);
   return 0;
 }
 int tb_gp_engine_info(tb_gp* gp, int* digit_products, double* error_estimate) {
@@ -1944,12 +1829,7 @@ int tb_gp_engine_info(tb_gp* gp, int* digit_products, double* error_estimate) {
   TB_TRY(tb::select_engine(gp, false, &e));
   int products = 0;
   double est = 0.0;
-  if (e != tb::Engine::F64) {
-    if (gp->oz5_mode == 5) products = 15;
-    else if (gp->oz5_mode == 3) products = 6;
-    else products = gp->dtype == TB_F32 ? 10 : 21;
-    est = gp->oz5_est;
-  }
+  if (e != tb::Engine::F64) tb::int8_info(gp, &products, &est);
   if (digit_products) *digit_products = products;
   if (error_estimate) *error_estimate = est;
   return 0;

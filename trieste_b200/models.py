@@ -12,7 +12,6 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
 from typing import Optional, Tuple
 
 import numpy as np
@@ -167,7 +166,7 @@ class GaussianProcessRegression:
 
     @property
     def engine(self) -> str:
-        return getattr(self, "_engine", "int8" if os.environ.get("TB_ENGINE", "int8") != "fp64" else "fp64")
+        return getattr(self, "_engine", "int8")  # the handle's default until set_engine is called
 
     def engine_info(self) -> Tuple[int, float]:
         """(int8 digit products per k-step of the variance GEMM — 15 / 21, fp32 models 6 / 10, 0 = native fp64 engine —,
