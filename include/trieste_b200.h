@@ -234,6 +234,15 @@ int tb_rff_eval(tb_rff* r, const void* Xc, int64_t M, void* out, double* min_val
  * adds the canonical features  sum_j v[b][j] k(x, X_j)  to trajectory b.  X [N,D] raw training inputs (host),
  * v [nb,N] column layout [trajectory][training point] (host or device).  N = 0 switches the term off. */
 int tb_rff_set_canonical(tb_rff* r, int kernel, const double* X, int64_t N, const double* v, int nb);
+/* feature_decomposition_trajectory.__call__ for x [M, B, D] (models/gpflow/sampler.py:901-936): point (m, b) under
+ * trajectory b only -> out [M, B]; grad (nullable) [M, B, D].  B == nb (and == the canonical weights' nb when set).
+ * Values are bit for bit those of tb_rff_eval on column b.  fp64, host or device pointers. */
+int tb_rff_eval_paired(tb_rff* r, const void* Xc, int64_t M, int B, void* out, void* grad);
+/* tb_acq_maximize's contract for the NEGATED trajectories: starts [R, nb, D], start (i, b) maximises -f_b inside the box;
+ * x_out [R, nb, D], f_out [R, nb] (= -f_b at x_out), success, nfev as tb_acq_maximize.  R * nb < 2^31. */
+int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const double* starts, int64_t R, int maxcor,
+                    int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
+                    int64_t* nfev);
 /* (K(X,X) + noise I)^-1 B = Linv^T (Linv B) through the cached triangular inverse: B, out [nrhs][N] (each right-hand side contiguous);
  * the v-weights of a decoupled trajectory (sampler.py:716, gpflux compute_A_inv_b).  fp64, host or device. */
 int tb_gp_kinv_apply(tb_gp* gp, const double* B, int nrhs, double* out);

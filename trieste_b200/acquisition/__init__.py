@@ -1,3 +1,8 @@
+from .continuous_thompson_sampling import (  # noqa: F401
+    GreedyContinuousThompsonSampling,
+    ParallelContinuousThompsonSampling,
+    negate_trajectory_function,
+)
 from .function import (  # noqa: F401
     AugmentedExpectedImprovement,
     augmented_expected_improvement,
@@ -41,4 +46,9 @@ from .interface import (  # noqa: F401
     SingleModelVectorizedAcquisitionBuilder,
     VectorizedAcquisitionFunctionBuilder,
 )
-from .utils import MultivariateNormalCDF, split_acquisition_function, split_acquisition_function_calls  # noqa: F401
+from .utils import (  # noqa: F401
+    MultivariateNormalCDF,
+    select_nth_output,
+    split_acquisition_function,
+    split_acquisition_function_calls,
+)

@@ -11,7 +11,8 @@ evaluation (:566-745), this module runs ONE multi-start projected L-BFGS over al
 iteration is a single fused value+gradient launch on the GPU for all active starts.  For the fused
 single-model functions (EI, log-EI, LCB, PI, AEI, MES) the per-start bookkeeping — two-loop recursion,
 line search, convergence tests — runs on the device as well (``tb_acq_maximize``, csrc/lbfgs.cuh; one
-warp per start); any other function with a ``value_and_gradient`` method goes through the vectorised
+warp per start), and so does it for the negated trajectories of continuous Thompson sampling (``tb_rff_maximize``, one
+problem per start and trajectory); any other function with a ``value_and_gradient`` method goes through the vectorised
 NumPy implementation of the same algorithm below (also selectable with ``TB_LBFGS=host``).  Same
 stopping rules as SciPy's defaults (gtol 1e-5 on the projected gradient, ftol 2.2e-9 relative
 decrease, maxiter).
@@ -178,10 +179,11 @@ def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points:
 
     R, V, D = starting_points.shape
     P = R * V
-    if V == 1 and hasattr(fn, "maximize_from") and os.environ.get("TB_LBFGS", "device") != "host" and m <= 16:
-        # fused single-model acquisition functions: the whole multi-start loop runs on the device (tb_acq_maximize)
-        ok, fun, xs, nf = fn.maximize_from(starting_points.reshape(P, D), lower, upper, maxcor=m, maxiter=maxiter, maxls=maxls,
-                                           gtol=gtol, ftol=ftol)
+    if hasattr(fn, "maximize_from") and os.environ.get("TB_LBFGS", "device") != "host" and m <= 16:
+        # the whole multi-start loop runs on the device: tb_acq_maximize for the fused single-model functions (starts
+        # [P, D]), tb_rff_maximize for the negated trajectories of continuous Thompson sampling (starts [R, V, D])
+        starts = starting_points.reshape(P, D) if V == 1 else starting_points
+        ok, fun, xs, nf = fn.maximize_from(starts, lower, upper, maxcor=m, maxiter=maxiter, maxls=maxls, gtol=gtol, ftol=ftol)
         return ok.reshape(R, V), fun.reshape(R, V), xs.reshape(R, V, D), nf.reshape(R, V)
     x = np.clip(starting_points.reshape(P, D).astype(np.float64), lower, upper)
 

@@ -1,5 +1,5 @@
-"""``split_acquisition_function`` / ``split_acquisition_function_calls`` — mirrors trieste/acquisition/utils.py:31-109 —
-and ``MultivariateNormalCDF`` (acquisition/function/utils.py:29-199).
+"""``split_acquisition_function`` / ``split_acquisition_function_calls`` / ``select_nth_output`` — mirrors
+trieste/acquisition/utils.py:31-123 — and ``MultivariateNormalCDF`` (acquisition/function/utils.py:29-199).
 
 In the reference these wrappers bound the memory of one TensorFlow evaluation by cutting the leading (candidate) axis into
 blocks.  Here the fused kernels already stream any batch through bounded scratch (``run_eval`` chunks at
@@ -57,6 +57,11 @@ def split_acquisition_function_calls(optimizer, split_size: int):
         return optimizer(search_space, (taf, n) if isinstance(f, tuple) else taf)
 
     return split_optimizer
+
+
+def select_nth_output(x, output_dim: int = 0):
+    """utils.py:112-123: the ``output_dim``-th output of ``x`` [..., B, L] as the trajectory, shape [..., B]."""
+    return x[..., output_dim]
 
 
 class MultivariateNormalCDF:

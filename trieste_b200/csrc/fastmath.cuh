@@ -145,15 +145,25 @@ struct TrigConsts {
   double s3 = -0x1.5555555555555p-3, s5 = 0x1.1111111111111p-7, s7 = -0x1.a01a01a01a01ap-13, s9 = 0x1.71de3a556c734p-19;
   double s11 = -0x1.ae64567f544e4p-26, s13 = 0x1.6124613a86d09p-33, s15 = -0x1.ae7f3e733b81fp-41, s17 = 0x1.952c77030ad4ap-49;
   double s19 = -0x1.2f49b46814157p-57;
+  // cos(r) Taylor coefficients 1 / (2j)! with signs, j = 2..10 (the r^2 one is -1/2, an immediate)
+  double c4 = 0x1.5555555555555p-5, c6 = -0x1.6c16c16c16c17p-10, c8 = 0x1.a01a01a01a01ap-16, c10 = -0x1.27e4fb7789f5cp-22;
+  double c12 = 0x1.1eed8eff8d898p-29, c14 = -0x1.93974a8c07c9dp-37, c16 = 0x1.ae7f3e733b81fp-45, c18 = -0x1.6827863b97d97p-53;
+  double c20 = 0x1.e542ba4020225p-62;
 };
 
-TB_FM_HD double cos_fast(double a, const TrigConsts& c) {
+// the shared argument reduction: a = r + (2k - 1) pi/2, r in [-pi/2, pi/2]; returns r, sets k
+TB_FM_HD double trig_reduce(double a, const TrigConsts& c, int& k) {
   const double t = fma(a, c.inv_pi, 0.5) + MAGIC;  // low word = k = rint(a / pi + 1/2)  (MAGIC + 0.5 is not representable)
-  const int k = lo_word(t);
+  k = lo_word(t);
   const double m = fma(2.0, t - MAGIC, -1.0);      // 2k - 1 (exact)
   double r = fma(m, -c.pio2_hi, a);
   r = fma(m, -c.pio2_mid, r);
   r = fma(m, -c.pio2_lo, r);
+  return r;
+}
+
+// cos(a) = (-1)^k sin(r) from the reduced argument
+TB_FM_HD double cos_reduced(double r, int k, const TrigConsts& c) {
   const double r2 = r * r;
   double p = fma(c.s19, r2, c.s17);
   p = fma(p, r2, c.s15);
@@ -165,6 +175,33 @@ TB_FM_HD double cos_fast(double a, const TrigConsts& c) {
   p = fma(p, r2, c.s3);
   const double sr = fma(p * r2, r, r);  // sin(r)
   return with_hi_word(sr, hi_word(sr) ^ (k << 31));  // (-1)^k
+}
+
+TB_FM_HD double cos_fast(double a, const TrigConsts& c) {
+  int k;
+  const double r = trig_reduce(a, c, k);
+  return cos_reduced(r, k, c);
+}
+
+// cos(a), returned bit for bit as cos_fast(a), and sin(a) into s, from one reduction: sin(a) = (-1)^(k+1) cos(r) with cos(r) by its
+// Taylor polynomial through r^20 (remainder < 2e-17 on [-pi/2, pi/2]); the absolute error is bounded like cos_fast's
+// (tools/sincos_check.cu).
+TB_FM_HD double sincos_fast(double a, const TrigConsts& c, double& s) {
+  int k;
+  const double r = trig_reduce(a, c, k);
+  const double r2 = r * r;
+  double p = fma(c.c20, r2, c.c18);
+  p = fma(p, r2, c.c16);
+  p = fma(p, r2, c.c14);
+  p = fma(p, r2, c.c12);
+  p = fma(p, r2, c.c10);
+  p = fma(p, r2, c.c8);
+  p = fma(p, r2, c.c6);
+  p = fma(p, r2, c.c4);
+  p = fma(p, r2, -0.5);
+  const double cr = fma(p, r2, 1.0);  // cos(r) >= 0
+  s = with_hi_word(cr, hi_word(cr) ^ ((k + 1) << 31));  // (-1)^(k+1)
+  return cos_reduced(r, k, c);
 }
 
 }  // namespace fm

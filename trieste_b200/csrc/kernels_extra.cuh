@@ -808,6 +808,108 @@ kdot_kernel(const double* __restrict__ Xs, const double* __restrict__ V, int64_t
   }
 }
 
+// K3b: paired trajectory evaluation: point t under its own trajectory b(t) = (pidx ? pidx[t] : idx0 + t) % nb only, times sgn (+-1,
+// exact), with the gradient when GRAD.  pidx carries the compacted problem indices of the device L-BFGS, idx0 + t the flat (m, b)
+// index of an [M, B, D] input.  The value repeats rff_eval_kernel's feature order and fma sequence over the DP padded pairs, cos_fast,
+// fma(acc, scale, mean), then adds kdot_kernel's canonical sum over j in ascending order, so it is bit for bit the per-column value.
+//   grad_d = (-scale sum_f theta_bf sin(a_f) W_fd + sum_j v_bj 2 k'(r2_j) (x~_d - x~_jd)) / l_d
+// Matern-12 at a coincident training point: r2 is clamped at 1e-36 as in mean_grad_kernel, and its zero difference makes the
+// contribution zero.  One thread per point; W and the bias stream through shared memory, theta_b and v_b are per-lane loads (rows
+// of arbitrary trajectories: L1 / L2 hits).  N = 0 (no canonical part): Xs and V are not read.
+template <int KIND, int DP, bool GRAD>
+__global__ void __launch_bounds__(RFF_THREADS, 1)  // minimum of one CTA per SM: without it ptxas spills at small DP
+rff_paired_kernel(const double* __restrict__ Wp, const double* __restrict__ bias, const double* __restrict__ theta,
+                  const double* __restrict__ Xs, const double* __restrict__ V, const double* __restrict__ Xc,
+                  const double* __restrict__ inv_ls, int D, int F, int N, int nb, int64_t M, int64_t idx0,
+                  const int* __restrict__ pidx, double scale, double mean_const, double variance, double sgn,
+                  const __grid_constant__ fm::TrigConsts tc, const __grid_constant__ fm::Consts fc, double* __restrict__ out,
+                  double* __restrict__ grad) {
+  extern __shared__ __align__(16) unsigned char rsm[];
+  double* sW = reinterpret_cast<double*>(rsm);  // [RFF_FCHUNK][DP]
+  double* sb = sW + RFF_FCHUNK * DP;            // [RFF_FCHUNK]
+  __shared__ double exp_tab[64];
+  if (threadIdx.x < 64) exp_tab[threadIdx.x] = fm::EXP2_TABLE_DEV[threadIdx.x];
+  const int64_t t = (int64_t)blockIdx.x * RFF_THREADS + threadIdx.x;
+  const bool valid = t < M;
+  const int b = valid ? (int)((pidx ? (int64_t)pidx[t] : idx0 + t) % nb) : 0;
+  const double* th = theta + (int64_t)b * F;
+  double x[DP], g[GRAD ? DP : 1];
+#pragma unroll
+  for (int d = 0; d < DP; ++d) x[d] = (valid && d < D) ? Xc[t * D + d] * inv_ls[d] : 0.0;
+#pragma unroll
+  for (int d = 0; d < (GRAD ? DP : 1); ++d) g[d] = 0.0;
+  double acc = 0.0;
+  for (int f0 = 0; f0 < F; f0 += RFF_FCHUNK) {
+    const int fcn = min(RFF_FCHUNK, F - f0);
+    __syncthreads();
+    for (int e = threadIdx.x; e < fcn * DP; e += RFF_THREADS) sW[e] = Wp[(int64_t)f0 * DP + e];
+    for (int e = threadIdx.x; e < fcn; e += RFF_THREADS) sb[e] = bias[f0 + e];
+    __syncthreads();
+    for (int f = 0; f < fcn; ++f) {
+      double a = sb[f];
+#pragma unroll
+      for (int d = 0; d < DP; d += 2) {
+        double2 w = *reinterpret_cast<const double2*>(sW + f * DP + d);
+        a = fma(w.x, x[d], a);
+        a = fma(w.y, x[d + 1], a);
+      }
+      const double tf = __ldg(th + f0 + f);
+      if constexpr (GRAD) {
+        double s;
+        acc = fma(tf, fm::sincos_fast(a, tc, s), acc);
+        const double ts = tf * s;
+#pragma unroll
+        for (int d = 0; d < DP; d += 2) {
+          double2 w = *reinterpret_cast<const double2*>(sW + f * DP + d);
+          g[d] = fma(ts, w.x, g[d]);
+          g[d + 1] = fma(ts, w.y, g[d + 1]);
+        }
+      } else {
+        acc = fma(tf, fm::cos_fast(a, tc), acc);
+      }
+    }
+  }
+  if (!valid) return;
+  double v = fma(acc, scale, mean_const);
+  if constexpr (GRAD) {
+#pragma unroll
+    for (int d = 0; d < DP; ++d) g[d] *= -scale;
+  }
+  if (N > 0) {
+    const double* vb = V + (int64_t)b * N;
+    double cacc = 0.0;
+    for (int k = 0; k < N; ++k) {
+      const double* xr = Xs + (int64_t)k * DP;
+      double r2 = 0.0;
+#pragma unroll
+      for (int d = 0; d < DP; d += 2) {
+        const double2 xv = __ldg(reinterpret_cast<const double2*>(xr + d));
+        const double d0 = x[d] - xv.x, d1 = x[d + 1] - xv.y;
+        r2 = fma(d0, d0, r2);
+        r2 = fma(d1, d1, r2);
+      }
+      const double vk = __ldg(vb + k);
+      cacc = fma(kernel_from_r2_fast<KIND>(r2, variance, exp_tab, fc), vk, cacc);
+      if constexpr (GRAD) {
+        const double w = 2.0 * kernel_dr2_fast<KIND>(r2, variance, exp_tab, fc) * vk;
+#pragma unroll
+        for (int d = 0; d < DP; d += 2) {
+          const double2 xv = __ldg(reinterpret_cast<const double2*>(xr + d));
+          g[d] = fma(w, x[d] - xv.x, g[d]);
+          g[d + 1] = fma(w, x[d + 1] - xv.y, g[d + 1]);
+        }
+      }
+    }
+    v += cacc;
+  }
+  out[t] = sgn * v;
+  if constexpr (GRAD) {
+#pragma unroll
+    for (int d = 0; d < DP; ++d)
+      if (d < D) grad[t * D + d] = sgn * g[d] * inv_ls[d];
+  }
+}
+
 // fold block winners per trajectory (grid.x = nb)
 __global__ void __launch_bounds__(256)
 rff_fold_kernel(const double* __restrict__ blk_best, const int64_t* __restrict__ blk_idx, int nblk,

@@ -2356,7 +2356,7 @@ struct tb_rff {
   double variance = 1.0, mean_const = 0.0;
   tb::DevBuf dW, dB, dTheta, dInvLs, sXc, sOut, sBlkBest, sBlkIdx, sRunV, sRunI;
   // canonical features of a decoupled trajectory: scaled training inputs + per-trajectory weights v [nbc, N]
-  tb::DevBuf dXs, dV, sCanon;
+  tb::DevBuf dXs, dV, sCanon, sGrad;
   int kernel = TB_MATERN52, nbc = 0;
   int64_t N = 0;
 };
@@ -2584,6 +2584,78 @@ int tb_rff_eval(tb_rff* r, const void* Xc, int64_t M, void* out, double* min_val
 
 }  // extern "C"
 
+namespace tb {
+// at most this many points per paired launch (the chunk of tb_rff_eval)
+constexpr int64_t RFF_PAIRED_CHUNK = (int64_t)1 << 22;
+
+// M (<= RFF_PAIRED_CHUNK) device points, point t under trajectory (pidx ? pidx[t] : idx0 + t) % nb: sgn * values -> out [M],
+// sgn * gradients -> grad [M, D] when grad is not null
+static int launch_rff_paired(tb_rff* r, const double* xc, int64_t M, int64_t idx0, const int* pidx, double sgn, double* out,
+                             double* grad) {
+  const int blocks = (int)((M + RFF_THREADS - 1) / RFF_THREADS);
+  const double scale = std::sqrt(2.0 * r->variance / (double)r->F);
+  const bool canon = r->N > 0;
+  return with_kind_dp(r->kernel, r->DP, [&](auto K, auto P) -> int {
+    constexpr int KIND = decltype(K)::value, DP = decltype(P)::value;
+    const size_t smem = sizeof(double) * ((size_t)RFF_FCHUNK * DP + RFF_FCHUNK);
+    auto launch = [&](auto kern) -> int {
+      TB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      kern<<<blocks, RFF_THREADS, smem, r->stream>>>(r->dW.as<double>(), r->dB.as<double>(), r->dTheta.as<double>(),
+                                                      canon ? r->dXs.as<double>() : nullptr, canon ? r->dV.as<double>() : nullptr,
+                                                      xc, r->dInvLs.as<double>(), r->D, r->F, (int)r->N, r->nb, M, idx0, pidx,
+                                                      scale, r->mean_const, r->variance, sgn, fm::TrigConsts(), fm::Consts(),
+                                                      out, grad);
+      TB_LAUNCHED();
+      TB_CUDA(cudaGetLastError());
+      return 0;
+    };
+    return grad ? launch(rff_paired_kernel<KIND, DP, true>) : launch(rff_paired_kernel<KIND, DP, false>);
+  });
+}
+
+static int check_rff_paired(tb_rff* r, const char* name) {
+  TB_CHECK(r->F > 0 && r->nb > 0, std::string(name) + ": features and theta must be set first");
+  TB_CHECK(r->N == 0 || r->nbc == r->nb,
+           std::string(name) + ": canonical weights and theta must have the same number of trajectories");
+  return 0;
+}
+}  // namespace tb
+
+extern "C" {
+
+int tb_rff_eval_paired(tb_rff* r, const void* Xc, int64_t M, int B, void* out, void* grad) {
+  TB_CHECK(r, "tb_rff_eval_paired: null handle");
+  TB_CHECK(M >= 0, "tb_rff_eval_paired: negative number of points");
+  TB_CHECK(M == 0 || (Xc && out), "tb_rff_eval_paired: null argument");
+  TB_TRY(tb::check_rff_paired(r, "tb_rff_eval_paired"));
+  TB_CHECK(B == r->nb, "tb_rff_eval_paired: the batch size must equal the number of trajectories");
+  if (M == 0) return 0;
+  TB_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = r->stream;
+  const int D = r->D;
+  const int64_t P = M * B;
+  const int64_t chunk = std::min<int64_t>(P, tb::RFF_PAIRED_CHUNK);
+  const tb::Staged<const double> xin((const double*)Xc, D, r->sXc, st);
+  const tb::Staged<double> outs((double*)out, 1, r->sOut, st);
+  const tb::Staged<double> grads((double*)grad, D, r->sGrad, st);
+  TB_TRY(xin.reserve(chunk));
+  TB_TRY(outs.reserve(chunk));
+  TB_TRY(grads.reserve(chunk));
+  for (int64_t c0 = 0; c0 < P; c0 += chunk) {
+    const int64_t mc = std::min<int64_t>(chunk, P - c0);
+    const double* xc;
+    TB_TRY(xin.in(c0, mc, &xc));
+    TB_TRY(tb::launch_rff_paired(r, xc, mc, c0, nullptr, 1.0, outs.out(c0), grads.out(c0)));
+    TB_TRY(outs.back(c0, mc));
+    TB_TRY(grads.back(c0, mc));
+  }
+  TB_CUDA(cudaStreamSynchronize(st));
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"
+
 
 extern "C" {
 
@@ -2597,26 +2669,24 @@ __global__ void lbfgs_finish_kernel(tb::lb::State s, int64_t P, double* __restri
   nfev[p] = (int64_t)s.nfev[p];
 }
 
-int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const double* upper, const double* starts, int64_t P,
-                    int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
-                    int32_t* success, int64_t* nfev) {
-  TB_CHECK(gp && lower && upper, "tb_acq_maximize: null argument");
-  TB_CHECK(P >= 0 && P < ((int64_t)1 << 31), "tb_acq_maximize: number of starts out of range");
-  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_acq_maximize: null argument");
-  bool pen = false;
-  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_maximize"));
-  if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
-    TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
-  if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
-  TB_CHECK(maxcor >= 1 && maxcor <= tb::lb::MMAX, "tb_acq_maximize: maxcor must be in [1, " + std::to_string(tb::lb::MMAX) + "]");
-  TB_CHECK(maxiter >= 1 && maxls >= 1, "tb_acq_maximize: maxiter and maxls must be positive");
-  TB_CHECK(gtol >= 0.0 && ftol >= 0.0, "tb_acq_maximize: tolerances must be non-negative");
-  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_maximize"));
-  if (P == 0) return 0;
-  TB_CUDA(cudaSetDevice(gp->device));
-  cudaStream_t st = gp->stream;
-  const int D = gp->D, m = maxcor;
+}  // extern "C"
+
+namespace tb {
+static int check_lbfgs_options(const std::string& name, int maxcor, int maxiter, int maxls, double gtol, double ftol) {
+  TB_CHECK(maxcor >= 1 && maxcor <= lb::MMAX, name + ": maxcor must be in [1, " + std::to_string(lb::MMAX) + "]");
+  TB_CHECK(maxiter >= 1 && maxls >= 1, name + ": maxiter and maxls must be positive");
+  TB_CHECK(gtol >= 0.0 && ftol >= 0.0, name + ": tolerances must be non-negative");
+  return 0;
+}
+
+// The multi-start L-BFGS round loop shared by every device maximiser: P (>= 1) problems in D dimensions on the stream st; each
+// round asks eval(xt [n, D], idx [n], n, vals [n], grad [n, D]) for the values and gradients of the function to MAXIMISE at the
+// trial points of the n active problems (all device arrays; idx holds their problem indices), then runs one step of each.
+template <class Eval>
+static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* lower, const double* upper, const double* starts,
+                     int64_t P, int maxcor, int maxiter, int maxls, double gtol, double ftol, Eval&& eval, double* x_out,
+                     double* f_out, int32_t* success, int64_t* nfev) {
+  const int m = maxcor;
   const size_t PD = (size_t)P * D;
   // per-problem state + compact evaluation buffers (freed on return)
   tb::DevBuf bx, bf, bg, bd, bt, bS, bY, brho, bgam, bint, bnfev, btrial, bidx, bxt, bval, bgrad, bbox, bcount, bres;
@@ -2665,15 +2735,7 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   for (int64_t round = 0; n_active > 0 && round < max_rounds; ++round) {
     const auto t_round = std::chrono::steady_clock::now();
     const int n_round = n_active;
-    tb::EvalRequest rq;
-    rq.acq = acq;
-    rq.pen = pen;
-    rq.param = param;
-    rq.Xc = bxt.as<double>();
-    rq.M = n_active;
-    rq.out_vals = bval.as<double>();
-    rq.out_grad = bgrad.as<double>();
-    TB_TRY(tb::run_eval(gp, rq));
+    TB_TRY(eval(bxt.as<double>(), bidx.as<int>(), n_active, bval.as<double>(), bgrad.as<double>()));
     tb::lb::lbfgs_step_kernel<<<(unsigned)((n_active + 7) / 8), 256, 0, st>>>(s, o, n_active, bidx.as<int>(), bxt.as<double>(),
                                                                              bval.as<double>(), bgrad.as<double>(), dlo, dup);
     TB_LAUNCHED();
@@ -2683,7 +2745,7 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   if (trace) {
     double total = 0.0;
     for (auto& r : trace_rows) total += r.second;
-    std::fprintf(stderr, "[tb_acq_maximize] P=%lld rounds=%zu total=%.2f ms:", (long long)P, trace_rows.size(), total);
+    std::fprintf(stderr, "[%s] P=%lld rounds=%zu total=%.2f ms:", name, (long long)P, trace_rows.size(), total);
     for (auto& r : trace_rows) std::fprintf(stderr, " %d:%.2f", r.first, r.second);
     std::fprintf(stderr, "\n");
   }
@@ -2700,6 +2762,65 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
   return 0;
+}
+}  // namespace tb
+
+extern "C" {
+
+int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const double* upper, const double* starts, int64_t P,
+                    int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
+                    int32_t* success, int64_t* nfev) {
+  TB_CHECK(gp && lower && upper, "tb_acq_maximize: null argument");
+  TB_CHECK(P >= 0 && P < ((int64_t)1 << 31), "tb_acq_maximize: number of starts out of range");
+  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_acq_maximize: null argument");
+  bool pen = false;
+  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_maximize"));
+  if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
+    TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
+  if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
+  TB_TRY(tb::check_lbfgs_options("tb_acq_maximize", maxcor, maxiter, maxls, gtol, ftol));
+  TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
+  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_maximize"));
+  if (P == 0) return 0;
+  TB_CUDA(cudaSetDevice(gp->device));
+  auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad) -> int {
+    tb::EvalRequest rq;
+    rq.acq = acq;
+    rq.pen = pen;
+    rq.param = param;
+    rq.Xc = xt;
+    rq.M = n;
+    rq.out_vals = vals;
+    rq.out_grad = grad;
+    return tb::run_eval(gp, rq);
+  };
+  return tb::lbfgs_run("tb_acq_maximize", gp->stream, gp->D, lower, upper, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
+                       x_out, f_out, success, nfev);
+}
+
+int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const double* starts, int64_t R, int maxcor,
+                    int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
+                    int64_t* nfev) {
+  TB_CHECK(r && lower && upper, "tb_rff_maximize: null argument");
+  TB_TRY(tb::check_rff_paired(r, "tb_rff_maximize"));
+  TB_CHECK(R >= 0 && R * r->nb < ((int64_t)1 << 31), "tb_rff_maximize: number of starts out of range");
+  const int64_t P = R * r->nb;
+  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_rff_maximize: null argument");
+  TB_TRY(tb::check_lbfgs_options("tb_rff_maximize", maxcor, maxiter, maxls, gtol, ftol));
+  if (P == 0) return 0;
+  TB_CUDA(cudaSetDevice(r->device));
+  const int D = r->D;
+  // problem p = (i, b) of the [R, nb, D] starts runs on trajectory p % nb; the step kernel maximises, so the values and gradients
+  // handed to it are those of -f_b
+  auto eval = [&](const double* xt, const int* idx, int n, double* vals, double* grad) -> int {
+    for (int64_t c0 = 0; c0 < n; c0 += tb::RFF_PAIRED_CHUNK) {
+      const int64_t mc = std::min<int64_t>(tb::RFF_PAIRED_CHUNK, n - c0);
+      TB_TRY(tb::launch_rff_paired(r, xt + c0 * D, mc, 0, idx + c0, -1.0, vals + c0, grad + c0 * D));
+    }
+    return 0;
+  };
+  return tb::lbfgs_run("tb_rff_maximize", r->stream, D, lower, upper, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval, x_out,
+                       f_out, success, nfev);
 }
 
 int tb_gp_covariance_between_points(tb_gp* gp, const void* X1, int64_t M1, const void* X2, int64_t M2, void* out) {

@@ -253,7 +253,8 @@ class ResampleableRandomFourierFeatureFunctions:
 class feature_decomposition_trajectory:
     """sampler.py:858-953: f(x) = phi(x) . theta + m(x) for a batch of B trajectories (B fixed by the
     first call); ``[N, B, D] -> [N, B, 1]``.  The cos-feature projection runs in one CUDA kernel
-    that never materialises the [N*B, F] feature matrix."""
+    that never materialises the [N*B, F] feature matrix; for B > 1 each point is evaluated under its own trajectory only
+    (``tb_rff_eval_paired``), which also gives ``value_and_gradient`` and the device L-BFGS of ``minimize_from``."""
 
     def __init__(self, feature_functions: ResampleableRandomFourierFeatureFunctions, weight_sampler, model):
         self._feature_functions = feature_functions
@@ -293,11 +294,12 @@ class feature_decomposition_trajectory:
         th = np.ascontiguousarray(self._weights_sample, dtype=np.float64)
         _lib.check(_lib.lib().tb_rff_set_theta(self._h, th.ctypes.data_as(C.POINTER(C.c_double)), th.shape[0]))
 
-    def __call__(self, x):
+    def _batch(self, x):
+        """x [N, B, D] as a contiguous fp64 array; the first call fixes the batch size B and draws the weights."""
         x, _ = _lib.as_f64_contiguous(x)
         if x.ndim != 3:
             raise ValueError(f"trajectory inputs must be [N, B, D], got shape {tuple(x.shape)}")
-        N, B, D = x.shape
+        B = x.shape[1]
         if not self._initialized:
             self._batch_size = B
             self.resample()
@@ -307,24 +309,55 @@ class feature_decomposition_trajectory:
                 f"This trajectory only supports batch sizes of {self._batch_size}. If you wish to change the batch "
                 "size you must get a new trajectory by calling the get_trajectory method of the trajectory sampler."
             )
+        return x
+
+    def __call__(self, x):
+        x = self._batch(x)
+        N, B, D = x.shape
         if B == 1:
             flat = x.reshape(N, D)
             out, po = _lib.empty_like_kind(flat, (N, 1))
             _lib.check(_lib.lib().tb_rff_eval(self._h, _ptr(flat), N, po, None, None))
             return out.reshape(N, 1, 1)
-        # B > 1: trajectory b is evaluated on its own column of inputs
-        outs = []
-        for b in range(B):
-            col = x[:, b, :]
-            col = col.contiguous() if _lib.is_torch(col) else np.ascontiguousarray(col)
-            o, po = _lib.empty_like_kind(col, (N, B))
-            _lib.check(_lib.lib().tb_rff_eval(self._h, _ptr(col), N, po, None, None))
-            outs.append(o[:, b])
-        if _lib.is_torch(x):
-            import torch
+        # B > 1: point (n, b) under trajectory b only, one paired launch per chunk
+        out, po = _lib.empty_like_kind(x, (N, B, 1))
+        _lib.check(_lib.lib().tb_rff_eval_paired(self._h, _ptr(x), N, B, po, None))
+        return out
 
-            return torch.stack(outs, dim=1)[..., None]
-        return np.stack(outs, axis=1)[..., None]
+    def value_and_gradient(self, x):
+        """x [N, B, D] -> (f_b(x_nb) [N, B, 1], grad_x f_b(x_nb) [N, B, D]): each point under its own trajectory."""
+        x = self._batch(x)
+        N, B, D = x.shape
+        out, po = _lib.empty_like_kind(x, (N, B, 1))
+        grad, pg = _lib.empty_like_kind(x, (N, B, D))
+        _lib.check(_lib.lib().tb_rff_eval_paired(self._h, _ptr(x), N, B, po, pg))
+        return out, grad
+
+    def minimize_from(self, starts, lower, upper, *, maxcor: int = 10, maxiter: int = 15000, maxls: int = 20,
+                      gtol: float = 1e-5, ftol: float = 2.220446049250313e-09):
+        """Device-side multi-start projected L-BFGS (``tb_rff_maximize`` on -f_b): start (i, b) of ``starts`` [R, B, D]
+        minimises trajectory b inside the box, with SciPy's option names and defaults.  Returns (success [R, B] bool,
+        f_b at the end points [R, B], x [R, B, D], nfev [R, B]).  The negated trajectory of the continuous
+        Thompson-sampling builders offers it as ``maximize_from``."""
+        x0 = starts.detach().cpu().numpy() if hasattr(starts, "detach") else starts
+        x0 = np.ascontiguousarray(x0, dtype=np.float64)
+        if x0.ndim != 3:
+            raise ValueError(f"starts must be [R, B, D], got {x0.shape}")
+        self._batch(x0[:1])
+        R, B, D = x0.shape
+        lo = np.ascontiguousarray(np.broadcast_to(np.asarray(lower, dtype=np.float64), (D,)))
+        up = np.ascontiguousarray(np.broadcast_to(np.asarray(upper, dtype=np.float64), (D,)))
+        x = np.empty((R, B, D))
+        f = np.empty((R, B))
+        ok = np.zeros((R, B), dtype=np.int32)
+        nfev = np.zeros((R, B), dtype=np.int64)
+        _lib.check(
+            _lib.lib().tb_rff_maximize(
+                self._h, lo.ctypes.data, up.ctypes.data, x0.ctypes.data, R, int(maxcor), int(maxiter), int(maxls),
+                float(gtol), float(ftol), x.ctypes.data, f.ctypes.data, ok.ctypes.data, nfev.ctypes.data,
+            )
+        )
+        return ok.astype(bool), -f, x, nfev
 
     def argmin_over(self, candidates):
         """Fused evaluate + argmin of every trajectory over one shared candidate set [M, D]:
