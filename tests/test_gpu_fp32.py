@@ -21,6 +21,12 @@ def _pair32(obj, N, D):
     return om32, nm
 
 
+def _assert_fp32_gradient(grad, ref):
+    """the stated fp32 tolerance, 1e-4 of each candidate's gradient scale (its largest component)"""
+    err = np.abs(grad.astype(np.float64) - ref) / np.abs(ref).max(axis=1, keepdims=True)
+    assert err.max() < 1e-4, (err.max(), int(np.argmax(err.max(axis=1))))
+
+
 @pytest.mark.parametrize("N,D", [(300, 6), (1024, 20)])
 def test_fp32_predict_and_log_ei(N, D):
     from trieste_b200.acquisition import log_expected_improvement
@@ -39,6 +45,9 @@ def test_fp32_predict_and_log_ei(N, D):
     assert val.dtype == np.float32 and grad.dtype == np.float32 and grad.shape == (3000, 1, D)
     ref = o.log_expected_improvement(omean, ovar, eta)
     np.testing.assert_allclose(val, ref, rtol=1e-4, atol=1e-4)
+    # 3000 candidates in one chunk: one warp per candidate in the gradient assembly
+    _, rg = o.log_ei_gradient(om, Xq.astype(np.float64), eta)
+    _assert_fp32_gradient(grad[:, 0, :], rg)
     idx, best = fn.fused_argmax(Xq)
     assert idx == int(np.argmax(ref[:, 0])) or abs(ref[idx, 0] - ref.max()) < 1e-4
 

@@ -282,7 +282,7 @@ def test_exact_thompson_sampler_and_rule_default():
 
 
 @pytest.mark.parametrize("engine", ["int8", "fp64"])
-@pytest.mark.parametrize("kind", ["rbf", "matern52"])
+@pytest.mark.parametrize("kind", ["rbf", "matern32", "matern52"])
 def test_covariance_between_points_matches_oracle(kind, engine):
     # models.py:188-254 (reference test: tests/unit/models/gpflow/test_models.py:282-305)
     om, nm = model_pair(o.hartmann_6, 300, 6, kind=kind, engine=engine)

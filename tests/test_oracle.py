@@ -98,6 +98,32 @@ def test_ei_eta_is_min_posterior_mean_and_gradient_fd():
         np.testing.assert_allclose(g[:, d], fd[:, 0], rtol=1e-4, atol=1e-9 * np.abs(g).max())
 
 
+@pytest.mark.parametrize(
+    "kind,D,exact",
+    [(k, D, False) for k in o.KERNEL_KINDS for D in (1, 6, 13)] + [("matern12", D, True) for D in (1, 6, 13)],
+    ids=lambda v: ("exact_L" if v else "oracle_L") if isinstance(v, bool) else str(v),
+)
+def test_posterior_gradients_match_central_differences(kind, D, exact):
+    # the GPU gradient tests hold the kernels to posterior_gradients at 1e-9 of the scale; this pins both of its terms,
+    # dmean and dvar, for every kernel, to central differences of predict.  exact: with the difference-form Cholesky the
+    # Matern-12 GPU tests compare against (tests/util.py)
+    from tests.util import with_exact_cholesky
+
+    om = o.synthetic_model(o.ackley, 64, D, kind=kind)
+    if exact:
+        om = with_exact_cholesky(om)
+    Xq = np.random.default_rng(3).uniform(size=(8, D))
+    dmean, dvar = o.posterior_gradients(om, Xq)
+    h = 1e-6
+    for d in range(D):
+        e = np.zeros(D)
+        e[d] = h
+        mp, vp = o.predict(om, Xq + e)
+        mm, vm = o.predict(om, Xq - e)
+        np.testing.assert_allclose(dmean[:, d], (mp - mm)[:, 0] / (2 * h), rtol=1e-5, atol=1e-7 * np.abs(dmean).max())
+        np.testing.assert_allclose(dvar[:, d], (vp - vm)[:, 0] / (2 * h), rtol=1e-5, atol=1e-7 * np.abs(dvar).max())
+
+
 def test_qei_q1_matches_ei_and_mvn_samples():
     # test_function.py:1359-1394 restated
     om = o.synthetic_model(o.branin, 20, 2)
