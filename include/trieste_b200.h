@@ -243,6 +243,12 @@ int tb_rff_eval_paired(tb_rff* r, const void* Xc, int64_t M, int B, void* out, v
 int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const double* starts, int64_t R, int maxcor,
                     int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
                     int64_t* nfev);
+/* tb_rff_maximize with one box per batch column (BatchTrustRegionBox over a TaggedMultiSearchSpace, acquisition/optimizer.py
+ * round robin): lower/upper [nbox, D], start (i, b) maximises -f_b inside box b % nbox.  nbox must divide nb (TB_ERR_INVALID
+ * otherwise); tb_rff_maximize is this call with nbox = 1. */
+int tb_rff_maximize_boxes(tb_rff* r, const double* lower, const double* upper, int nbox, const double* starts, int64_t R,
+                          int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
+                          int32_t* success, int64_t* nfev);
 /* (K(X,X) + noise I)^-1 B = Linv^T (Linv B) through the cached triangular inverse: B, out [nrhs][N] (each right-hand side contiguous);
  * the v-weights of a decoupled trajectory (sampler.py:716, gpflux compute_A_inv_b).  fp64, host or device. */
 int tb_gp_kinv_apply(tb_gp* gp, const double* B, int nrhs, double* out);

@@ -63,6 +63,7 @@ SIGNATURES = {
     "tb_rff_set_canonical": (_i32, [_vp, _i32, C.POINTER(_f64), _i64, _vp, _i32]),
     "tb_rff_eval_paired": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp]),
     "tb_rff_maximize": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
+    "tb_rff_maximize_boxes": (_i32, [_vp, _vp, _vp, _i32, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
     "tb_gp_kinv_apply": (_i32, [_vp, _vp, _i32, _vp]),
     "tb_launch_count": (_i64, []),
     "tb_launch_count_reset": (None, []),

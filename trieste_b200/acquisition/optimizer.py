@@ -24,7 +24,7 @@ from typing import Callable, Iterator, Optional, Tuple, Union
 
 import numpy as np
 
-from ..space import Box, DiscreteSearchSpace, SearchSpace
+from ..space import Box, DiscreteSearchSpace, SearchSpace, TaggedMultiSearchSpace
 
 NUM_SAMPLES_MIN = 5000  # optimizer.py:46-66
 NUM_SAMPLES_DIM = 1000
@@ -105,6 +105,20 @@ def sample_from_space(num_samples: int, batch_size: Optional[int] = None, vector
     return sampler
 
 
+def _tile_samples(samples: np.ndarray, V: int, what: str) -> np.ndarray:
+    """Samples [n, D] or, from a multi-region space, [n, S, D] -> [n, V, D]: column v holds a sample of subspace v mod S."""
+    if samples.ndim == 3:
+        if V % samples.shape[1] != 0:
+            raise ValueError(
+                f"The vectorization of the target function {V} must be a multiple of the batch shape of {what} "
+                f"{samples.shape[1]}."
+            )
+        return np.tile(samples, [1, V // samples.shape[1], 1])
+    if samples.ndim == 2:
+        return np.tile(samples[:, None, :], [1, V, 1])
+    raise ValueError(f"The {what} must be a tensor of rank 2, got a tensor of rank {samples.ndim}.")
+
+
 def generate_initial_points(num_initial_points: int, initial_sampler, space: SearchSpace, target_func,
                             vectorization: int = 1) -> np.ndarray:
     """optimizer.py:247-341: running top-k of the acquisition values over the sampler's chunks.
@@ -115,18 +129,7 @@ def generate_initial_points(num_initial_points: int, initial_sampler, space: Sea
     top_cands = None  # [V, k, D]
     V = vectorization
     for candidates in initial_sampler(space):
-        candidates = np.asarray(candidates)
-        if candidates.ndim == 3:
-            if V % candidates.shape[1] != 0:
-                raise ValueError(
-                    f"The vectorization of the target function {V} must be a multiple of the batch shape of initial "
-                    f"samples {candidates.shape[1]}."
-                )
-            tiled = np.tile(candidates, [1, V // candidates.shape[1], 1])
-        elif candidates.ndim == 2:
-            tiled = np.tile(candidates[:, None, :], [1, V, 1])
-        else:
-            raise ValueError(f"The initial samples must be a tensor of rank 2, got a tensor of rank {candidates.ndim}.")
+        tiled = _tile_samples(np.asarray(candidates), V, "initial samples")
         values = _to_numpy(target_func(tiled))  # [samples, V]
         if values.ndim != 2 or values.shape[-1] != V:
             raise ValueError(
@@ -169,8 +172,11 @@ def _value_and_gradient(fn, x: np.ndarray):
 
 
 def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points: np.ndarray, optimizer_args: dict):
-    """Maximise ``fn`` from every start [R, V, D] inside the box.  Returns
-    (success [R, V] bool, fun [R, V] (maximised values), x [R, V, D], nfev [R, V])."""
+    """Maximise ``fn`` from every start [R, V, D], problem p = (r, v) = r * V + v inside box p mod nbox of ``lower`` /
+    ``upper``: one box [D], one box per subspace of a multi-region space [nbox, D] with nbox dividing V (column v searches
+    subspace v mod nbox, the reference's round robin, optimizer.py:859-890), or one box per problem [R * V, D].  Returns
+    (success [R, V] bool, fun [R, V] (maximised values), x [R, V, D], nfev [R, V]).  The device optimisers take at most
+    one box per column, so per-problem boxes need the host implementation (``TB_LBFGS=host``)."""
     m = int(optimizer_args.get("maxcor", 10))
     maxiter = int(optimizer_args.get("maxiter", 15000))
     gtol = float(optimizer_args.get("gtol", 1e-5))
@@ -179,12 +185,26 @@ def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points:
 
     R, V, D = starting_points.shape
     P = R * V
+    boxes = [np.atleast_2d(np.asarray(b, dtype=np.float64)) for b in (lower, upper)]
+    nbox = max(len(boxes[0]), len(boxes[1]))
+    if V % nbox != 0 and nbox != P:
+        raise ValueError(f"The vectorization of the target function {V} must be a multiple of the number of subspaces {nbox}.")
+    lo_b, up_b = (np.broadcast_to(b, (nbox, D)) for b in boxes)
     if hasattr(fn, "maximize_from") and os.environ.get("TB_LBFGS", "device") != "host" and m <= 16:
         # the whole multi-start loop runs on the device: tb_acq_maximize for the fused single-model functions (starts
-        # [P, D]), tb_rff_maximize for the negated trajectories of continuous Thompson sampling (starts [R, V, D])
+        # [P, D], one box), tb_rff_maximize_boxes for the negated trajectories of continuous Thompson sampling (starts
+        # [R, V, D], column v in box v mod nbox)
+        if V % nbox != 0:
+            raise ValueError(
+                f"{nbox} per-problem boxes for {V} columns: the device L-BFGS takes one box per column at most; set "
+                "TB_LBFGS=host for one box per problem"
+            )
         starts = starting_points.reshape(P, D) if V == 1 else starting_points
-        ok, fun, xs, nf = fn.maximize_from(starts, lower, upper, maxcor=m, maxiter=maxiter, maxls=maxls, gtol=gtol, ftol=ftol)
+        lo_d, up_d = (lo_b[0], up_b[0]) if nbox == 1 else (lo_b, up_b)
+        ok, fun, xs, nf = fn.maximize_from(starts, lo_d, up_d, maxcor=m, maxiter=maxiter, maxls=maxls, gtol=gtol, ftol=ftol)
         return ok.reshape(R, V), fun.reshape(R, V), xs.reshape(R, V, D), nf.reshape(R, V)
+    box_of = np.arange(P) % nbox
+    lower, upper = lo_b[box_of], up_b[box_of]  # [P, D]: the box of every problem
     x = np.clip(starting_points.reshape(P, D).astype(np.float64), lower, upper)
 
     def evaluate(idx, pts):
@@ -212,10 +232,10 @@ def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points:
     done = ~np.isfinite(f)
     success = np.zeros(P, dtype=bool)
 
-    def proj_grad(xx, gg):
-        return xx - np.clip(xx - gg, lower, upper)
+    def proj_grad(idx, xx, gg):
+        return xx - np.clip(xx - gg, lower[idx], upper[idx])
 
-    conv = np.max(np.abs(proj_grad(x, g)), axis=1) <= gtol
+    conv = np.max(np.abs(proj_grad(np.arange(P), x, g)), axis=1) <= gtol
     success |= conv & ~done
     done |= conv
 
@@ -225,7 +245,7 @@ def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points:
             break
         xa, ga = x[act], g[act]
         # free variables: not pinned at a bound with the gradient pushing outward
-        free = ~(((xa <= lower) & (ga > 0)) | ((xa >= upper) & (ga < 0)))
+        free = ~(((xa <= lower[act]) & (ga > 0)) | ((xa >= upper[act]) & (ga < 0)))
         q = np.where(free, ga, 0.0)
         order = [(head - 1 - i) % m for i in range(m)]  # newest first
         alphas = []
@@ -259,7 +279,7 @@ def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points:
             pidx = np.nonzero(pending)[0]
             if pidx.size == 0:
                 break
-            xt = np.clip(xa[pidx] + t[pidx, None] * d[pidx], lower, upper)
+            xt = np.clip(xa[pidx] + t[pidx, None] * d[pidx], lower[act[pidx]], upper[act[pidx]])
             ft, gt = evaluate(act[pidx], xt)
             nfev[act[pidx]] += 1
             step = xt - xa[pidx]
@@ -291,7 +311,7 @@ def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points:
 
         f_old = f[ai].copy()
         x[ai], f[ai], g[ai] = x_new[acc], f_new[acc], g_new[acc]
-        conv_g = np.max(np.abs(proj_grad(x[ai], g[ai])), axis=1) <= gtol
+        conv_g = np.max(np.abs(proj_grad(ai, x[ai], g[ai])), axis=1) <= gtol
         conv_f = (f_old - f[ai]) <= ftol * np.maximum(np.maximum(np.abs(f_old), np.abs(f[ai])), 1.0)
         conv = conv_g | conv_f
         success[ai[conv]] = True
@@ -302,10 +322,11 @@ def _perform_parallel_continuous_optimization(fn, lower, upper, starting_points:
 
 def generate_continuous_optimizer(num_initial_samples: int = NUM_SAMPLES_MIN, num_optimization_runs: int = 10,
                                   num_recovery_runs: int = 10, optimizer_args: Optional[dict] = None):
-    """optimizer.py:344-563 for ``Box`` spaces: best ``num_optimization_runs`` of
+    """optimizer.py:344-563 for ``Box`` and ``TaggedMultiSearchSpace`` spaces: best ``num_optimization_runs`` of
     ``num_initial_samples`` random points -> parallel local maximisation -> argmax over runs;
     recovery runs from fresh random starts if every run failed; ``FailedOptimizationError``
-    otherwise."""
+    otherwise.  Over a multi-region space of S subspaces, column v of a function vectorised over V (a multiple of S)
+    starts from and stays in subspace v mod S."""
     if num_initial_samples <= 0:
         raise ValueError(f"num_initial_samples must be positive, got {num_initial_samples}")
     if num_optimization_runs <= 0:
@@ -318,9 +339,9 @@ def generate_continuous_optimizer(num_initial_samples: int = NUM_SAMPLES_MIN, nu
         raise ValueError(f"num_recovery_runs must be zero or greater, got {num_recovery_runs}")
     args = dict(optimizer_args or {})
 
-    def optimize_continuous(space: Box, target_func: TargetFunc) -> np.ndarray:
-        if not isinstance(space, Box):
-            raise NotImplementedError("generate_continuous_optimizer here supports Box search spaces")
+    def optimize_continuous(space: SearchSpace, target_func: TargetFunc) -> np.ndarray:
+        if not isinstance(space, (Box, TaggedMultiSearchSpace)):
+            raise NotImplementedError("generate_continuous_optimizer here supports Box and TaggedMultiSearchSpace search spaces")
         fn, V = _split(target_func)
         initial = generate_initial_points(
             num_optimization_runs, sample_from_space(num_initial_samples), space, fn, vectorization=V
@@ -331,7 +352,7 @@ def generate_continuous_optimizer(num_initial_samples: int = NUM_SAMPLES_MIN, nu
         recovery = 0
         while not np.all(ok_any) and recovery < num_recovery_runs:
             # optimizer.py:462-522: random restarts until some run succeeds for every function
-            rnd = np.tile(space.sample(1)[:, None, :], [1, V, 1])
+            rnd = _tile_samples(space.sample(1), V, "random samples")
             s2, f2, x2, n2 = _perform_parallel_continuous_optimization(fn, space.lower, space.upper, rnd, args)
             success = np.concatenate([success, s2])
             fun = np.concatenate([fun, f2])
@@ -412,7 +433,7 @@ def automatic_optimizer_selector(space: SearchSpace, target_func: TargetFunc) ->
     """optimizer.py:90-121."""
     if isinstance(space, DiscreteSearchSpace):
         return optimize_discrete(space, target_func)
-    if isinstance(space, Box):
+    if isinstance(space, (Box, TaggedMultiSearchSpace)):
         num_samples = max(NUM_SAMPLES_MIN, NUM_SAMPLES_DIM * space.dimension)
         num_runs = NUM_RUNS_DIM * space.dimension
         return generate_continuous_optimizer(num_initial_samples=num_samples, num_optimization_runs=num_runs)(space, target_func)

@@ -3,7 +3,9 @@
 // history; one warp owns one problem (lane = input dimension, D <= 32), so the two-loop recursion is m warp-reductions.
 // The host loop is: batched value+gradient evaluation of the trial points of all ACTIVE problems (the fused GP kernels)
 // -> lbfgs_step_kernel (line-search decision, history update, convergence tests, next direction and trial point)
-// -> compaction of the active set.  Minimises f = -acquisition inside the box [lower, upper].
+// -> compaction of the active set.  Minimises f = -acquisition inside problem p's box: lower/upper hold nbox boxes [nbox, D]
+// and problem p uses box p % nbox (with starts laid out [R, nb, D] and nbox | nb, column b uses box b % nbox).  The box is
+// looked up from the original problem index, never from a compacted slot.
 #pragma once
 #include "common.cuh"
 
@@ -24,7 +26,7 @@ struct State {
 };
 
 struct Options {
-  int D, m, maxiter, maxls;
+  int D, m, maxiter, maxls, nbox;
   double gtol, ftol;
 };
 
@@ -90,7 +92,8 @@ lbfgs_step_kernel(State s, Options o, int n_active, const int* __restrict__ idx,
   const long long p = idx[w];
   const int D = o.D, m = o.m;
   const bool in = lane < D;
-  const double lo = in ? lower[lane] : 0.0, up = in ? upper[lane] : 0.0;
+  const long long box = (p % o.nbox) * D;
+  const double lo = in ? lower[box + lane] : 0.0, up = in ? upper[box + lane] : 0.0;
   const double xn = in ? xt[(long long)w * D + lane] : 0.0;
   const double fn = -acq_val[w];
   const double gn = in ? -acq_grad[(long long)w * D + lane] : 0.0;
@@ -217,13 +220,14 @@ __global__ void lbfgs_gather_kernel(const double* __restrict__ xtrial, const int
   xt[e] = xtrial[(long long)idx[i] * D + d];
 }
 
-// starting points clipped into the box; all problems active in phase INIT
+// starting points clipped into their problems' boxes; all problems active in phase INIT
 __global__ void lbfgs_init_kernel(const double* __restrict__ starts, long long P, int D, const double* __restrict__ lower,
-                                  const double* __restrict__ upper, State s) {
+                                  const double* __restrict__ upper, int nbox, State s) {
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= P * D) return;
   const int d = (int)(e % D);
-  s.xtrial[e] = clampd(starts[e], lower[d], upper[d]);
+  const long long b = ((e / D) % nbox) * D + d;
+  s.xtrial[e] = clampd(starts[e], lower[b], upper[b]);
   s.x[e] = s.xtrial[e];
   s.g[e] = 0.0;
   s.d[e] = 0.0;

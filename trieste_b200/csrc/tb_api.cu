@@ -2679,12 +2679,13 @@ static int check_lbfgs_options(const std::string& name, int maxcor, int maxiter,
   return 0;
 }
 
-// The multi-start L-BFGS round loop shared by every device maximiser: P (>= 1) problems in D dimensions on the stream st; each
+// The multi-start L-BFGS round loop shared by every device maximiser: P (>= 1) problems in D dimensions on the stream st, problem
+// p inside box p % nbox of lower/upper [nbox, D]; each
 // round asks eval(xt [n, D], idx [n], n, vals [n], grad [n, D]) for the values and gradients of the function to MAXIMISE at the
 // trial points of the n active problems (all device arrays; idx holds their problem indices), then runs one step of each.
 template <class Eval>
-static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* lower, const double* upper, const double* starts,
-                     int64_t P, int maxcor, int maxiter, int maxls, double gtol, double ftol, Eval&& eval, double* x_out,
+static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* lower, const double* upper, int nbox,
+                     const double* starts, int64_t P, int maxcor, int maxiter, int maxls, double gtol, double ftol, Eval&& eval, double* x_out,
                      double* f_out, int32_t* success, int64_t* nfev) {
   const int m = maxcor;
   const size_t PD = (size_t)P * D;
@@ -2695,7 +2696,7 @@ static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* low
   TB_TRY(bS.reserve(8 * PD * m)); TB_TRY(bY.reserve(8 * PD * m)); TB_TRY(brho.reserve(8 * (size_t)P * m));
   TB_TRY(bint.reserve(sizeof(int) * 6 * (size_t)P)); TB_TRY(bnfev.reserve(8 * (size_t)P));
   TB_TRY(bidx.reserve(sizeof(int) * (size_t)P)); TB_TRY(bxt.reserve(8 * PD)); TB_TRY(bval.reserve(8 * (size_t)P));
-  TB_TRY(bgrad.reserve(8 * PD)); TB_TRY(bbox.reserve(8 * 2 * (size_t)D)); TB_TRY(bcount.reserve(sizeof(int)));
+  TB_TRY(bgrad.reserve(8 * PD)); TB_TRY(bbox.reserve(8 * 2 * (size_t)nbox * D)); TB_TRY(bcount.reserve(sizeof(int)));
   tb::lb::State s;
   s.x = bx.as<double>(); s.f = bf.as<double>(); s.g = bg.as<double>(); s.d = bd.as<double>(); s.t = bt.as<double>();
   s.S = bS.as<double>(); s.Y = bY.as<double>(); s.rho = brho.as<double>(); s.gam = bgam.as<double>();
@@ -2704,16 +2705,16 @@ static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* low
   s.nfev = bnfev.as<long long>();
   s.xtrial = btrial.as<double>();
   double* dlo = bbox.as<double>();
-  double* dup = dlo + D;
-  TB_CUDA(cudaMemcpyAsync(dlo, lower, 8 * (size_t)D, cudaMemcpyDefault, st));
-  TB_CUDA(cudaMemcpyAsync(dup, upper, 8 * (size_t)D, cudaMemcpyDefault, st));
+  double* dup = dlo + (size_t)nbox * D;
+  TB_CUDA(cudaMemcpyAsync(dlo, lower, 8 * (size_t)nbox * D, cudaMemcpyDefault, st));
+  TB_CUDA(cudaMemcpyAsync(dup, upper, 8 * (size_t)nbox * D, cudaMemcpyDefault, st));
   TB_CUDA(cudaMemcpyAsync(bxt.p, starts, 8 * PD, cudaMemcpyDefault, st));  // staged through the trial buffer
   TB_CUDA(cudaMemsetAsync(bS.p, 0, 8 * PD * m, st));
   TB_CUDA(cudaMemsetAsync(bY.p, 0, 8 * PD * m, st));
   TB_CUDA(cudaMemsetAsync(brho.p, 0, 8 * (size_t)P * m, st));
-  tb::lb::lbfgs_init_kernel<<<(unsigned)((PD + 255) / 256), 256, 0, st>>>(bxt.as<double>(), P, D, dlo, dup, s);
+  tb::lb::lbfgs_init_kernel<<<(unsigned)((PD + 255) / 256), 256, 0, st>>>(bxt.as<double>(), P, D, dlo, dup, nbox, s);
   TB_LAUNCHED();
-  tb::lb::Options o{D, m, maxiter, maxls, gtol, ftol};
+  tb::lb::Options o{D, m, maxiter, maxls, nbox, gtol, ftol};
   int n_active = 0;
   auto compact = [&]() -> int {
     tb::lb::lbfgs_compact_kernel<<<1, 1024, 0, st>>>(s.status, P, bidx.as<int>(), bcount.as<int>());
@@ -2794,15 +2795,17 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
     rq.out_grad = grad;
     return tb::run_eval(gp, rq);
   };
-  return tb::lbfgs_run("tb_acq_maximize", gp->stream, gp->D, lower, upper, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
+  return tb::lbfgs_run("tb_acq_maximize", gp->stream, gp->D, lower, upper, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
                        x_out, f_out, success, nfev);
 }
 
-int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const double* starts, int64_t R, int maxcor,
-                    int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
-                    int64_t* nfev) {
+int tb_rff_maximize_boxes(tb_rff* r, const double* lower, const double* upper, int nbox, const double* starts, int64_t R,
+                          int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
+                          int32_t* success, int64_t* nfev) {
   TB_CHECK(r && lower && upper, "tb_rff_maximize: null argument");
   TB_TRY(tb::check_rff_paired(r, "tb_rff_maximize"));
+  TB_CHECK(nbox >= 1 && r->nb % nbox == 0, "tb_rff_maximize_boxes: the number of boxes " + std::to_string(nbox) +
+                                               " must divide the trajectory batch size " + std::to_string(r->nb));
   TB_CHECK(R >= 0 && R * r->nb < ((int64_t)1 << 31), "tb_rff_maximize: number of starts out of range");
   const int64_t P = R * r->nb;
   TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_rff_maximize: null argument");
@@ -2810,8 +2813,8 @@ int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const d
   if (P == 0) return 0;
   TB_CUDA(cudaSetDevice(r->device));
   const int D = r->D;
-  // problem p = (i, b) of the [R, nb, D] starts runs on trajectory p % nb; the step kernel maximises, so the values and gradients
-  // handed to it are those of -f_b
+  // problem p = (i, b) of the [R, nb, D] starts runs on trajectory p % nb inside box p % nbox = b % nbox (nbox divides nb); the
+  // step kernel maximises, so the values and gradients handed to it are those of -f_b
   auto eval = [&](const double* xt, const int* idx, int n, double* vals, double* grad) -> int {
     for (int64_t c0 = 0; c0 < n; c0 += tb::RFF_PAIRED_CHUNK) {
       const int64_t mc = std::min<int64_t>(tb::RFF_PAIRED_CHUNK, n - c0);
@@ -2819,8 +2822,14 @@ int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const d
     }
     return 0;
   };
-  return tb::lbfgs_run("tb_rff_maximize", r->stream, D, lower, upper, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval, x_out,
-                       f_out, success, nfev);
+  return tb::lbfgs_run("tb_rff_maximize", r->stream, D, lower, upper, nbox, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
+                       x_out, f_out, success, nfev);
+}
+
+int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const double* starts, int64_t R, int maxcor,
+                    int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
+                    int64_t* nfev) {
+  return tb_rff_maximize_boxes(r, lower, upper, 1, starts, R, maxcor, maxiter, maxls, gtol, ftol, x_out, f_out, success, nfev);
 }
 
 int tb_gp_covariance_between_points(tb_gp* gp, const void* X1, int64_t M1, const void* X2, int64_t M2, void* out) {

@@ -335,25 +335,28 @@ class feature_decomposition_trajectory:
 
     def minimize_from(self, starts, lower, upper, *, maxcor: int = 10, maxiter: int = 15000, maxls: int = 20,
                       gtol: float = 1e-5, ftol: float = 2.220446049250313e-09):
-        """Device-side multi-start projected L-BFGS (``tb_rff_maximize`` on -f_b): start (i, b) of ``starts`` [R, B, D]
-        minimises trajectory b inside the box, with SciPy's option names and defaults.  Returns (success [R, B] bool,
-        f_b at the end points [R, B], x [R, B, D], nfev [R, B]).  The negated trajectory of the continuous
-        Thompson-sampling builders offers it as ``maximize_from``."""
+        """Device-side multi-start projected L-BFGS (``tb_rff_maximize_boxes`` on -f_b): start (i, b) of ``starts``
+        [R, B, D] minimises trajectory b inside its box, with SciPy's option names and defaults.  ``lower`` / ``upper`` are
+        one box [D] or ``nbox`` boxes [nbox, D] with nbox dividing B; column b uses box ``b % nbox`` (the round robin of a
+        multi-region search space).  Returns (success [R, B] bool, f_b at the end points [R, B], x [R, B, D], nfev [R, B]).
+        The negated trajectory of the continuous Thompson-sampling builders offers it as ``maximize_from``."""
         x0 = starts.detach().cpu().numpy() if hasattr(starts, "detach") else starts
         x0 = np.ascontiguousarray(x0, dtype=np.float64)
         if x0.ndim != 3:
             raise ValueError(f"starts must be [R, B, D], got {x0.shape}")
         self._batch(x0[:1])
         R, B, D = x0.shape
-        lo = np.ascontiguousarray(np.broadcast_to(np.asarray(lower, dtype=np.float64), (D,)))
-        up = np.ascontiguousarray(np.broadcast_to(np.asarray(upper, dtype=np.float64), (D,)))
+        lo, up = (np.atleast_2d(np.asarray(v, dtype=np.float64)) for v in (lower, upper))
+        nbox = max(lo.shape[0], up.shape[0])
+        lo = np.ascontiguousarray(np.broadcast_to(lo, (nbox, D)))
+        up = np.ascontiguousarray(np.broadcast_to(up, (nbox, D)))
         x = np.empty((R, B, D))
         f = np.empty((R, B))
         ok = np.zeros((R, B), dtype=np.int32)
         nfev = np.zeros((R, B), dtype=np.int64)
         _lib.check(
-            _lib.lib().tb_rff_maximize(
-                self._h, lo.ctypes.data, up.ctypes.data, x0.ctypes.data, R, int(maxcor), int(maxiter), int(maxls),
+            _lib.lib().tb_rff_maximize_boxes(
+                self._h, lo.ctypes.data, up.ctypes.data, nbox, x0.ctypes.data, R, int(maxcor), int(maxiter), int(maxls),
                 float(gtol), float(ftol), x.ctypes.data, f.ctypes.data, ok.ctypes.data, nfev.ctypes.data,
             )
         )
