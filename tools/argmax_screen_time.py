@@ -8,7 +8,7 @@ For each: median time per fused_argmax call with TB_ARGMAX_SCREEN=1 and =0, the 
 process; the candidates that went through the variance GEMM (profile counters: the survivors padded to whole tiles, plus
 the probe's tile) against M; from one profiled screened call (torch.profiler, CUDA activities), the device time of the
 fp32 bound pass (mean_bounds_kernel), of the compaction and of the rest (probe, survivors' K* digits and means, GEMM, tail,
-folds); and the survivor count of the bound screen (acq(lo) >= tau - margin, lo from tb_gp_mean_bounds) next to the count
+folds), the rest and the compaction also per kernel name with their launch counts; and the survivor count of the bound screen (acq(lo) >= tau - margin, lo from tb_gp_mean_bounds) next to the count
 the same screen gives on the exact fp64 means (predict), tau being the call's exact best value (EI only).  The card name
 and power limit are read in the same run.
 
@@ -31,6 +31,15 @@ def card():
                        capture_output=True, text=True, check=True).stdout.strip()
     name, power, clock = [s.strip() for s in q.split(",")]
     return {"gpu": name, "power_limit": power, "sm_clock_max": clock}
+
+
+def kernel_name(key):
+    """'void tb::oz5::kstar_digits_kernel<3, 10, 5>(double const*, ...)' -> 'kstar_digits_kernel'; 'Memcpy HtoD (...)' ->
+    'Memcpy HtoD'"""
+    base = key.split("(")[0].split("<")[0].strip()
+    if not base.startswith("void "):
+        return base or key
+    return base.split()[-1].split("::")[-1]
 
 
 def main():
@@ -124,16 +133,21 @@ def main():
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             call(fn, x, 1)
         bound_us = compact_us = rest_us = 0.0
+        rest_by_kernel = {}
         for e in prof.key_averages():
             us = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
             if us <= 0:
                 continue
             if "mean_bounds_kernel" in e.key:
                 bound_us += us
-            elif "compact_kernel" in e.key:
+                continue
+            if "compact_kernel" in e.key:
                 compact_us += us
             else:
                 rest_us += us
+            name = kernel_name(e.key)
+            ms, cnt = rest_by_kernel.get(name, (0.0, 0))
+            rest_by_kernel[name] = (ms + us / 1e3, cnt + e.count)
         surv = survivors(m, fn, x, best[k][1][1])
         row[k] = {
             "candidates": int(x.shape[0]),
@@ -142,6 +156,7 @@ def main():
             "speedup": med(t[k][0]) / med(t[k][1]),
             "gemm_candidates": fl.value / float(N) ** 2, "gemm_launches": int(n.value),
             "device_ms": {"bound_pass": bound_us / 1e3, "compaction": compact_us / 1e3, "probe_survivors_rest": rest_us / 1e3},
+            "rest_by_kernel": {k: {"ms": v[0], "launches": v[1]} for k, v in sorted(rest_by_kernel.items(), key=lambda kv: -kv[1][0])},
             "survivors": surv,
             "best": list(best[k][1]),
         }

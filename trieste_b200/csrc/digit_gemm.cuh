@@ -18,6 +18,8 @@
 // K* digits stay in L2; the serpentine row-block assignment gives every group the same cost).
 //   EPI_SUMSQ: partial[g][t] = Σ_{rows n of group g} A[n,t]^2  (variance path)
 //   EPI_STORE: A itself, fp64, candidate-major [t][lda]  (joint / gradient paths)
+//   EPI_SPLIT: split-K over (tile, chunk, row-block, stage range) units, the int32 levels summed in a scratch, and
+//              split_epilogue_kernel runs the EPI_SUMSQ epilogue on the sums (the screened argmax's rounds of few tiles)
 // a_planes / b_planes: digit planes STORED per stage of the left / right operand (>= S): a GEMM computing with S digits reads
 // the S most significant planes of a wider split.  full_rows = 0: lower-triangular left factor (Linv), row-block I spans
 // stages [0, 2(I+1)), packed triangularly; full_rows = 1: dense square left factor, every row-block spans all nst stages.
@@ -60,9 +62,10 @@ constexpr int THREADS = CONSUMER_WARPS * 32 + 128;    // + the producer warpgrou
 // per-thread registers after setmaxnreg: 128 · 40 + 256 · 232 = 64512 of the 64K register file, which is also what the
 // launch allocates (168 per thread at __launch_bounds__(384, 1))
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
-enum { EPI_SUMSQ = 0, EPI_STORE = 1 };
+enum { EPI_SUMSQ = 0, EPI_STORE = 1, EPI_SPLIT = 2 };
 
-template <int S> __host__ __device__ constexpr int chunk_cols() { return S >= 6 ? 32 : 64; }
+__host__ __device__ constexpr int chunk_cols_of(int S) { return S >= 6 ? 32 : 64; }
+template <int S> __host__ __device__ constexpr int chunk_cols() { return chunk_cols_of(S); }
 template <int S> __host__ __device__ constexpr int stage_bytes() { return S * (ATILE + chunk_cols<S>() * KST); }
 template <int S> __host__ __device__ constexpr size_t smem_bytes() {  // stages + barriers + per-warp column sums
   return (size_t)STAGES * stage_bytes<S>() + 256 + (size_t)CONSUMER_WARPS * chunk_cols<S>() * sizeof(double);
@@ -127,12 +130,111 @@ __device__ __forceinline__ double int_to_double(uint32_t t) {
   return __hiloint2double(0x43300000, (int)(t ^ 0x80000000u)) - 4503601774854144.0;  // 2^52 + 2^31
 }
 
+__host__ __device__ inline int rowblock_stages(int I, int nst, int full_rows) { return full_rows ? nst : min(2 * (I + 1), nst); }
+
+// EPI_SPLIT work units per (candidate tile, chunk): every row-block's stages in ranges of kper, numbered by row-block, then range
+__host__ __device__ inline int split_units(int NB, int nst, int full_rows, int kper) {
+  int u = 0;
+  for (int I = 0; I < NB; ++I) u += (rowblock_stages(I, nst, full_rows) + kper - 1) / kper;
+  return u;
+}
+
+// The i-th (row-block I, stages [k0, k1)) of work item g of a (tile, chunk); false past the last.  EPI_SUMSQ / EPI_STORE: g is a
+// row-block group, whose row-blocks are taken whole in serpentine order; EPI_SPLIT: g is a unit, one range of one row-block.
+template <int EPI>
+__device__ __forceinline__ bool item_range(int g, int i, int G, int NB, int nst, int full_rows, int kper, int& I, int& k0, int& k1) {
+  if constexpr (EPI == EPI_SPLIT) {
+    if (i > 0) return false;
+    for (I = 0; I < NB; ++I) {
+      const int nk = rowblock_stages(I, nst, full_rows), p = (nk + kper - 1) / kper;
+      if (g < p) {
+        k0 = g * kper;
+        k1 = min(nk, k0 + kper);
+        return true;
+      }
+      g -= p;
+    }
+    return false;
+  } else {
+    I = serpentine_rowblock(i, g, G);
+    k0 = 0;
+    k1 = rowblock_stages(I, nst, full_rows);
+    return I < NB;
+  }
+}
+
+// The epilogue of one row-block from its S levels of int32 accumulators in the m64nCN fragment layout of consumer warp `warp`:
+// register 4j + e holds row 16 wq + lane/4 (+8 for e >= 2) of warpgroup wg's 64, column 8j + 2 (lane % 4) + (e & 1) of the
+// chunk.  EPI_SUMSQ adds the warp's 16 rows of A^2 to colbuf[warp] (row-blocks in the order of the calls); EPI_STORE writes A.
+template <int S, int EPI, int NTB>
+__device__ __forceinline__ void rowblock_epilogue(const uint32_t (&acc)[S][chunk_cols<S>() / 2], int I, int tile, int c, int warp, int lane,
+                                                  const double* __restrict__ rowscale, const double* __restrict__ rowsum,
+                                                  double out_scale, double half_var, double (*colbuf)[chunk_cols<S>()],
+                                                  double* __restrict__ Aplain, int64_t lda) {
+  constexpr int CN = chunk_cols<S>();
+  const int wg = warp >> 2, wq = warp & 3;
+  const int64_t r0 = (int64_t)I * 128 + wg * 64 + wq * 16 + (lane >> 2), r1 = r0 + 8;
+  const double rs0 = rowscale[r0] * out_scale * 0x1p-16, rs1 = rowscale[r1] * out_scale * 0x1p-16;
+  const double rc0 = rowsum ? rowsum[r0] * half_var : 0.0, rc1 = rowsum ? rowsum[r1] * half_var : 0.0;
+#pragma unroll
+  for (int j = 0; j < CN / 8; ++j) {
+    double a[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      // Horner over the levels, least significant first: v = ((T_{S+1} 2^-8 + T_S) 2^-8 + ...) + T_2
+      double v = int_to_double(acc[S - 1][4 * j + e]);
+#pragma unroll
+      for (int l = S - 2; l >= 0; --l) v = fma(v, 0x1p-8, int_to_double(acc[l][4 * j + e]));
+      a[e] = e < 2 ? fma(v, rs0, rc0) : fma(v, rs1, rc1);
+    }
+    const int col = 8 * j + 2 * (lane & 3);
+    if constexpr (EPI == EPI_STORE) {
+      double* dst = Aplain + ((int64_t)tile * NTB + (int64_t)c * CN + col) * lda;
+      dst[r0] = a[0];
+      dst[lda + r0] = a[1];
+      dst[r1] = a[2];
+      dst[lda + r1] = a[3];
+    } else {
+      double s0 = fma(a[0], a[0], a[2] * a[2]), s1 = fma(a[1], a[1], a[3] * a[3]);
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+      }
+      if (lane < 4) {  // the warp's 16 rows, accumulated over the item's row-blocks in a fixed order
+        colbuf[warp][col] += s0;
+        colbuf[warp][col + 1] += s1;
+      }
+    }
+  }
+}
+
+// EPI_SUMSQ, after an item's last row-block: dst[col] = Σ_w colbuf[w][col] in warp order, colbuf zeroed.  Threads 0 .. 255
+// (the consumer warps) take part.
+template <int CN>
+__device__ __forceinline__ void colbuf_flush(double (*colbuf)[CN], double* __restrict__ dst) {
+  asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_WARPS * 32) : "memory");
+  if (threadIdx.x < CN) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < CONSUMER_WARPS; ++w) {
+      s += colbuf[w][threadIdx.x];
+      colbuf[w][threadIdx.x] = 0.0;
+    }
+    dst[threadIdx.x] = s;
+  }
+  asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_WARPS * 32) : "memory");
+}
+
+// EPI_SPLIT (split-K for a few candidate tiles, whose row-block groups would leave most SMs idle): G units per (tile, chunk),
+// each adds its int32 level accumulators to the zeroed acc_out[(tile NCH + chunk) NB + I][S NR][256 consumer threads].
+// Integer addition is exact and commutative, so the sums are those one CTA would accumulate; split_epilogue_kernel finishes.
 template <int S, int EPI, int NTB>
 __global__ void __launch_bounds__(THREADS, 1)
 digit_gemm_kernel(const int8_t* __restrict__ AS, const int8_t* __restrict__ BS, const double* __restrict__ rowscale,
                   const double* __restrict__ rowsum, int NB, int nst, int G, int tiles, int64_t McPad, double out_scale,
                   double half_var, int a_planes, int b_planes, int full_rows, double* __restrict__ partial,
-                  double* __restrict__ Aplain, int64_t lda) {
+                  double* __restrict__ Aplain, int64_t lda, int kper, int* __restrict__ acc_out) {
   constexpr int CN = chunk_cols<S>(), NCH = NTB / CN, BCH = CN * KST, BTILE = NTB * KST, STAGE = stage_bytes<S>(), NR = CN / 2;
   static_assert(NTB % CN == 0, "a candidate tile is a whole number of column chunks");
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -161,12 +263,10 @@ digit_gemm_kernel(const int8_t* __restrict__ AS, const int8_t* __restrict__ BS, 
       for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
         const int g = item % G, tc = item / G, tile = tc / NCH, c = tc % NCH;
         const int8_t* bTile = BS + (int64_t)tile * nst * ((int64_t)b_planes * BTILE) + (int64_t)c * BCH;
-        for (int i = 0;; ++i) {
-          const int I = serpentine_rowblock(i, g, G);
-          if (I >= NB) break;
-          const int nk = full_rows ? nst : min(2 * (I + 1), nst);
+        int I, k0, k1;
+        for (int i = 0; item_range<EPI>(g, i, G, NB, nst, full_rows, kper, I, k0, k1); ++i) {
           const int8_t* aRow = AS + (full_rows ? (int64_t)I * nst : oz::a_stage_offset(I)) * ((int64_t)a_planes * ATILE);
-          for (int kc = 0; kc < nk; ++kc) {
+          for (int kc = k0; kc < k1; ++kc) {
             mbar_wait(&empty[st], ph ^ 1);
             unsigned char* dst = smem + (size_t)st * STAGE;
             mbar_expect_tx(&full[st], STAGE);
@@ -192,17 +292,15 @@ digit_gemm_kernel(const int8_t* __restrict__ AS, const int8_t* __restrict__ BS, 
   uint32_t ph = 0;
   for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
     const int g = item % G, tc = item / G, tile = tc / NCH, c = tc % NCH;
-    for (int i = 0;; ++i) {
-      const int I = serpentine_rowblock(i, g, G);
-      if (I >= NB) break;
-      const int nk = full_rows ? nst : min(2 * (I + 1), nst);
+    int I, k0, k1;
+    for (int i = 0; item_range<EPI>(g, i, G, NB, nst, full_rows, kper, I, k0, k1); ++i) {
 #pragma unroll
       for (int l = 0; l < S; ++l)
 #pragma unroll
         for (int j = 0; j < NR; ++j) acc[l][j] = 0u;
       fence_acc(acc);
       int held = -1;  // the previous stage: its last MMA group may still be running
-      for (int kc = 0; kc < nk; ++kc) {
+      for (int kc = k0; kc < k1; ++kc) {
         mbar_wait(&full[st], ph);
         const uint32_t base = smem_u32(smem + (size_t)st * STAGE);
         const uint64_t b0 = smem_desc(base + (uint32_t)(S * ATILE));
@@ -232,57 +330,45 @@ digit_gemm_kernel(const int8_t* __restrict__ AS, const int8_t* __restrict__ BS, 
       fence_acc(acc);
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[held]);
-      // epilogue of the row-block.  Fragment of m64nN: register 4j + e holds row 16 wq + lane/4 (+8 for e >= 2) of the
-      // warpgroup's 64, column 8j + 2 (lane % 4) + (e & 1) of the chunk
-      const int64_t r0 = (int64_t)I * 128 + wg * 64 + wq * 16 + (lane >> 2), r1 = r0 + 8;
-      const double rs0 = rowscale[r0] * out_scale * 0x1p-16, rs1 = rowscale[r1] * out_scale * 0x1p-16;
-      const double rc0 = rowsum ? rowsum[r0] * half_var : 0.0, rc1 = rowsum ? rowsum[r1] * half_var : 0.0;
+      if constexpr (EPI == EPI_SPLIT) {
+        int* dst = acc_out + ((int64_t)tc * NB + I) * (S * NR * CONSUMER_WARPS * 32) + threadIdx.x;
 #pragma unroll
-      for (int j = 0; j < CN / 8; ++j) {
-        double a[4];
+        for (int l = 0; l < S; ++l)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          // Horner over the levels, least significant first: v = ((T_{S+1} 2^-8 + T_S) 2^-8 + ...) + T_2
-          double v = int_to_double(acc[S - 1][4 * j + e]);
-#pragma unroll
-          for (int l = S - 2; l >= 0; --l) v = fma(v, 0x1p-8, int_to_double(acc[l][4 * j + e]));
-          a[e] = e < 2 ? fma(v, rs0, rc0) : fma(v, rs1, rc1);
-        }
-        const int col = 8 * j + 2 * (lane & 3);
-        if (EPI == EPI_STORE) {
-          double* dst = Aplain + ((int64_t)tile * NTB + (int64_t)c * CN + col) * lda;
-          dst[r0] = a[0];
-          dst[lda + r0] = a[1];
-          dst[r1] = a[2];
-          dst[lda + r1] = a[3];
-        } else {
-          double s0 = fma(a[0], a[0], a[2] * a[2]), s1 = fma(a[1], a[1], a[3] * a[3]);
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-          }
-          if (lane < 4) {  // the warp's 16 rows, accumulated over the item's row-blocks in a fixed order
-            colbuf[warp][col] += s0;
-            colbuf[warp][col + 1] += s1;
-          }
-        }
+          for (int j = 0; j < NR; ++j) atomicAdd(dst + (l * NR + j) * (CONSUMER_WARPS * 32), (int)acc[l][j]);
+      } else {
+        rowblock_epilogue<S, EPI, NTB>(acc, I, tile, c, warp, lane, rowscale, rowsum, out_scale, half_var, colbuf, Aplain, lda);
       }
     }
-    if (EPI == EPI_SUMSQ) {
-      asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_WARPS * 32) : "memory");
-      if (threadIdx.x < CN) {
-        double s = 0.0;
-#pragma unroll
-        for (int w = 0; w < CONSUMER_WARPS; ++w) {
-          s += colbuf[w][threadIdx.x];
-          colbuf[w][threadIdx.x] = 0.0;
-        }
-        partial[(int64_t)g * McPad + (int64_t)tile * NTB + (int64_t)c * CN + threadIdx.x] = s;
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_WARPS * 32) : "memory");
-    }
+    if constexpr (EPI == EPI_SUMSQ) colbuf_flush<CN>(colbuf, partial + (int64_t)g * McPad + (int64_t)tile * NTB + (int64_t)c * CN);
   }
+}
+
+// The EPI_SUMSQ epilogue of a split-K GEMM (EPI_SPLIT) of `tiles` candidate tiles over G row-block groups: CTA (tile, chunk, g)
+// loads the summed accumulators of group g's row-blocks in serpentine order into the same fragment layout, per consumer
+// thread, and runs the same epilogue, so partial[g][t] is byte for byte what digit_gemm_kernel<S, EPI_SUMSQ> writes.
+template <int S, int NTB>
+__global__ void __launch_bounds__(CONSUMER_WARPS * 32, 1)
+split_epilogue_kernel(const int* __restrict__ acc_in, const double* __restrict__ rowscale, const double* __restrict__ rowsum, int NB,
+                      int G, int64_t McPad, double out_scale, double half_var, double* __restrict__ partial) {
+  constexpr int CN = chunk_cols<S>(), NCH = NTB / CN, NR = CN / 2;
+  __shared__ double colbuf[CONSUMER_WARPS][CN];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = blockIdx.x % G, tc = blockIdx.x / G, tile = tc / NCH, c = tc % NCH;
+  for (int i = threadIdx.x; i < CONSUMER_WARPS * CN; i += blockDim.x) colbuf[i / CN][i % CN] = 0.0;
+  __syncthreads();
+  for (int i = 0;; ++i) {
+    const int I = serpentine_rowblock(i, g, G);
+    if (I >= NB) break;
+    const int* src = acc_in + ((int64_t)tc * NB + I) * (S * NR * CONSUMER_WARPS * 32) + threadIdx.x;
+    uint32_t acc[S][NR];
+#pragma unroll
+    for (int l = 0; l < S; ++l)
+#pragma unroll
+      for (int j = 0; j < NR; ++j) acc[l][j] = (uint32_t)src[(l * NR + j) * (CONSUMER_WARPS * 32)];
+    rowblock_epilogue<S, EPI_SUMSQ, NTB>(acc, I, tile, c, warp, lane, rowscale, rowsum, out_scale, half_var, colbuf, nullptr, 0);
+  }
+  colbuf_flush<CN>(colbuf, partial + (int64_t)g * McPad + (int64_t)tile * NTB + (int64_t)c * CN);
 }
 
 // ---- host side ----
@@ -303,14 +389,47 @@ inline int set_smem() {
 template <int S, int EPI, int NTB>
 inline int launch(cudaStream_t st, const int8_t* AS, const int8_t* BS, const double* rowscale, const double* rowsum, int NB, int nst,
                   int G, int tiles, int64_t McPad, double out_scale, double half_var, int a_planes, int b_planes, int full_rows,
-                  double* partial, double* Aplain, int64_t lda) {
+                  double* partial, double* Aplain, int64_t lda, int kper = 0, int* acc = nullptr) {
   int sms = 0;
   TB_TRY(sm_count(&sms));
   const int64_t items = (int64_t)tiles * (NTB / chunk_cols<S>()) * G;
   const int grid = (int)std::min<int64_t>(sms, items);
   if (grid <= 0) return 0;
   digit_gemm_kernel<S, EPI, NTB><<<grid, THREADS, smem_bytes<S>(), st>>>(AS, BS, rowscale, rowsum, NB, nst, G, tiles, McPad, out_scale,
-                                                                         half_var, a_planes, b_planes, full_rows, partial, Aplain, lda);
+                                                                         half_var, a_planes, b_planes, full_rows, partial, Aplain, lda,
+                                                                         kper, acc);
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Split-K for an EPI_SUMSQ GEMM whose tiles * NCH * G work items fill less than one wave of SMs: the stages per unit, the
+// fewest (at least 8: each unit adds S * 128 * CN int32 to the scratch) that keep the units within one wave, at most a whole
+// row-block.  0: no split.
+inline int split_kper(int S, int NTB, int tiles, int G, int NB, int nst, int full_rows) {
+  const int nch = NTB / chunk_cols_of(S);
+  if ((int64_t)tiles * nch * G >= NUM_SMS) return 0;
+  int64_t stages = 0;
+  for (int I = 0; I < NB; ++I) stages += rowblock_stages(I, nst, full_rows);
+  stages *= (int64_t)tiles * nch;
+  int kper = (int)std::min<int64_t>(nst, std::max<int64_t>(8, (stages + NUM_SMS - 1) / NUM_SMS));
+  while (kper < nst && (int64_t)tiles * nch * split_units(NB, nst, full_rows, kper) > NUM_SMS) ++kper;
+  return kper;
+}
+template <int S> inline size_t split_acc_bytes(int tiles, int NTB, int NB) {
+  return (size_t)tiles * (NTB / chunk_cols<S>()) * NB * S * (chunk_cols<S>() / 2) * (CONSUMER_WARPS * 32) * sizeof(int);
+}
+
+// EPI_SUMSQ through the split: zero the accumulator scratch acc (split_acc_bytes), the units, then the epilogue over G groups
+template <int S, int NTB>
+inline int launch_split(cudaStream_t st, const int8_t* AS, const int8_t* BS, const double* rowscale, const double* rowsum, int NB,
+                        int nst, int G, int tiles, int64_t McPad, double out_scale, double half_var, int a_planes, int b_planes,
+                        int full_rows, int kper, int* acc, double* partial) {
+  TB_CUDA(cudaMemsetAsync(acc, 0, split_acc_bytes<S>(tiles, NTB, NB), st));
+  TB_TRY((launch<S, EPI_SPLIT, NTB>(st, AS, BS, rowscale, rowsum, NB, nst, split_units(NB, nst, full_rows, kper), tiles, McPad,
+                                    out_scale, half_var, a_planes, b_planes, full_rows, nullptr, nullptr, 0, kper, acc)));
+  split_epilogue_kernel<S, NTB><<<tiles * (NTB / chunk_cols<S>()) * G, CONSUMER_WARPS * 32, 0, st>>>(acc, rowscale, rowsum, NB, G, McPad,
+                                                                                                   out_scale, half_var, partial);
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
   return 0;

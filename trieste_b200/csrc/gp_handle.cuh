@@ -222,6 +222,9 @@ struct tb_gp {
   // screened argmax (tb_api.cu, argmax_screened): the screen bound ub of all M candidates, the survivors' coordinates / global
   // indices, and the bound pass's per-block winners + probe pair + survivor counts
   tb::DevBuf sScrUb, sScrX, sScrIdx, sScrBlk;
+  // its rounds of few candidate tiles: the kernel values of the wide K* generation [nst*64][tiles NT], the int32 level
+  // accumulators of the split-K variance GEMM
+  tb::DevBuf sKval, sSplitAcc;
   // mirrors of the posterior for the bound pass (prescreen.cuh), rebuilt when cache_gen moves: pre_tc (tensor-core pass): its
   // stages of fp16 B fragments and |σ_f² α| (pre_nsl n8 slices, the first pre_npos_sl with α > 0); otherwise (CUDA-core pass)
   // fp32 rows [nst*64][W] of (x', |x'|^2, σ_f² α, |σ_f² α|); the centre [DP] subtracted from scaled inputs, and the constants

@@ -16,6 +16,10 @@ int int8_init() {  // each digit GEMM instantiation once
   TB_TRY((dg::set_smem<4, dg::EPI_SUMSQ, oz::Geo<4>::NT>()));
   TB_TRY((dg::set_smem<4, dg::EPI_STORE, oz::Geo<4>::NT>()));
   TB_TRY((dg::set_smem<3, dg::EPI_SUMSQ, oz::Geo<3>::NT>()));
+  TB_TRY((dg::set_smem<6, dg::EPI_SPLIT, oz::Geo<6>::NT>()));
+  TB_TRY((dg::set_smem<5, dg::EPI_SPLIT, oz::Geo<5>::NT>()));
+  TB_TRY((dg::set_smem<4, dg::EPI_SPLIT, oz::Geo<4>::NT>()));
+  TB_TRY((dg::set_smem<3, dg::EPI_SPLIT, oz::Geo<3>::NT>()));
   return 0;
 }
 
@@ -236,7 +240,8 @@ static int kstar_21(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, int8
 }
 
 template <int S>
-static int kstar_single_pass(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean, const KSplit* split) {
+static int kstar_single_pass(tb_gp* gp, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean, const KSplit* split,
+                             bool wide) {
   const double* Xs = gp->dXs.as<double>();
   const double* al = gp->dAlpha.as<double>();
   const double* il = gp->dInvLs.as<double>();
@@ -251,6 +256,23 @@ static int kstar_single_pass(tb_gp* gp, const double* Xc_dev, int64_t mc, int ti
   const KSplit ks = split ? *split : int8_kstar_split(gp, true, tiles);
   const int ksplit = ks.ksplit, kc_per = ks.kc_per;
   const int64_t mstride = (int64_t)tiles * oz::Geo<S>::NT;
+  if (wide) {
+    // the k-stages over ~4 CTAs per SM, the kernel values to gp->sKval, then the means of split ks replayed from them
+    const int wsplit = (int)std::min<int64_t>(nst, (4 * NUM_SMS + ctas - 1) / ctas);
+    const int wkc = (nst + wsplit - 1) / wsplit;
+    TB_TRY(gp->sKval.reserve(sizeof(double) * (size_t)nst * oz::KST * mstride));
+    double* kval = gp->sKval.as<double>();
+    with_kind_dp(gp->kernel, gp->DP, [&](auto K, auto P) {
+      oz5::kstar_digits_kernel<decltype(K)::value, decltype(P)::value, S, true><<<dim3(ctas, (nst + wkc - 1) / wkc), TH, 0, st>>>(
+          Xs, X2, al, Xc_dev, il, N, nst, D, mc, var, inv_b, dig_c, mc0, fm::Consts(), tiles, wkc, BS, kval);
+    });
+    TB_LAUNCHED();
+    oz5::mean_replay_kernel<<<(unsigned)(mstride * 4 / oz5::REPLAY_THREADS), oz5::REPLAY_THREADS, 0, st>>>(kval, al, nst, ksplit, kc_per,
+                                                                                                        mstride, mc0, mean);
+    TB_LAUNCHED();
+    TB_CUDA(cudaGetLastError());
+    return 0;
+  }
   double* mean_dst = mean;
   if (ksplit > 1) {
     TB_TRY(gp->sMeanPart.reserve(sizeof(double) * (size_t)ksplit * mstride));
@@ -270,10 +292,18 @@ static int kstar_single_pass(tb_gp* gp, const double* Xc_dev, int64_t mc, int ti
 }
 
 int int8_kstar(tb_gp* gp, bool single_pass, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean,
-               const KSplit* split) {
+               const KSplit* split, bool wide) {
   if (!single_pass) return kstar_21(gp, Xc_dev, mc, tiles, BS, mean);
-  return gp->digits.linv.planes == 5 ? kstar_single_pass<5>(gp, Xc_dev, mc, tiles, BS, mean, split)
-                                     : kstar_single_pass<4>(gp, Xc_dev, mc, tiles, BS, mean, split);
+  return gp->digits.linv.planes == 5 ? kstar_single_pass<5>(gp, Xc_dev, mc, tiles, BS, mean, split, wide)
+                                     : kstar_single_pass<4>(gp, Xc_dev, mc, tiles, BS, mean, split, wide);
+}
+
+// digits the variance GEMM computes with: the single-pass engine's admitted mode; the 21-product split's 6, or its 4 leading
+// planes on fp32 handles (10 products, error ~1e-7 σ_f² << the fp32 tolerance)
+static int variance_digits(const tb_gp* gp, bool single_pass) { return single_pass ? gp->digits.mode : gp->dtype == TB_F32 ? 4 : 6; }
+
+int int8_split_kper(const tb_gp* gp, bool single_pass, int tiles, int G) {
+  return dg::split_kper(variance_digits(gp, single_pass), int8_tile_width(gp, single_pass), tiles, G, gp->NB, nst_of(gp), 0);
 }
 
 // ---- digit GEMM --------------------------------------------------------------------------------------------------------
@@ -281,14 +311,22 @@ int int8_kstar(tb_gp* gp, bool single_pass, const double* Xc_dev, int64_t mc, in
 // The digit GEMM of both engines: `left` (Linv, full_rows = 0, or K^-1, full_rows = 1) times the K* digits BS, computing with
 // the S leading planes of both on K* tiles of Geo<S>::NT candidates.  out_scale: the K* scale; h: the K* centre, added through
 // left's row sums (the single-pass split; none on the 21-product one).
+// kper > 0 (EPI_SUMSQ): split-K in units of kper stages (dg::launch_split), the accumulators in gp->sSplitAcc.
 template <int EPI>
 static int digit_gemm(tb_gp* gp, const DigitOperand& left, int full_rows, int S, double out_scale, double h, const int8_t* BS,
-                      int tiles, int G, int64_t McPad, double* partial, double* out, int64_t lda) {
+                      int tiles, int G, int64_t McPad, double* partial, double* out, int64_t lda, int kper = 0) {
   auto launch = [&](auto SV) {
-    constexpr int s = decltype(SV)::value;
-    return dg::launch<s, EPI, oz::Geo<s>::NT>(gp->stream, left.digits.as<int8_t>(), BS, left.scale.as<double>(), left.sum.as<double>(),
-                                              gp->NB, nst_of(gp), G, tiles, McPad, out_scale, h, left.planes, left.planes, full_rows,
-                                              partial, out, lda);
+    constexpr int s = decltype(SV)::value, NT = oz::Geo<s>::NT;
+    if constexpr (EPI == dg::EPI_SUMSQ) {
+      if (kper > 0) {
+        TB_TRY(gp->sSplitAcc.reserve(dg::split_acc_bytes<s>(tiles, NT, gp->NB)));
+        return dg::launch_split<s, NT>(gp->stream, left.digits.as<int8_t>(), BS, left.scale.as<double>(), left.sum.as<double>(), gp->NB,
+                                       nst_of(gp), G, tiles, McPad, out_scale, h, left.planes, left.planes, full_rows, kper,
+                                       gp->sSplitAcc.as<int>(), partial);
+      }
+    }
+    return dg::launch<s, EPI, NT>(gp->stream, left.digits.as<int8_t>(), BS, left.scale.as<double>(), left.sum.as<double>(), gp->NB,
+                                  nst_of(gp), G, tiles, McPad, out_scale, h, left.planes, left.planes, full_rows, partial, out, lda);
   };
   switch (S) {
     case 6: return launch(std::integral_constant<int, 6>{});
@@ -299,15 +337,15 @@ static int digit_gemm(tb_gp* gp, const DigitOperand& left, int full_rows, int S,
   return fail("digit GEMM: no store kernel computes with " + std::to_string(S) + " digits", ERR_RUNTIME);
 }
 
-int int8_variance(tb_gp* gp, bool single_pass, const int8_t* BS, int tiles, int G, int64_t McPad, double* partial) {
+int int8_variance(tb_gp* gp, bool single_pass, const int8_t* BS, int tiles, int G, int64_t McPad, double* partial, int kper) {
   const DigitState& d = gp->digits;
   const double var = gp->variance;
+  const int S = variance_digits(gp, single_pass);
   if (single_pass)
-    return digit_gemm<dg::EPI_SUMSQ>(gp, d.linv, 0, d.mode, 0.5 * var / oz::FILL, h_eff(var, d.linv.planes), BS, tiles, G, McPad,
-                                     partial, nullptr, 0);
-  // fp32 handles: the 4 leading planes (10 products), error ~1e-7 σ_f² << the fp32 tolerance
-  return digit_gemm<dg::EPI_SUMSQ>(gp, d.linv21, 0, gp->dtype == TB_F32 ? 4 : 6, std::ldexp(1.0, bscale_exp(var)), 0.0, BS, tiles, G,
-                                   McPad, partial, nullptr, 0);
+    return digit_gemm<dg::EPI_SUMSQ>(gp, d.linv, 0, S, 0.5 * var / oz::FILL, h_eff(var, d.linv.planes), BS, tiles, G, McPad, partial,
+                                     nullptr, 0, kper);
+  return digit_gemm<dg::EPI_SUMSQ>(gp, d.linv21, 0, S, std::ldexp(1.0, bscale_exp(var)), 0.0, BS, tiles, G, McPad, partial, nullptr, 0,
+                                   kper);
 }
 
 int int8_store(tb_gp* gp, bool single_pass, bool kinv, const int8_t* BS, int tiles, int G, int64_t McPad, double* out, int64_t lda) {

@@ -20,11 +20,15 @@ struct KSplit {
 };
 KSplit int8_kstar_split(const tb_gp* gp, bool single_pass, int tiles);  // the split a launch over `tiles` candidate tiles uses
 // K* digit tiles of mc device candidates into BS, their posterior means into mean.  split == nullptr: int8_kstar_split(gp,
-// single_pass, tiles); otherwise that split (the screened argmax reproduces a chunk's means)
+// single_pass, tiles); otherwise that split (the screened argmax reproduces a chunk's means).  wide (single-pass engine): the
+// k-stages spread over many more CTAs than `split` has, the same digits and means.
 int int8_kstar(tb_gp* gp, bool single_pass, const double* Xc_dev, int64_t mc, int tiles, int8_t* BS, double* mean,
-               const KSplit* split = nullptr);
-// variance path: partial[g][t] = sum over the rows of group g of A[n,t]^2, A = Linv K*
-int int8_variance(tb_gp* gp, bool single_pass, const int8_t* BS, int tiles, int G, int64_t McPad, double* partial);
+               const KSplit* split = nullptr, bool wide = false);
+// variance path: partial[g][t] = sum over the rows of group g of A[n,t]^2, A = Linv K*.  kper > 0: split-K in units of kper
+// stages (int8_split_kper), the same partial.
+int int8_variance(tb_gp* gp, bool single_pass, const int8_t* BS, int tiles, int G, int64_t McPad, double* partial, int kper = 0);
+// The split-K stages per unit for a variance GEMM over `tiles` tiles and G row-block groups, 0 when its groups fill a wave
+int int8_split_kper(const tb_gp* gp, bool single_pass, int tiles, int G);
 // store path: out[t][lda] = (left K*)[., t], kinv = false: Linv (A of the joint paths), true: dense K^-1 (V of the gradient path)
 int int8_store(tb_gp* gp, bool single_pass, bool kinv, const int8_t* BS, int tiles, int G, int64_t McPad, double* out, int64_t lda);
 // after int8_select: digit products of the variance GEMM, and the single-pass engine's a-priori error estimate (0 when it

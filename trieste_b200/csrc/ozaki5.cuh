@@ -43,10 +43,13 @@ __global__ void row_norms_kernel(const double* __restrict__ Xs, int64_t rows_hav
 //   inv_bscale_2p = 2^(8S) / sB,  sB = h / FILL,  h = variance / 2
 // A candidate's mean depends on (ksplit = gridDim.y, kc_per) only: the screened argmax (tb_api.cu) reproduces the mean of a
 // candidate of an unscreened chunk by launching with that chunk's split.
+// KVAL (the screened argmax's gathered tiles): no mean; every kernel value goes to mean_out as kval[ntiles NT][nst 64] instead, so
+// that the k-stages can be split far finer than the mean's chain allows, and mean_replay_kernel rebuilds the chain of any split.
 // ------------------------------------------------------------------------------------------------
 constexpr int KGEN_WARPS = 8;
-template <int KIND, int DP, int S>
-__global__ void __launch_bounds__(KGEN_WARPS * 32, DP <= 12 ? 4 : 3)  // 64 registers / 32 warps per SM (80 / 24 for D > 12: no spills)
+// (KVAL launches are a few CTAs per SM at most: 128 registers, 255 for D > 12; no spills)
+template <int KIND, int DP, int S, bool KVAL = false>
+__global__ void __launch_bounds__(KGEN_WARPS * 32, KVAL ? (DP <= 12 ? 2 : 1) : DP <= 12 ? 4 : 3)  // 64 registers / 32 warps per SM (80 / 24 for D > 12: no spills)
 kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2, const double* __restrict__ alpha,
                     const double* __restrict__ Xc, const double* __restrict__ inv_ls, int N, int nst, int D, int64_t M, double variance,
                     double inv_bscale_2p, double dig_c, double mean_const, const __grid_constant__ fm::Consts fc, int ntiles,
@@ -111,7 +114,7 @@ kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2
   //   fma(k, inv, dig_c),  dig_c = 1.5 2^52 + 0x80..80 - c,  c = the INTEGER nearest to h inv (host: the centre actually
   //   subtracted is h_eff = c / inv, and the epilogue's row constant uses the same h_eff, so no bias is introduced);
   // the int8 digits are the low S bytes XOR 0x80 (digit_bytes, folded)
-  double macc = 0.0;
+  double macc = 0.0, kprev = 0.0;
   for (int kc = kc0; kc < kc1; ++kc) {
     const int buf = (kc - kc0) & 1;
     if (kc + 1 < kc1) {
@@ -149,7 +152,16 @@ kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2
         }
       }
       const double kval = kernel_from_r2_fast<KIND>(r2, variance, exp_tab, fc);
-      macc = fma(kval, al_s[buf][kv], macc);
+      if constexpr (KVAL) {  // kval[t][k]: the lane's 16 values of a stage are 128 contiguous bytes
+        if (!(j & 1)) {
+          kprev = kval;
+        } else if (tile_id < ntiles) {
+          *reinterpret_cast<double2*>(mean_out + (tile_id * NT + t_local) * (int64_t)nst * KST + (int64_t)kc * KST + kl - 1) =
+              make_double2(kprev, kval);
+        }
+      } else {
+        macc = fma(kval, al_s[buf][kv], macc);
+      }
       const double tb = fma(kval, inv_bscale_2p, dig_c);
       const uint32_t wl = (uint32_t)__double2loint(tb) ^ 0x80808080u, wh = (uint32_t)__double2hiint(tb) ^ 0x80u;
       oz::scatter_rt<S>(pk, j, wl, wh);
@@ -161,10 +173,12 @@ kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2
     }
     __syncthreads();
   }
-  macc += __shfl_xor_sync(0xffffffffu, macc, 8);
-  macc += __shfl_xor_sync(0xffffffffu, macc, 16);
-  if (ch == 0 && tile_id < ntiles)
-    mean_out[(int64_t)blockIdx.y * ntiles * NT + tile_id * NT + t_local] = gridDim.y == 1 ? macc + mean_const : macc;
+  if constexpr (!KVAL) {
+    macc += __shfl_xor_sync(0xffffffffu, macc, 8);
+    macc += __shfl_xor_sync(0xffffffffu, macc, 16);
+    if (ch == 0 && tile_id < ntiles)
+      mean_out[(int64_t)blockIdx.y * ntiles * NT + tile_id * NT + t_local] = gridDim.y == 1 ? macc + mean_const : macc;
+  }
 }
 
 // mean[t] = mean_const + Σ_s part[s][t] (fixed order: results do not depend on the scheduling of the k-split CTAs)
@@ -175,6 +189,50 @@ __global__ void mean_reduce_kernel(const double* __restrict__ part, int ksplit, 
   double s = 0.0;
   for (int i = 0; i < ksplit; ++i) s += part[(int64_t)i * stride + t];
   mean_out[t] = s + mean_const;
+}
+
+// The means of kstar_digits_kernel<.., KVAL = false> launched with split (ksplit, kc_per), bit for bit, from the kernel
+// values kval[stride][nst 64] of its KVAL launch: per candidate and 16-wide k chunk ch the same fma chain over the stages of
+// each split and the same lanes (candidate lane % 8, chunk lane / 8), the same xor-8 / xor-16 shuffle combine, and for
+// ksplit > 1 the same fixed-order sum as mean_reduce_kernel.  stride = tiles NT; threads = 4 stride, in whole warps.  The
+// chain is latency-bound: small CTAs spread it over many SMs, and each lane loads a stage's values while it sums the last.
+constexpr int REPLAY_THREADS = 64;
+__global__ void __launch_bounds__(REPLAY_THREADS)
+mean_replay_kernel(const double* __restrict__ kval, const double* __restrict__ alpha, int nst, int ksplit, int kc_per, int64_t stride,
+                   double mean_const, double* __restrict__ mean_out) {
+  const int lane = threadIdx.x & 31, cl = lane & 7, ch = lane >> 3;
+  const int64_t t = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 8 + cl;
+  if (t - cl >= stride) return;  // whole warps leave together
+  const double* kt = kval + t * (int64_t)nst * KST + ch * 16;
+  double s = 0.0, macc = 0.0;
+  const double* at = alpha + ch * 16;
+  double2 kv[8], av[8];
+  auto load = [&](int kc) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      kv[j] = *reinterpret_cast<const double2*>(kt + kc * KST + 2 * j);
+      av[j] = *reinterpret_cast<const double2*>(at + kc * KST + 2 * j);
+    }
+  };
+  load(0);
+  for (int sp = 0; sp < ksplit; ++sp) {
+    const int kc0 = sp * kc_per, kc1 = min(nst, kc0 + kc_per);
+    macc = 0.0;
+    for (int kc = kc0; kc < kc1; ++kc) {
+      const double2 k2[8] = {kv[0], kv[1], kv[2], kv[3], kv[4], kv[5], kv[6], kv[7]};
+      const double2 a2[8] = {av[0], av[1], av[2], av[3], av[4], av[5], av[6], av[7]};
+      if (kc + 1 < nst) load(kc + 1);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        macc = fma(k2[j].x, a2[j].x, macc);
+        macc = fma(k2[j].y, a2[j].y, macc);
+      }
+    }
+    macc += __shfl_xor_sync(0xffffffffu, macc, 8);
+    macc += __shfl_xor_sync(0xffffffffu, macc, 16);
+    s += macc;
+  }
+  if (ch == 0) mean_out[t] = ksplit == 1 ? macc + mean_const : s + mean_const;
 }
 
 }  // namespace oz5

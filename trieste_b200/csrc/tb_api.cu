@@ -1210,19 +1210,19 @@ static int eng_groups(const tb_gp* gp, Engine e, int tiles) {
 }
 
 // K* of mc device candidates into gp->sKs (fp64 panels or digit tiles), their posterior means into gp->sMean.
-// split: the int8 engines' k-split (nullptr: the one int8_kstar_split gives for this many tiles)
-static int eng_kstar(tb_gp* gp, Engine e, const double* xc, int64_t mc, int tiles, const KSplit* split = nullptr) {
+// split: the int8 engines' k-split (nullptr: the one int8_kstar_split gives for this many tiles); wide: int8_kstar's
+static int eng_kstar(tb_gp* gp, Engine e, const double* xc, int64_t mc, int tiles, const KSplit* split = nullptr, bool wide = false) {
   double* mean = gp->sMean.as<double>();
   if (e == Engine::F64) return launch_kstar(gp, xc, mc, tiles, gp->sKs.as<double>(), mean);
-  return int8_kstar(gp, e == Engine::OZ15, xc, mc, tiles, gp->sKs.as<int8_t>(), mean, split);
+  return int8_kstar(gp, e == Engine::OZ15, xc, mc, tiles, gp->sKs.as<int8_t>(), mean, split, wide);
 }
 
 // Variance GEMM: sums of squares of A = Linv K* over G row-block groups into gp->sPartial.  fp64 engine with packed_a: A
-// also goes to gp->sA as packed panels, the operand of its V GEMM.
-static int eng_variance(tb_gp* gp, Engine e, int tiles, int G, int64_t McPad, bool packed_a) {
+// also goes to gp->sA as packed panels, the operand of its V GEMM.  kper > 0 (int8 engines): split-K (int8_split_kper).
+static int eng_variance(tb_gp* gp, Engine e, int tiles, int G, int64_t McPad, bool packed_a, int kper = 0) {
   cudaStream_t st = gp->stream;
   double* partial = gp->sPartial.as<double>();
-  if (e != Engine::F64) return int8_variance(gp, e == Engine::OZ15, gp->sKs.as<int8_t>(), tiles, G, McPad, partial);
+  if (e != Engine::F64) return int8_variance(gp, e == Engine::OZ15, gp->sKs.as<int8_t>(), tiles, G, McPad, partial, kper);
   if (packed_a)
     trigemm_kernel<false, EPI_SUMSQ_PACKED><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
         gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, gp->sA.as<double>(), nullptr, 0);
@@ -1326,7 +1326,9 @@ struct EvalOut {
 
 // One chunk of n device candidates at xc: K* and the means, the variance GEMM over G row-block groups, the gradient when
 // o.grad is set, the acquisition tail and the argmax fold.  c0: global index of the first candidate.  The screened argmax's
-// gathered candidates pass their global indices in idx_map instead, and the k-split of the chunk they come from.
+// gathered candidates pass their global indices in idx_map instead, and the k-split of the chunk they come from; when they
+// are too few tiles for the row-block groups to fill the SMs, the int8 engines spread them wider (split-K variance GEMM, wide
+// K* generation) with the same results.
 static int eval_chunk(tb_gp* gp, const EvalRequest& rq, Engine e, const double* xc, int64_t n, int64_t c0, int G, const EvalOut& o,
                       const int64_t* idx_map = nullptr, const KSplit* split = nullptr) {
   cudaStream_t st = gp->stream;
@@ -1335,9 +1337,10 @@ static int eval_chunk(tb_gp* gp, const EvalRequest& rq, Engine e, const double* 
   const int64_t McPad = (int64_t)tiles * nt;
   const double* partial = gp->sPartial.as<double>();
   const double* mean = gp->sMean.as<double>();
-  TB_TRY(eng_kstar(gp, e, xc, n, tiles, split));
+  const int kper = idx_map && e != Engine::F64 ? int8_split_kper(gp, e == Engine::OZ15, tiles, G) : 0;
+  TB_TRY(eng_kstar(gp, e, xc, n, tiles, split, kper > 0));
   TB_TRY(profiled_gemm(gp, (double)McPad * (double)gp->N * (double)gp->N,
-                       [&] { return eng_variance(gp, e, tiles, G, McPad, o.grad != nullptr); }));
+                       [&] { return eng_variance(gp, e, tiles, G, McPad, o.grad != nullptr, kper); }));
   if (o.grad) {
     TB_TRY(launch_partials(gp, st, rq.acq, rq.param, partial, G, McPad, mean, xc, n));
     TB_TRY(eng_store_v(gp, e, tiles, McPad));
