@@ -32,6 +32,7 @@ extern "C" {
 
 typedef struct tb_gp tb_gp;   /* exact-GPR posterior: owns device copies of X, Linv, alpha, hyper-params */
 typedef struct tb_rff tb_rff; /* random-Fourier-feature trajectory: owns W, b, theta */
+typedef struct tb_ehvi tb_ehvi; /* expected hypervolume improvement over L borrowed tb_gp handles: owns the partition cells */
 
 enum tb_status {
   TB_OK = 0,
@@ -252,6 +253,26 @@ int tb_rff_maximize_boxes(tb_rff* r, const double* lower, const double* upper, i
 /* (K(X,X) + noise I)^-1 B = Linv^T (Linv B) through the cached triangular inverse: B, out [nrhs][N] (each right-hand side contiguous);
  * the v-weights of a decoupled trajectory (sampler.py:716, gpflux compute_A_inv_b).  fp64, host or device. */
 int tb_gp_kinv_apply(tb_gp* gp, const double* B, int nrhs, double* out);
+
+/* ---- expected hypervolume improvement over a stack of GPs ---------------------------------------
+ * expected_hv_improvement (acquisition/function/multi_objective.py:145-250) over L one-output models, one tb_gp per
+ * objective: EHVI(x) = sum_k prod_l g_kl(mean_l(x), var_l(x)) over the K cells of the non-dominated partition.
+ * tb_ehvi_create borrows the handles (they must outlive the object): 2 <= L <= 8, distinct handles with data, on one
+ * device, with one dtype and one input dimension D; TB_ERR_INVALID otherwise. */
+int tb_ehvi_create(tb_ehvi** out, tb_gp* const* models, int L);
+int tb_ehvi_destroy(tb_ehvi* h);
+/* the cells' bounds lower, upper [K, L] (fp64, host or device) as prepare_default_non_dominated_partition_bounds returns
+ * them, in the objectives' minimisation orientation; K >= 1. */
+int tb_ehvi_set_cells(tb_ehvi* h, const double* lower, const double* upper, int64_t K);
+/* Xc [M, D] -> out [M]; grad (nullable) [M, D].  The members' dtype, host or device pointers.  TB_ERR_INVALID if the cells
+ * are not set or a member's posterior cache is not built. */
+int tb_ehvi_eval(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad);
+/* tb_acq_argmax's contract for EHVI: first-max index and value over Xc [M, D]; out [M] nullable. */
+int tb_ehvi_argmax(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* best_value, int64_t* best_index);
+/* tb_acq_maximize's contract for EHVI: the device multi-start L-BFGS maximising EHVI inside the box [lower, upper] ([D]). */
+int tb_ehvi_maximize(tb_ehvi* h, const double* lower, const double* upper, const double* starts, int64_t P, int maxcor,
+                     int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
+                     int64_t* nfev);
 
 /* ---- instrumentation (bench / tests) ---------------------------------------------------------
  * kernels launched by this library in this process since the last reset; device time (ms) of the

@@ -5,7 +5,7 @@ Hand-written sm_90a CUDA behind a C-ABI (``include/trieste_b200.h``); no CPU fal
 from . import _lib  # noqa: F401
 from .data import Dataset  # noqa: F401
 from .kernels import RBF, Constant, Matern12, Matern32, Matern52, SquaredExponential  # noqa: F401
-from .models import GaussianProcessRegression, GPRSpec, build_gpr  # noqa: F401
+from .models import GaussianProcessRegression, GPRSpec, ModelStack, TrainableModelStack, build_gpr  # noqa: F401
 from .space import Box, DiscreteSearchSpace, TaggedMultiSearchSpace  # noqa: F401
 
 __version__ = "0.1.0"

@@ -38,6 +38,7 @@ from .greedy_batch import (  # noqa: F401
     local_penalizer,
     soft_local_penalizer,
 )
+from .multi_objective import ExpectedHypervolumeImprovement, expected_hv_improvement  # noqa: F401
 from .interface import (  # noqa: F401
     AcquisitionFunctionBuilder,
     GreedyAcquisitionFunctionBuilder,

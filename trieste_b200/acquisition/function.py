@@ -53,6 +53,16 @@ class _FusedSingleQuery(AcquisitionFunctionClass):
     def _before_call(self) -> None:
         """state that lives in the native handle and must be current before a launch (none by default)"""
 
+    # the native calls behind the shape handling below; a function over several handles overrides all three
+    def _native_eval(self, px, M, po, pg) -> int:
+        return _lib.lib().tb_acq_eval(self._model.handle, self._acq, self._param, px, M, po, pg)
+
+    def _native_argmax(self, px, M, best, idx) -> int:
+        return _lib.lib().tb_acq_argmax(self._model.handle, self._acq, self._param, px, M, None, best, idx)
+
+    def _native_maximize(self, lo, up, x0, P, *args) -> int:
+        return _lib.lib().tb_acq_maximize(self._model.handle, self._acq, self._param, lo, up, x0, P, *args)
+
     def _squeeze(self, x):
         self._before_call()
         x, _ = _lib.as_contiguous(x, self._model.dtype)
@@ -67,7 +77,7 @@ class _FusedSingleQuery(AcquisitionFunctionClass):
         flat, lead = self._squeeze(x)
         M = flat.shape[0]
         out, po = _lib.empty_like_kind(flat, (M, 1), self._model.dtype)
-        _lib.check(_lib.lib().tb_acq_eval(self._model.handle, self._acq, self._param, _ptr(flat), M, po, None))
+        _lib.check(self._native_eval(_ptr(flat), M, po, None))
         return out.reshape(lead + (1,))
 
     def value_and_gradient(self, x):
@@ -77,7 +87,7 @@ class _FusedSingleQuery(AcquisitionFunctionClass):
         M, D = flat.shape
         out, po = _lib.empty_like_kind(flat, (M, 1), self._model.dtype)
         grad, pg = _lib.empty_like_kind(flat, (M, D), self._model.dtype)
-        _lib.check(_lib.lib().tb_acq_eval(self._model.handle, self._acq, self._param, _ptr(flat), M, po, pg))
+        _lib.check(self._native_eval(_ptr(flat), M, po, pg))
         return out.reshape(lead + (1,)), grad.reshape(lead + (1, D))
 
     def maximize_from(self, starts, lower, upper, *, maxcor: int = 10, maxiter: int = 15000, maxls: int = 20,
@@ -99,10 +109,9 @@ class _FusedSingleQuery(AcquisitionFunctionClass):
         ok = np.zeros(P, dtype=np.int32)
         nfev = np.zeros(P, dtype=np.int64)
         _lib.check(
-            _lib.lib().tb_acq_maximize(
-                self._model.handle, self._acq, self._param, lo.ctypes.data, up.ctypes.data, x0.ctypes.data, P,
-                int(maxcor), int(maxiter), int(maxls), float(gtol), float(ftol),
-                x.ctypes.data, f.ctypes.data, ok.ctypes.data, nfev.ctypes.data,
+            self._native_maximize(
+                lo.ctypes.data, up.ctypes.data, x0.ctypes.data, P, int(maxcor), int(maxiter), int(maxls), float(gtol),
+                float(ftol), x.ctypes.data, f.ctypes.data, ok.ctypes.data, nfev.ctypes.data,
             )
         )
         return ok.astype(bool), f, x, nfev
@@ -117,11 +126,7 @@ class _FusedSingleQuery(AcquisitionFunctionClass):
         self._model._check_dim(pts)
         best = C.c_double() if self._model.dtype == np.float64 else C.c_float()
         idx = C.c_int64()
-        _lib.check(
-            _lib.lib().tb_acq_argmax(
-                self._model.handle, self._acq, self._param, _ptr(pts), pts.shape[0], None, C.byref(best), C.byref(idx)
-            )
-        )
+        _lib.check(self._native_argmax(_ptr(pts), pts.shape[0], C.byref(best), C.byref(idx)))
         return int(idx.value), float(best.value)
 
 

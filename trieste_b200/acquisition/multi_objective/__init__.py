@@ -1,0 +1,10 @@
+"""Multi-objective geometry on the host (Pareto dominance, fronts, hypervolume, non-dominated partitions) and the
+expected hypervolume improvement, whose per-candidate work runs on the device."""
+from .dominance import non_dominated  # noqa: F401
+from .function import ExpectedHypervolumeImprovement, expected_hv_improvement  # noqa: F401
+from .pareto import Pareto, get_reference_point  # noqa: F401
+from .partition import (  # noqa: F401
+    DividedAndConquerNonDominated,
+    ExactPartition2dNonDominated,
+    prepare_default_non_dominated_partition_bounds,
+)

@@ -659,9 +659,7 @@ acq_partials_kernel(const double* __restrict__ partial, int G, int64_t McPad, co
                     double* __restrict__ gib_coef = nullptr) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= Mc) return;
-  double ss = 0.0;
-  for (int g = 0; g < G; ++g) ss += partial[(int64_t)g * McPad + t];
-  const double raw = variance - ss;
+  const double raw = chunk_raw_variance(partial, G, McPad, t, variance);
   const bool clipped = raw < 1e-12;
   double dm, dv;
   if (acq == TB_ACQ_MES) {

@@ -523,6 +523,15 @@ __device__ __forceinline__ void block_best_store(double bv, int64_t bi, double* 
   }
 }
 
+// the posterior variance of candidate t before clipping: the prior variance less its sums of squares over the G row-block
+// groups of the variance GEMM, summed in group order.  Every tail of a chunk (values, partials, EHVI) reads it from here.
+__device__ __forceinline__ double chunk_raw_variance(const double* __restrict__ partial, int G, int64_t McPad, int64_t t,
+                                                     double variance) {
+  double ss = 0.0;
+  for (int g = 0; g < G; ++g) ss += partial[(int64_t)g * McPad + t];
+  return variance - ss;
+}
+
 // one thread per candidate of the chunk; block-level first-max argmax.  PEN: the value (and the gradient, when
 // pen.grad is set) is multiplied by the local penalty before the argmax.  The argmax index of candidate t is idx_map[t]
 // when idx_map is set (the compacted survivors of the screened argmax), else idx0 + t.
@@ -537,9 +546,7 @@ tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const doub
   int64_t bi = INT64_MAX;
   double vb = 0.0;  // PEN: the base value of this candidate
   if (t < Mc) {
-    double ss = 0.0;
-    for (int g = 0; g < G; ++g) ss += partial[(int64_t)g * McPad + t];
-    double var = fmax(variance - ss, 1e-12);
+    double var = fmax(chunk_raw_variance(partial, G, McPad, t, variance), 1e-12);
     double mu = mean[t];
     if (out_mean) out_mean[t] = mu;
     if (out_var) out_var[t] = var;

@@ -4,6 +4,7 @@
 #include "kernels_extra.cuh"
 #include "prescreen.cuh"
 #include "batch_ei.cuh"
+#include "ehvi.cuh"
 #include "int8_engines.h"
 #include <chrono>
 #include "factor.cuh"
@@ -2954,6 +2955,306 @@ int tb_mvn_cdf(int device, const double* x, const double* mean, const double* co
   TB_CHECK_CODE(herr == 0, "Cholesky decomposition was not successful. The input might not be valid "
                       "(cov + jitter*I of a row is not positive definite)", tb::ERR_NUMERIC);
   return 0;
+}
+
+}  // extern "C"
+
+// =================================================================================================
+// expected hypervolume improvement over a stack of L handles (ehvi.cuh)
+// =================================================================================================
+struct tb_ehvi {
+  std::vector<tb_gp*> m;  // borrowed member handles, one per objective
+  int L = 0, D = 0, device = 0, dtype = TB_F64;
+  int64_t K = 0;          // cells; 0: not set
+  tb::DevBuf dCells;      // lower [K][L] then upper [K][L]
+  tb::DevBuf sXc, sVals, sGrad, sGradL;  // staged candidates, values, gradient, and the members' gradients [L][mc][D]
+  std::vector<cudaEvent_t> ev;           // ev[l] orders member l's stream against the first member's (ev[0]: the other way)
+};
+
+namespace tb {
+
+struct EhviRequest {
+  const double* Xc = nullptr;  // host or device, [M, D]
+  int64_t M = 0;
+  double* out_vals = nullptr;  // host or device (nullable)
+  double* out_grad = nullptr;  // [M, D] (nullable)
+  bool want_argmax = false;
+  double best_value = 0.0;
+  int64_t best_index = -1;
+};
+
+template <int L>
+static void launch_ehvi_l(bool grad, const EhviMembers& mb, const double* cells, int64_t K, int64_t mc, int64_t c0, double* vals,
+                          double* bb, int64_t* bi, cudaStream_t st) {
+  const unsigned blocks = (unsigned)((mc + 255) / 256);
+  if (grad)
+    ehvi_kernel<L, true><<<blocks, 256, 0, st>>>(mb, cells, K, mc, c0, vals, bb, bi);
+  else
+    ehvi_kernel<L, false><<<blocks, 256, 0, st>>>(mb, cells, K, mc, c0, vals, bb, bi);
+}
+
+static int launch_ehvi(tb_ehvi* h, bool grad, const EhviMembers& mb, int64_t mc, int64_t c0, double* vals, bool argmax) {
+  tb_gp* g0 = h->m[0];
+  double* bb = argmax ? g0->sBlkBest.as<double>() : nullptr;
+  int64_t* bi = argmax ? g0->sBlkIdx.as<int64_t>() : nullptr;
+  const double* cells = h->dCells.as<double>();
+  switch (h->L) {
+    case 2: launch_ehvi_l<2>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 3: launch_ehvi_l<3>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 4: launch_ehvi_l<4>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 5: launch_ehvi_l<5>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 6: launch_ehvi_l<6>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 7: launch_ehvi_l<7>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    default: launch_ehvi_l<8>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+  }
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// what every EHVI evaluation needs of the object and its members, checked before anything is staged
+static int ehvi_check(const tb_ehvi* h, const char* who) {
+  TB_CHECK(h->K >= 1, std::string(who) + ": the partition cells are not set (tb_ehvi_set_cells)");
+  for (int l = 0; l < h->L; ++l) {
+    const tb_gp* gp = h->m[l];
+    TB_CHECK(gp->cache_valid, std::string(who) + ": posterior cache of member " + std::to_string(l) +
+                                  " is not built: call tb_gp_update_posterior_cache first");
+    TB_CHECK(gp->D == h->D, std::string(who) + ": member " + std::to_string(l) + " has input dimension " + std::to_string(gp->D) +
+                                ", the stack " + std::to_string(h->D));
+  }
+  return 0;
+}
+
+// The EHVI chunk loop.  The candidates are staged once, on the first member's stream st; each chunk runs every member's K*
+// and variance GEMM (and V for a gradient) on the member's own stream, then one EHVI kernel on st over all members' chunk
+// outputs, then the members' gradient assemblies and their fixed-order sum, then the argmax fold.  Events order the member
+// streams against st both ways; the host waits once, at the end.
+static int ehvi_run(tb_ehvi* h, EhviRequest& rq) {
+  TB_CUDA(cudaSetDevice(h->device));
+  const int L = h->L, D = h->D;
+  tb_gp* g0 = h->m[0];
+  cudaStream_t st = g0->stream;
+  const bool grad = rq.out_grad != nullptr;
+  if (rq.want_argmax) {
+    TB_TRY(g0->sRun.reserve(16));
+    TB_TRY(argmax_reset(g0));
+  }
+  if (rq.M == 0) return 0;
+  std::vector<Engine> eng(L);
+  std::vector<ChunkPlan> plan(L);
+  int64_t chunk_cap = rq.M;
+  for (int l = 0; l < L; ++l) {
+    TB_TRY(select_engine(h->m[l], grad, &eng[l]));
+    plan[l] = plan_chunks(h->m[l], eng[l], grad, rq.M);
+    chunk_cap = std::min(chunk_cap, plan[l].chunk_cap);
+  }
+  // Row-block groups as plan_chunks chooses them, for the common chunk: fixed for the call from its first chunk where the
+  // member's plan fixes them (int8 values), else per chunk.  A member whose own chunk size is the common one therefore sums
+  // each candidate's variance exactly as its tb_gp_predict does; the others agree with it to rounding.
+  std::vector<int> gfix(L, 0);
+  for (int l = 0; l < L; ++l) {
+    tb_gp* gp = h->m[l];
+    const int nt = eng_tile_width(gp, eng[l]);
+    const int64_t tiles_cap = (chunk_cap + nt - 1) / nt, pad_cap = tiles_cap * nt;
+    if (plan[l].G) gfix[l] = eng_groups(gp, eng[l], (int)tiles_cap);
+    TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, eng[l])));
+    TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)gp->NB * pad_cap));
+    TB_TRY(gp->sMean.reserve(sizeof(double) * pad_cap));
+    if (grad) {
+      if (eng[l] == Engine::F64) TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));
+      TB_TRY(gp->sV.reserve((size_t)pad_cap * gp->NB * BM * sizeof(double)));
+      TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * chunk_cap));
+    }
+  }
+  const Staged<const double> xin(rq.Xc, D, h->sXc, st);
+  const Staged<double> vals(rq.out_vals, 1, h->sVals, st), grads(rq.out_grad, D, h->sGrad, st);
+  TB_TRY(xin.reserve(chunk_cap));
+  TB_TRY(vals.reserve(chunk_cap));
+  if (grad) {
+    TB_TRY(grads.reserve(chunk_cap));
+    TB_TRY(h->sGradL.reserve(sizeof(double) * (size_t)L * chunk_cap * D));
+  }
+  if (rq.want_argmax) {
+    const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
+    TB_TRY(g0->sBlkBest.reserve(sizeof(double) * tail_blocks_cap));
+    TB_TRY(g0->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
+  }
+  // st -> members (ev[0]) and member l -> st (ev[l])
+  auto fan_out = [&]() -> int {
+    TB_CUDA(cudaEventRecord(h->ev[0], st));
+    for (int l = 1; l < L; ++l) TB_CUDA(cudaStreamWaitEvent(h->m[l]->stream, h->ev[0], 0));
+    return 0;
+  };
+  auto join = [&](int l) -> int {
+    if (l == 0) return 0;
+    TB_CUDA(cudaEventRecord(h->ev[l], h->m[l]->stream));
+    TB_CUDA(cudaStreamWaitEvent(st, h->ev[l], 0));
+    return 0;
+  };
+  for (int64_t c0 = 0; c0 < rq.M; c0 += chunk_cap) {
+    const int64_t mc = std::min<int64_t>(chunk_cap, rq.M - c0);
+    const double* xc;
+    TB_TRY(xin.in(c0, mc, &xc));
+    TB_TRY(fan_out());
+    EhviMembers mb{};
+    for (int l = 0; l < L; ++l) {
+      tb_gp* gp = h->m[l];
+      const Engine e = eng[l];
+      const int nt = eng_tile_width(gp, e);
+      const int tiles = (int)((mc + nt - 1) / nt);
+      const int64_t McPad = (int64_t)tiles * nt;
+      const int G = gfix[l] ? gfix[l] : eng_groups(gp, e, tiles);
+      TB_TRY(eng_kstar(gp, e, xc, mc, tiles));
+      TB_TRY(profiled_gemm(gp, (double)McPad * (double)gp->N * (double)gp->N,
+                           [&] { return eng_variance(gp, e, tiles, G, McPad, grad); }));
+      if (grad) TB_TRY(eng_store_v(gp, e, tiles, McPad));
+      TB_TRY(join(l));
+      mb.partial[l] = gp->sPartial.as<double>();
+      mb.mean[l] = gp->sMean.as<double>();
+      mb.dmv[l] = grad ? gp->sMisc.as<double>() : nullptr;
+      mb.McPad[l] = McPad;
+      mb.G[l] = G;
+      mb.variance[l] = gp->variance;
+    }
+    TB_TRY(launch_ehvi(h, grad, mb, mc, c0, vals.out(c0), rq.want_argmax));
+    if (grad) {
+      TB_TRY(fan_out());
+      double* gl = h->sGradL.as<double>();
+      for (int l = 0; l < L; ++l) {
+        TB_TRY(launch_grad(h->m[l], xc, mc, gl + (size_t)l * mc * D));
+        TB_TRY(join(l));
+      }
+      ehvi_grad_sum_kernel<<<(unsigned)((mc * D + 255) / 256), 256, 0, st>>>(gl, L, mc * D, grads.out(c0));
+      TB_LAUNCHED();
+      TB_CUDA(cudaGetLastError());
+    }
+    if (rq.want_argmax) TB_TRY(argmax_fold(g0, mc));
+    TB_TRY(grads.back(c0, mc));
+    TB_TRY(vals.back(c0, mc));
+  }
+  EvalRequest best;
+  if (rq.want_argmax) TB_TRY(argmax_read(g0, best));
+  TB_CUDA(cudaStreamSynchronize(st));
+  TB_CUDA(cudaGetLastError());
+  rq.best_value = best.best_value;
+  rq.best_index = best.best_index;
+  for (int l = 0; l < L; ++l) TB_TRY(profile_fold(h->m[l]));
+  return 0;
+}
+
+}  // namespace tb
+
+extern "C" {
+
+int tb_ehvi_create(tb_ehvi** out, tb_gp* const* models, int L) {
+  TB_CHECK(out && models, "tb_ehvi_create: null argument");
+  TB_CHECK(L >= 2 && L <= tb::EHVI_LMAX, "tb_ehvi_create: the number of objectives must be in [2, " +
+                                             std::to_string(tb::EHVI_LMAX) + "], got " + std::to_string(L));
+  for (int l = 0; l < L; ++l) {
+    TB_CHECK(models[l], "tb_ehvi_create: null model handle");
+    TB_CHECK(models[l]->have_data, "tb_ehvi_create: member " + std::to_string(l) + " has no data");
+    for (int j = 0; j < l; ++j) TB_CHECK(models[j] != models[l], "tb_ehvi_create: the same model handle appears twice");
+    TB_CHECK(models[l]->device == models[0]->device, "tb_ehvi_create: the members must be on one device");
+    TB_CHECK(models[l]->dtype == models[0]->dtype, "tb_ehvi_create: the members must have one dtype");
+    TB_CHECK(models[l]->D == models[0]->D, "tb_ehvi_create: the members must have one input dimension");
+  }
+  TB_CUDA(cudaSetDevice(models[0]->device));
+  tb_ehvi* h = new tb_ehvi();
+  h->m.assign(models, models + L);
+  h->L = L;
+  h->D = models[0]->D;
+  h->device = models[0]->device;
+  h->dtype = models[0]->dtype;
+  h->ev.assign(L, nullptr);
+  for (int l = 0; l < L; ++l) {
+    if (cudaEventCreateWithFlags(&h->ev[l], cudaEventDisableTiming) != cudaSuccess) {
+      cudaGetLastError();
+      tb_ehvi_destroy(h);
+      return tb::fail("tb_ehvi_create: cudaEventCreate failed", tb::ERR_RUNTIME);
+    }
+  }
+  *out = h;
+  return 0;
+}
+
+int tb_ehvi_destroy(tb_ehvi* h) {
+  if (!h) return 0;
+  cudaSetDevice(h->device);
+  for (cudaEvent_t e : h->ev)
+    if (e) cudaEventDestroy(e);
+  delete h;  // frees the device buffers; the member handles are borrowed
+  return 0;
+}
+
+int tb_ehvi_set_cells(tb_ehvi* h, const double* lower, const double* upper, int64_t K) {
+  TB_CHECK(h && lower && upper, "tb_ehvi_set_cells: null argument");
+  TB_CHECK(K >= 1, "tb_ehvi_set_cells: need at least one cell");
+  TB_CUDA(cudaSetDevice(h->device));
+  const size_t n = (size_t)K * h->L;
+  cudaStream_t st = h->m[0]->stream;
+  TB_TRY(h->dCells.reserve(sizeof(double) * 2 * n));
+  TB_CUDA(cudaMemcpyAsync(h->dCells.p, lower, sizeof(double) * n, cudaMemcpyDefault, st));
+  TB_CUDA(cudaMemcpyAsync(h->dCells.as<double>() + n, upper, sizeof(double) * n, cudaMemcpyDefault, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  h->K = K;
+  return 0;
+}
+
+int tb_ehvi_eval(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad) {
+  TB_CHECK(h && (M == 0 || (Xc && out)), "tb_ehvi_eval: null argument");
+  TB_CHECK(M >= 0, "tb_ehvi_eval: negative candidate count");
+  TB_TRY(tb::ehvi_check(h, "tb_ehvi_eval"));
+  tb::EhviRequest rq;
+  rq.M = M;
+  tb::DtypeBridge br(h->m[0]);
+  TB_TRY(br.in(Xc, M * h->D, &rq.Xc));
+  TB_TRY(br.out(out, M, &rq.out_vals));
+  TB_TRY(br.out(grad, M * h->D, &rq.out_grad));
+  TB_TRY(tb::ehvi_run(h, rq));
+  return br.finish();
+}
+
+int tb_ehvi_argmax(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* best_value, int64_t* best_index) {
+  TB_CHECK(h && Xc && best_value && best_index, "tb_ehvi_argmax: null argument");
+  TB_CHECK(M > 0, "tb_ehvi_argmax: argmax over an empty candidate set");
+  TB_TRY(tb::ehvi_check(h, "tb_ehvi_argmax"));
+  tb::EhviRequest rq;
+  rq.M = M;
+  rq.want_argmax = true;
+  tb::DtypeBridge br(h->m[0]);
+  TB_TRY(br.in(Xc, M * h->D, &rq.Xc));
+  TB_TRY(br.out(out, M, &rq.out_vals));
+  TB_TRY(tb::ehvi_run(h, rq));
+  if (rq.best_index == INT64_MAX) {  // every value was NaN: tf.math.argmax still returns a valid index
+    rq.best_index = 0;
+    rq.best_value = std::nan("");
+  }
+  if (h->dtype == TB_F32) *(float*)best_value = (float)rq.best_value;
+  else *(double*)best_value = rq.best_value;
+  *best_index = rq.best_index;
+  return br.finish();
+}
+
+int tb_ehvi_maximize(tb_ehvi* h, const double* lower, const double* upper, const double* starts, int64_t P, int maxcor,
+                     int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
+                     int64_t* nfev) {
+  TB_CHECK(h && lower && upper, "tb_ehvi_maximize: null argument");
+  TB_CHECK(P >= 0 && P < ((int64_t)1 << 31), "tb_ehvi_maximize: number of starts out of range");
+  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_ehvi_maximize: null argument");
+  TB_TRY(tb::check_lbfgs_options("tb_ehvi_maximize", maxcor, maxiter, maxls, gtol, ftol));
+  TB_TRY(tb::ehvi_check(h, "tb_ehvi_maximize"));
+  if (P == 0) return 0;
+  TB_CUDA(cudaSetDevice(h->device));
+  auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad) -> int {
+    tb::EhviRequest rq;
+    rq.Xc = xt;
+    rq.M = n;
+    rq.out_vals = vals;
+    rq.out_grad = grad;
+    return tb::ehvi_run(h, rq);
+  };
+  return tb::lbfgs_run("tb_ehvi_maximize", h->m[0]->stream, h->D, lower, upper, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol,
+                       eval, x_out, f_out, success, nfev);
 }
 
 }  // extern "C"

@@ -448,3 +448,56 @@ class GaussianProcessRegression:
 
 def _ptr(a) -> int:
     return a.data_ptr() if _lib.is_torch(a) else a.ctypes.data
+
+
+class ModelStack:
+    """Independent models side by side along the output axis (interfaces.py:337-397): ``ModelStack((m1, 1), (m2, 1))``.
+    ``predict`` and ``sample`` concatenate the members' outputs along the last axis in member order."""
+
+    def __init__(self, model_with_event_size, *models_with_event_sizes):
+        pairs = (model_with_event_size,) + models_with_event_sizes
+        self._models, self._event_sizes = (tuple(x) for x in zip(*pairs))
+
+    @property
+    def models(self):
+        return self._models
+
+    @property
+    def event_sizes(self):
+        return self._event_sizes
+
+    def predict(self, query_points):
+        means, vars_ = zip(*(m.predict(query_points) for m in self._models))
+        return _concat_last(means), _concat_last(vars_)
+
+    def sample(self, query_points, num_samples: int):
+        return _concat_last([m.sample(query_points, num_samples) for m in self._models])
+
+    def log(self, dataset: Optional[Dataset] = None) -> None:
+        for m in self._models:
+            m.log(dataset)
+
+
+class TrainableModelStack(ModelStack):
+    """A :class:`ModelStack` of trainable members (interfaces.py:400-443): ``update`` and ``optimize`` give member i the
+    observation columns of its event."""
+
+    def _split(self, dataset: Dataset):
+        obs = np.asarray(dataset.observations)
+        edges = np.cumsum(self._event_sizes)[:-1]
+        return [Dataset(dataset.query_points, o) for o in np.split(obs, edges, axis=-1)]
+
+    def update(self, dataset: Dataset) -> None:
+        for m, d in zip(self._models, self._split(dataset)):
+            m.update(d)
+
+    def optimize(self, dataset: Dataset):
+        return [m.optimize(d) for m, d in zip(self._models, self._split(dataset))]
+
+
+def _concat_last(parts):
+    if _lib.is_torch(parts[0]):
+        import torch
+
+        return torch.cat(list(parts), dim=-1)
+    return np.concatenate([np.asarray(p) for p in parts], axis=-1)

@@ -55,3 +55,52 @@ def hartmann_6(x):
     a = np.array([1.0, 1.2, 3.0, 3.2])
     inner = -(_H6_A * (x[..., None, :] - _H6_P) ** 2).sum(-1)
     return -(a * np.exp(inner)).sum(-1, keepdims=True)
+
+
+# ---- multi-objective (trieste/objectives/multi_objectives.py): minimisation, values [..., L] ----
+def vlmop2(x, d: int):
+    """VLMOP2 (:60-73): 1 - exp(-|x - 1/sqrt(d)|^2) and 1 - exp(-|x + 1/sqrt(d)|^2), on [-2, 2]^d."""
+    x = np.asarray(x, dtype=np.float64)
+    if x.shape[-1] != d:
+        raise ValueError(f"x must have trailing dimension {d}, got {x.shape}")
+    t = 1.0 / math.sqrt(d)
+    y1 = 1.0 - np.exp(-np.sum((x - t) ** 2, axis=-1))
+    y2 = 1.0 - np.exp(-np.sum((x + t) ** 2, axis=-1))
+    return np.stack([y1, y2], axis=-1)
+
+
+def vlmop2_pareto_optimal_points(n: int, d: int):
+    """n points of the VLMOP2 Pareto front (:88-92): the images of the segment x_i = s, s in [-1/sqrt(d), 1/sqrt(d)]."""
+    if n <= 0:
+        raise ValueError(f"n must be positive, got {n}")
+    t = 1.0 / math.sqrt(d)
+    x = np.tile(np.linspace(-t, t, n)[:, None], (1, d))
+    return vlmop2(x, d)
+
+
+def dtlz2(x, m: int, d: int):
+    """DTLZ2 (:184-212) with m objectives on [0, 1]^d (d > m): objective i is
+    (1 + g) prod_{j < m-1-i} cos(pi x_j / 2), times sin(pi x_{m-1-i} / 2) for i > 0, with g = sum_{j >= m-1} (x_j - 1/2)^2."""
+    x = np.asarray(x, dtype=np.float64)
+    if x.shape[-1] != d:
+        raise ValueError(f"x must have trailing dimension {d}, got {x.shape}")
+    if not 0 < m < d:
+        raise ValueError(f"need 0 < m < d, got m = {m}, d = {d}")
+    g = np.sum((x[..., m - 1:] - 0.5) ** 2, axis=-1)
+    cos = np.cos(0.5 * math.pi * x)
+    out = []
+    for i in range(m):
+        y = 1.0 + g
+        y = y * np.prod(cos[..., : m - 1 - i], axis=-1)
+        if i > 0:
+            y = y * np.sin(0.5 * math.pi * x[..., m - 1 - i])
+        out.append(y)
+    return np.stack(out, axis=-1)
+
+
+def dtlz2_pareto_optimal_points(n: int, m: int, seed=None):
+    """n points of the DTLZ2 Pareto front (:226-230): the positive orthant of the unit sphere in m objectives."""
+    if m < 2:
+        raise ValueError(f"need at least two objectives, got {m}")
+    r = np.random.default_rng(seed).standard_normal((n, m))
+    return np.abs(r / np.linalg.norm(r, axis=-1, keepdims=True))
