@@ -1270,7 +1270,9 @@ static int eng_store_v(tb_gp* gp, Engine e, int tiles, int64_t McPad) {
 // per-candidate driver
 // =================================================================================================
 
-// the running argmax of a call in gp->sRun (best value, then its index)
+// The running argmax of a call in gp->sRun (best value, then its index).  argmax_begin reserves it, and the tail's per-block
+// winners of chunks of up to chunk_cap candidates, and resets it; argmax_fold folds one chunk's winners in; argmax_end reads
+// the winner into rq (the caller synchronises).
 static int argmax_reset(tb_gp* gp) {
   const double init_v = -INFINITY;  // a candidate worth -inf still beats "nothing seen" through the lower-index tie rule
   const int64_t init_i = INT64_MAX;
@@ -1278,13 +1280,20 @@ static int argmax_reset(tb_gp* gp) {
   TB_CUDA(cudaMemcpyAsync((char*)gp->sRun.p + 8, &init_i, 8, cudaMemcpyHostToDevice, gp->stream));
   return 0;
 }
+static int argmax_begin(tb_gp* gp, int64_t chunk_cap) {
+  const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
+  TB_TRY(gp->sRun.reserve(16));
+  TB_TRY(gp->sBlkBest.reserve(sizeof(double) * tail_blocks_cap));
+  TB_TRY(gp->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
+  return argmax_reset(gp);
+}
 static int argmax_fold(tb_gp* gp, int64_t n) {  // the tail's per-block winners of n candidates into gp->sRun
   argmax_fold_kernel<<<1, 256, 0, gp->stream>>>(gp->sBlkBest.as<double>(), gp->sBlkIdx.as<int64_t>(), (int)((n + 255) / 256),
                                                 gp->sRun.as<double>(), reinterpret_cast<int64_t*>((char*)gp->sRun.p + 8));
   TB_LAUNCHED();
   return 0;
 }
-static int argmax_read(tb_gp* gp, EvalRequest& rq) {
+static int argmax_end(tb_gp* gp, EvalRequest& rq) {
   TB_CUDA(cudaMemcpyAsync(&rq.best_value, gp->sRun.p, 8, cudaMemcpyDeviceToHost, gp->stream));
   TB_CUDA(cudaMemcpyAsync(&rq.best_index, (char*)gp->sRun.p + 8, 8, cudaMemcpyDeviceToHost, gp->stream));
   return 0;
@@ -1325,26 +1334,38 @@ struct EvalOut {
   double *vals = nullptr, *mean = nullptr, *var = nullptr, *grad = nullptr;
 };
 
-// One chunk of n device candidates at xc: K* and the means, the variance GEMM over G row-block groups, the gradient when
-// o.grad is set, the acquisition tail and the argmax fold.  c0: global index of the first candidate.  The screened argmax's
-// gathered candidates pass their global indices in idx_map instead, and the k-split of the chunk they come from; when they
-// are too few tiles for the row-block groups to fill the SMs, the int8 engines spread them wider (split-K variance GEMM, wide
-// K* generation) with the same results.
-static int eval_chunk(tb_gp* gp, const EvalRequest& rq, Engine e, const double* xc, int64_t n, int64_t c0, int G, const EvalOut& o,
-                      const int64_t* idx_map = nullptr, const KSplit* split = nullptr) {
-  cudaStream_t st = gp->stream;
+// One handle's share of a chunk of n device candidates at xc, on the handle's stream: K* and the means (gp->sKs, gp->sMean),
+// the variance sums of squares (gp->sPartial) and, with grad, V = K^-1 K* (gp->sV).  Gfix: the call's row-block groups (0:
+// eng_groups of this chunk); *G and *McPad return the groups and the candidates padded to whole tiles, the layout of
+// gp->sPartial.  The screened argmax passes the k-split of the chunk its candidates come from, and spread: when they are too
+// few tiles for the row-block groups to fill the SMs, the int8 engines spread them wider (split-K variance GEMM, wide K*
+// generation) with the same results.
+static int member_step(tb_gp* gp, Engine e, const double* xc, int64_t n, int Gfix, bool grad, int* G, int64_t* McPad,
+                       const KSplit* split = nullptr, bool spread = false) {
   const int nt = eng_tile_width(gp, e);
   const int tiles = (int)((n + nt - 1) / nt);
-  const int64_t McPad = (int64_t)tiles * nt;
+  *G = Gfix ? Gfix : eng_groups(gp, e, tiles);
+  *McPad = (int64_t)tiles * nt;
+  const int kper = spread && e != Engine::F64 ? int8_split_kper(gp, e == Engine::OZ15, tiles, *G) : 0;
+  TB_TRY(eng_kstar(gp, e, xc, n, tiles, split, kper > 0));
+  TB_TRY(profiled_gemm(gp, (double)*McPad * (double)gp->N * (double)gp->N,
+                       [&] { return eng_variance(gp, e, tiles, *G, *McPad, grad, kper); }));
+  return grad ? eng_store_v(gp, e, tiles, *McPad) : 0;
+}
+
+// One chunk of n device candidates at xc: member_step, then with o.grad the partials d acq / d (mean, var) and the gradient
+// assembly, then the acquisition tail and the argmax fold.  c0: global index of the first candidate.  The screened argmax's
+// gathered candidates pass their global indices in idx_map instead, and the k-split of the chunk they come from.
+static int eval_chunk(tb_gp* gp, const EvalRequest& rq, Engine e, const double* xc, int64_t n, int64_t c0, int Gfix, const EvalOut& o,
+                      const int64_t* idx_map = nullptr, const KSplit* split = nullptr) {
+  cudaStream_t st = gp->stream;
   const double* partial = gp->sPartial.as<double>();
   const double* mean = gp->sMean.as<double>();
-  const int kper = idx_map && e != Engine::F64 ? int8_split_kper(gp, e == Engine::OZ15, tiles, G) : 0;
-  TB_TRY(eng_kstar(gp, e, xc, n, tiles, split, kper > 0));
-  TB_TRY(profiled_gemm(gp, (double)McPad * (double)gp->N * (double)gp->N,
-                       [&] { return eng_variance(gp, e, tiles, G, McPad, o.grad != nullptr, kper); }));
+  int G;
+  int64_t McPad;
+  TB_TRY(member_step(gp, e, xc, n, Gfix, o.grad != nullptr, &G, &McPad, split, idx_map != nullptr));
   if (o.grad) {
     TB_TRY(launch_partials(gp, st, rq.acq, rq.param, partial, G, McPad, mean, xc, n));
-    TB_TRY(eng_store_v(gp, e, tiles, McPad));
     TB_TRY(launch_grad(gp, xc, n, o.grad));
   }
   TB_TRY(launch_tail(gp, st, rq, partial, G, McPad, mean, n, c0, o.vals, o.mean, o.var, xc, o.grad, idx_map));
@@ -1426,39 +1447,66 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, Engine e, int64_t c
   return 0;
 }
 
-// Chunk geometry of run_eval: candidates per tile (nt), candidates per chunk (chunk_cap) and the row-block groups G, fixed
-// for the call when G > 0, else eng_groups of each chunk.  The screened argmax and the k-split of the single-pass engine
-// reproduce these chunks, so they must not drift.
+// Chunk geometry of a call over the n handles gps with engines eng (one for run_eval, the members for ehvi_run): candidates
+// per chunk (chunk_cap, the smallest of the handles' own) and each handle's row-block groups G[l], fixed for the call when
+// G[l] > 0, else eng_groups of each chunk.  The screened argmax and the k-split of the single-pass engine reproduce these
+// chunks, so they must not drift; with one handle chunk_cap is a whole number of its tiles.  A handle's own chunk size:
 //   int8 engines, values: K* digit scratch within 1,280 MB, whole pairs of waves (or one wave), at most 8 waves; G of the
 //                         first chunk for the whole call
 //   single-pass engine, gradients: K* digits or V (NB*128 doubles per candidate), whichever is larger, within 1,280 MB,
 //                         whole waves
 //   fp64 engine, and the 21-product engine's gradients: chunk_tiles
+// A handle whose own chunk size is the common one therefore sums each candidate's variance exactly as its tb_gp_predict does;
+// the others agree with it to rounding.
 struct ChunkPlan {
-  int nt = BT;
   int64_t chunk_cap = 0;
-  int G = 0;
+  int G[EHVI_LMAX] = {};
 };
-static ChunkPlan plan_chunks(const tb_gp* gp, Engine e, bool grad, int64_t M) {
+static ChunkPlan plan_chunks(tb_gp* const* gps, const Engine* eng, int n, bool grad, int64_t M) {
   ChunkPlan p;
-  p.nt = eng_tile_width(gp, e);
   const size_t budget = (size_t)1280 << 20;
-  int64_t max_tiles;
-  if (e != Engine::F64 && !grad) {
-    max_tiles = std::max<int64_t>(1, (int64_t)(budget / eng_tile_bytes(gp, e)));
-    if (max_tiles >= 2 * NUM_SMS) max_tiles = (max_tiles / (2 * NUM_SMS)) * (2 * NUM_SMS);
-    else if (max_tiles >= NUM_SMS) max_tiles = NUM_SMS;
-    max_tiles = std::min<int64_t>(max_tiles, 8 * NUM_SMS);
-  } else if (e == Engine::OZ15) {
-    const size_t v_bytes = (size_t)p.nt * gp->NB * BM * sizeof(double);
-    max_tiles = std::max<int64_t>(1, (int64_t)(budget / std::max(eng_tile_bytes(gp, e), v_bytes)));
-    if (max_tiles >= NUM_SMS) max_tiles = (max_tiles / NUM_SMS) * NUM_SMS;
-  } else {
-    max_tiles = chunk_tiles(gp);
+  for (int l = 0; l < n; ++l) {
+    const tb_gp* gp = gps[l];
+    const Engine e = eng[l];
+    const int nt = eng_tile_width(gp, e);
+    int64_t max_tiles;
+    if (e != Engine::F64 && !grad) {
+      max_tiles = std::max<int64_t>(1, (int64_t)(budget / eng_tile_bytes(gp, e)));
+      if (max_tiles >= 2 * NUM_SMS) max_tiles = (max_tiles / (2 * NUM_SMS)) * (2 * NUM_SMS);
+      else if (max_tiles >= NUM_SMS) max_tiles = NUM_SMS;
+      max_tiles = std::min<int64_t>(max_tiles, 8 * NUM_SMS);
+    } else if (e == Engine::OZ15) {
+      const size_t v_bytes = (size_t)nt * gp->NB * BM * sizeof(double);
+      max_tiles = std::max<int64_t>(1, (int64_t)(budget / std::max(eng_tile_bytes(gp, e), v_bytes)));
+      if (max_tiles >= NUM_SMS) max_tiles = (max_tiles / NUM_SMS) * NUM_SMS;
+    } else {
+      max_tiles = chunk_tiles(gp);
+    }
+    const int64_t cap = std::min<int64_t>(max_tiles * nt, ((M + nt - 1) / nt) * nt);
+    p.chunk_cap = l == 0 ? cap : std::min(p.chunk_cap, cap);
   }
-  p.chunk_cap = std::min<int64_t>(max_tiles * p.nt, ((M + p.nt - 1) / p.nt) * p.nt);
-  if (e != Engine::F64 && !grad) p.G = eng_groups(gp, e, (int)(p.chunk_cap / p.nt));
+  for (int l = 0; l < n; ++l) {
+    const int nt = eng_tile_width(gps[l], eng[l]);
+    if (eng[l] != Engine::F64 && !grad) p.G[l] = eng_groups(gps[l], eng[l], (int)((p.chunk_cap + nt - 1) / nt));
+  }
   return p;
+}
+
+// One handle's chunk scratch for chunks of up to chunk_cap candidates (padded to its tiles) on engine e: K*, the variance sums
+// of squares over G row-block groups (0: per chunk, at most NB), the means and, with grad, the packed A (fp64 engine), V and
+// d acq / d (mean, var)
+static int reserve_chunk(tb_gp* gp, Engine e, bool grad, int64_t chunk_cap, int G) {
+  const int nt = eng_tile_width(gp, e);
+  const int64_t tiles_cap = (chunk_cap + nt - 1) / nt, pad_cap = tiles_cap * nt;
+  TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
+  TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)(G ? G : gp->NB) * pad_cap));
+  TB_TRY(gp->sMean.reserve(sizeof(double) * pad_cap));
+  if (grad) {
+    if (e == Engine::F64) TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));  // packed A
+    TB_TRY(gp->sV.reserve((size_t)pad_cap * gp->NB * BM * sizeof(double)));
+    TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * pad_cap));
+  }
+  return 0;
 }
 
 // the argument checks of run_eval, made before anything is staged
@@ -1476,58 +1524,42 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
   cudaStream_t st = gp->stream;
   const int D = gp->D;
   const bool grad = rq.out_grad != nullptr;
-  if (rq.want_argmax) {
-    TB_TRY(gp->sRun.reserve(16));
-    TB_TRY(argmax_reset(gp));
-  }
   if (rq.M == 0) return 0;
   if (grad) TB_CHECK(rq.acq >= 0, "gradients need an acquisition kind");
   Engine e;
   TB_TRY(select_engine(gp, grad, &e));
-  const ChunkPlan cp = plan_chunks(gp, e, grad, rq.M);
-  const int64_t chunk_cap = cp.chunk_cap, tiles_cap = chunk_cap / cp.nt;
+  const ChunkPlan cp = plan_chunks(&gp, &e, 1, grad, rq.M);
+  const int64_t chunk_cap = cp.chunk_cap;
   // a host out_mean is copied from gp->sMean, which the K* step fills anyway
   const Staged<const double> xin(rq.Xc, D, gp->sXc, st);
   const Staged<double> vals(rq.out_vals, 1, gp->sVals, st), mean(rq.out_mean, 1, gp->sMean, st), var(rq.out_var, 1, gp->sVar, st),
       grads(rq.out_grad, D, gp->sGrad, st);
-  TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, e)));
-  TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)(cp.G ? cp.G : gp->NB) * chunk_cap));
-  TB_TRY(gp->sMean.reserve(sizeof(double) * chunk_cap));
+  TB_TRY(reserve_chunk(gp, e, grad, chunk_cap, cp.G[0]));
   TB_TRY(xin.reserve(chunk_cap));
   TB_TRY(vals.reserve(chunk_cap));
   TB_TRY(var.reserve(chunk_cap));
-  if (grad) {
-    if (e == Engine::F64) TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));  // packed A
-    TB_TRY(gp->sV.reserve((size_t)chunk_cap * gp->NB * BM * sizeof(double)));
-    TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * chunk_cap));
-    TB_TRY(grads.reserve(chunk_cap));
-  }
-  if (rq.want_argmax) {
-    const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
-    TB_TRY(gp->sBlkBest.reserve(sizeof(double) * tail_blocks_cap));
-    TB_TRY(gp->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
-  }
+  TB_TRY(grads.reserve(chunk_cap));
+  if (rq.want_argmax) TB_TRY(argmax_begin(gp, chunk_cap));
 
   bool screened = false;
-  if (e != Engine::F64 && argmax_screen_wanted(rq, xin.dev)) TB_TRY(argmax_screened(gp, rq, e, chunk_cap, cp.G, &screened));
+  if (e != Engine::F64 && argmax_screen_wanted(rq, xin.dev)) TB_TRY(argmax_screened(gp, rq, e, chunk_cap, cp.G[0], &screened));
   const int64_t m_loop = screened ? 0 : rq.M;  // the screened path has folded its survivors into gp->sRun already
   for (int64_t c0 = 0; c0 < m_loop; c0 += chunk_cap) {
     const int64_t mc = std::min<int64_t>(chunk_cap, rq.M - c0);
     const double* xc;
     TB_TRY(xin.in(c0, mc, &xc));
-    const int G = cp.G ? cp.G : eng_groups(gp, e, (int)((mc + cp.nt - 1) / cp.nt));
     EvalOut o;
     o.vals = vals.out(c0);
     o.mean = mean.host() ? nullptr : mean.out(c0);
     o.var = var.out(c0);
     o.grad = grads.out(c0);
-    TB_TRY(eval_chunk(gp, rq, e, xc, mc, c0, G, o));
+    TB_TRY(eval_chunk(gp, rq, e, xc, mc, c0, cp.G[0], o));
     TB_TRY(grads.back(c0, mc));
     TB_TRY(vals.back(c0, mc));
     TB_TRY(mean.back(c0, mc));
     TB_TRY(var.back(c0, mc));
   }
-  if (rq.want_argmax) TB_TRY(argmax_read(gp, rq));
+  if (rq.want_argmax) TB_TRY(argmax_end(gp, rq));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
   return profile_fold(gp);
@@ -1679,8 +1711,10 @@ int tb_gp_mean_gradient(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* 
   return br.finish();
 }
 
-// TB_ACQ_PENALIZED is stripped from acq here: every kernel and check below sees the plain kind
-static int split_penalized(const tb_gp* gp, int& acq, bool& pen, const char* who) {
+// The acquisition arguments of tb_acq_eval, tb_acq_argmax and tb_acq_maximize, and the handle state their kind reads (the
+// local penalty, min-value samples, GIBBON's pending points, whose derived state is brought up to date with the posterior
+// cache here).  TB_ACQ_PENALIZED is stripped from acq into pen: every kernel and check below sees the plain kind.
+static int check_acq(tb_gp* gp, int& acq, double param, bool& pen, const char* who) {
   pen = (acq & TB_ACQ_PENALIZED) != 0;
   acq &= ~TB_ACQ_PENALIZED;
   TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_GIBBON, std::string(who) + ": unknown acquisition kind");
@@ -1689,12 +1723,9 @@ static int split_penalized(const tb_gp* gp, int& acq, bool& pen, const char* who
   if (pen)
     TB_CHECK(gp->penP > 0 && gp->penD == gp->D,
              std::string(who) + ": a penalised acquisition needs the local penalty first (tb_acq_set_penalization)");
-  return 0;
-}
-
-// the handle state a GIBBON kind reads: min-value samples for the quality term; pending points for the repulsion term, whose
-// derived state is brought up to date with the posterior cache here
-static int prepare_gibbon(tb_gp* gp, int acq, const char* who) {
+  if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
+    TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
+  if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
   if (acq < TB_ACQ_GIBBON_QUALITY) return 0;
   if (acq != TB_ACQ_GIBBON_REPULSION)
     TB_CHECK(gp->mesS > 0, std::string(who) + ": GIBBON's quality term needs the min-value samples first (tb_acq_set_min_value_samples)");
@@ -1706,56 +1737,44 @@ static int prepare_gibbon(tb_gp* gp, int acq, const char* who) {
   return 0;
 }
 
-int tb_acq_eval(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad) {
-  TB_CHECK(gp && (M == 0 || (Xc && out)), "tb_acq_eval: null argument");
-  bool pen = false;
-  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_eval"));
-  if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
-    TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
-  if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
-  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_eval"));
+// The winner of an argmax as the ABI returns it, best_value in the handle's dtype.  Every value NaN: index 0 and value NaN,
+// as tf.math.argmax still returns a valid index (optimizer.py:149).
+static void argmax_result(const tb::EvalRequest& rq, int dtype, void* best_value, int64_t* best_index) {
+  const bool none = rq.best_index == INT64_MAX;
+  const double v = none ? std::nan("") : rq.best_value;
+  if (dtype == TB_F32) *(float*)best_value = (float)v;
+  else *(double*)best_value = v;
+  *best_index = none ? 0 : rq.best_index;
+}
+
+// tb_acq_eval, and tb_acq_argmax when best_index is set
+static int acq_call(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad, void* best_value,
+                    int64_t* best_index, const char* who) {
   tb::EvalRequest rq;
+  TB_TRY(check_acq(gp, acq, param, rq.pen, who));
   rq.acq = acq;
-  rq.pen = pen;
   rq.param = param;
   rq.M = M;
+  rq.want_argmax = best_index != nullptr;
   TB_TRY(tb::check_eval(gp, rq));
   tb::DtypeBridge br(gp);
   TB_TRY(br.in(Xc, M * gp->D, &rq.Xc));
   TB_TRY(br.out(out, M, &rq.out_vals));
   TB_TRY(br.out(grad, M * gp->D, &rq.out_grad));
   TB_TRY(tb::run_eval(gp, rq));
+  if (best_index) argmax_result(rq, gp->dtype, best_value, best_index);
   return br.finish();
+}
+
+int tb_acq_eval(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* grad) {
+  TB_CHECK(gp && (M == 0 || (Xc && out)), "tb_acq_eval: null argument");
+  return acq_call(gp, acq, param, Xc, M, out, grad, nullptr, nullptr, "tb_acq_eval");
 }
 
 int tb_acq_argmax(tb_gp* gp, int acq, double param, const void* Xc, int64_t M, void* out, void* best_value,
                   int64_t* best_index) {
   TB_CHECK(gp && Xc && best_value && best_index, "tb_acq_argmax: null argument");
-  bool pen = false;
-  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_argmax"));
-  if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
-    TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
-  if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
-  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_argmax"));
-  tb::EvalRequest rq;
-  rq.acq = acq;
-  rq.pen = pen;
-  rq.param = param;
-  rq.M = M;
-  rq.want_argmax = true;
-  TB_TRY(tb::check_eval(gp, rq));
-  tb::DtypeBridge br(gp);
-  TB_TRY(br.in(Xc, M * gp->D, &rq.Xc));
-  TB_TRY(br.out(out, M, &rq.out_vals));
-  TB_TRY(tb::run_eval(gp, rq));
-  if (rq.best_index == INT64_MAX) {  // every value was NaN: tf.math.argmax still returns a valid index (optimizer.py:149)
-    rq.best_index = 0;
-    rq.best_value = std::nan("");
-  }
-  if (gp->dtype == TB_F32) *(float*)best_value = (float)rq.best_value;
-  else *(double*)best_value = rq.best_value;
-  *best_index = rq.best_index;
-  return br.finish();
+  return acq_call(gp, acq, param, Xc, M, out, nullptr, best_value, best_index, "tb_acq_argmax");
 }
 
 int tb_acq_set_min_value_samples(tb_gp* gp, const double* samples, int S) {
@@ -2676,10 +2695,14 @@ __global__ void lbfgs_finish_kernel(tb::lb::State s, int64_t P, double* __restri
 }  // extern "C"
 
 namespace tb {
-static int check_lbfgs_options(const std::string& name, int maxcor, int maxiter, int maxls, double gtol, double ftol) {
-  TB_CHECK(maxcor >= 1 && maxcor <= lb::MMAX, name + ": maxcor must be in [1, " + std::to_string(lb::MMAX) + "]");
-  TB_CHECK(maxiter >= 1 && maxls >= 1, name + ": maxiter and maxls must be positive");
-  TB_CHECK(gtol >= 0.0 && ftol >= 0.0, name + ": tolerances must be non-negative");
+// the arguments of every device maximiser: P starts (and their outputs) and the L-BFGS options
+static int check_starts(const std::string& who, int64_t P, const double* starts, const double* x_out, const double* f_out,
+                        const int32_t* success, const int64_t* nfev, int maxcor, int maxiter, int maxls, double gtol, double ftol) {
+  TB_CHECK(P >= 0 && P < ((int64_t)1 << 31), who + ": number of starts out of range");
+  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), who + ": null argument");
+  TB_CHECK(maxcor >= 1 && maxcor <= lb::MMAX, who + ": maxcor must be in [1, " + std::to_string(lb::MMAX) + "]");
+  TB_CHECK(maxiter >= 1 && maxls >= 1, who + ": maxiter and maxls must be positive");
+  TB_CHECK(gtol >= 0.0 && ftol >= 0.0, who + ": tolerances must be non-negative");
   return 0;
 }
 
@@ -2776,16 +2799,10 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
                     int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
                     int32_t* success, int64_t* nfev) {
   TB_CHECK(gp && lower && upper, "tb_acq_maximize: null argument");
-  TB_CHECK(P >= 0 && P < ((int64_t)1 << 31), "tb_acq_maximize: number of starts out of range");
-  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_acq_maximize: null argument");
-  bool pen = false;
-  TB_TRY(split_penalized(gp, acq, pen, "tb_acq_maximize"));
-  if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
-    TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
-  if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
-  TB_TRY(tb::check_lbfgs_options("tb_acq_maximize", maxcor, maxiter, maxls, gtol, ftol));
+  TB_TRY(tb::check_starts("tb_acq_maximize", P, starts, x_out, f_out, success, nfev, maxcor, maxiter, maxls, gtol, ftol));
   TB_CHECK(gp->cache_valid, "posterior cache is not built: call tb_gp_update_posterior_cache first");
-  TB_TRY(prepare_gibbon(gp, acq, "tb_acq_maximize"));
+  bool pen = false;
+  TB_TRY(check_acq(gp, acq, param, pen, "tb_acq_maximize"));
   if (P == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
   auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad) -> int {
@@ -2810,10 +2827,8 @@ int tb_rff_maximize_boxes(tb_rff* r, const double* lower, const double* upper, i
   TB_TRY(tb::check_rff_paired(r, "tb_rff_maximize"));
   TB_CHECK(nbox >= 1 && r->nb % nbox == 0, "tb_rff_maximize_boxes: the number of boxes " + std::to_string(nbox) +
                                                " must divide the trajectory batch size " + std::to_string(r->nb));
-  TB_CHECK(R >= 0 && R * r->nb < ((int64_t)1 << 31), "tb_rff_maximize: number of starts out of range");
-  const int64_t P = R * r->nb;
-  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_rff_maximize: null argument");
-  TB_TRY(tb::check_lbfgs_options("tb_rff_maximize", maxcor, maxiter, maxls, gtol, ftol));
+  const int64_t P = R * r->nb;  // nb >= 1 (check_rff_paired): P < 0 exactly when R < 0
+  TB_TRY(tb::check_starts("tb_rff_maximize", P, starts, x_out, f_out, success, nfev, maxcor, maxiter, maxls, gtol, ftol));
   if (P == 0) return 0;
   TB_CUDA(cudaSetDevice(r->device));
   const int D = r->D;
@@ -2973,16 +2988,6 @@ struct tb_ehvi {
 
 namespace tb {
 
-struct EhviRequest {
-  const double* Xc = nullptr;  // host or device, [M, D]
-  int64_t M = 0;
-  double* out_vals = nullptr;  // host or device (nullable)
-  double* out_grad = nullptr;  // [M, D] (nullable)
-  bool want_argmax = false;
-  double best_value = 0.0;
-  int64_t best_index = -1;
-};
-
 template <int L>
 static void launch_ehvi_l(bool grad, const EhviMembers& mb, const double* cells, int64_t K, int64_t mc, int64_t c0, double* vals,
                           double* bb, int64_t* bi, cudaStream_t st) {
@@ -3025,60 +3030,29 @@ static int ehvi_check(const tb_ehvi* h, const char* who) {
   return 0;
 }
 
-// The EHVI chunk loop.  The candidates are staged once, on the first member's stream st; each chunk runs every member's K*
-// and variance GEMM (and V for a gradient) on the member's own stream, then one EHVI kernel on st over all members' chunk
-// outputs, then the members' gradient assemblies and their fixed-order sum, then the argmax fold.  Events order the member
-// streams against st both ways; the host waits once, at the end.
-static int ehvi_run(tb_ehvi* h, EhviRequest& rq) {
+// The EHVI chunk loop (rq.acq unused).  The candidates are staged once, on the first member's stream st; each chunk runs every
+// member's member_step on the member's own stream, then one EHVI kernel on st over all members' chunk outputs, then the
+// members' gradient assemblies and their fixed-order sum, then the argmax fold.  Events order the member streams against st
+// both ways; the host waits once, at the end.
+static int ehvi_run(tb_ehvi* h, EvalRequest& rq) {
   TB_CUDA(cudaSetDevice(h->device));
   const int L = h->L, D = h->D;
   tb_gp* g0 = h->m[0];
   cudaStream_t st = g0->stream;
   const bool grad = rq.out_grad != nullptr;
-  if (rq.want_argmax) {
-    TB_TRY(g0->sRun.reserve(16));
-    TB_TRY(argmax_reset(g0));
-  }
   if (rq.M == 0) return 0;
-  std::vector<Engine> eng(L);
-  std::vector<ChunkPlan> plan(L);
-  int64_t chunk_cap = rq.M;
-  for (int l = 0; l < L; ++l) {
-    TB_TRY(select_engine(h->m[l], grad, &eng[l]));
-    plan[l] = plan_chunks(h->m[l], eng[l], grad, rq.M);
-    chunk_cap = std::min(chunk_cap, plan[l].chunk_cap);
-  }
-  // Row-block groups as plan_chunks chooses them, for the common chunk: fixed for the call from its first chunk where the
-  // member's plan fixes them (int8 values), else per chunk.  A member whose own chunk size is the common one therefore sums
-  // each candidate's variance exactly as its tb_gp_predict does; the others agree with it to rounding.
-  std::vector<int> gfix(L, 0);
-  for (int l = 0; l < L; ++l) {
-    tb_gp* gp = h->m[l];
-    const int nt = eng_tile_width(gp, eng[l]);
-    const int64_t tiles_cap = (chunk_cap + nt - 1) / nt, pad_cap = tiles_cap * nt;
-    if (plan[l].G) gfix[l] = eng_groups(gp, eng[l], (int)tiles_cap);
-    TB_TRY(gp->sKs.reserve((size_t)tiles_cap * eng_tile_bytes(gp, eng[l])));
-    TB_TRY(gp->sPartial.reserve(sizeof(double) * (size_t)gp->NB * pad_cap));
-    TB_TRY(gp->sMean.reserve(sizeof(double) * pad_cap));
-    if (grad) {
-      if (eng[l] == Engine::F64) TB_TRY(gp->sA.reserve((size_t)tiles_cap * gp->NB * (BM / BK) * PANEL * sizeof(double)));
-      TB_TRY(gp->sV.reserve((size_t)pad_cap * gp->NB * BM * sizeof(double)));
-      TB_TRY(gp->sMisc.reserve(sizeof(double) * 2 * chunk_cap));
-    }
-  }
+  Engine eng[EHVI_LMAX];
+  for (int l = 0; l < L; ++l) TB_TRY(select_engine(h->m[l], grad, &eng[l]));
+  const ChunkPlan cp = plan_chunks(h->m.data(), eng, L, grad, rq.M);
+  const int64_t chunk_cap = cp.chunk_cap;
+  for (int l = 0; l < L; ++l) TB_TRY(reserve_chunk(h->m[l], eng[l], grad, chunk_cap, cp.G[l]));
   const Staged<const double> xin(rq.Xc, D, h->sXc, st);
   const Staged<double> vals(rq.out_vals, 1, h->sVals, st), grads(rq.out_grad, D, h->sGrad, st);
   TB_TRY(xin.reserve(chunk_cap));
   TB_TRY(vals.reserve(chunk_cap));
-  if (grad) {
-    TB_TRY(grads.reserve(chunk_cap));
-    TB_TRY(h->sGradL.reserve(sizeof(double) * (size_t)L * chunk_cap * D));
-  }
-  if (rq.want_argmax) {
-    const int tail_blocks_cap = (int)((chunk_cap + 255) / 256);
-    TB_TRY(g0->sBlkBest.reserve(sizeof(double) * tail_blocks_cap));
-    TB_TRY(g0->sBlkIdx.reserve(sizeof(int64_t) * tail_blocks_cap));
-  }
+  TB_TRY(grads.reserve(chunk_cap));
+  if (grad) TB_TRY(h->sGradL.reserve(sizeof(double) * (size_t)L * chunk_cap * D));
+  if (rq.want_argmax) TB_TRY(argmax_begin(g0, chunk_cap));
   // st -> members (ev[0]) and member l -> st (ev[l])
   auto fan_out = [&]() -> int {
     TB_CUDA(cudaEventRecord(h->ev[0], st));
@@ -3099,21 +3073,11 @@ static int ehvi_run(tb_ehvi* h, EhviRequest& rq) {
     EhviMembers mb{};
     for (int l = 0; l < L; ++l) {
       tb_gp* gp = h->m[l];
-      const Engine e = eng[l];
-      const int nt = eng_tile_width(gp, e);
-      const int tiles = (int)((mc + nt - 1) / nt);
-      const int64_t McPad = (int64_t)tiles * nt;
-      const int G = gfix[l] ? gfix[l] : eng_groups(gp, e, tiles);
-      TB_TRY(eng_kstar(gp, e, xc, mc, tiles));
-      TB_TRY(profiled_gemm(gp, (double)McPad * (double)gp->N * (double)gp->N,
-                           [&] { return eng_variance(gp, e, tiles, G, McPad, grad); }));
-      if (grad) TB_TRY(eng_store_v(gp, e, tiles, McPad));
+      TB_TRY(member_step(gp, eng[l], xc, mc, cp.G[l], grad, &mb.G[l], &mb.McPad[l]));
       TB_TRY(join(l));
       mb.partial[l] = gp->sPartial.as<double>();
       mb.mean[l] = gp->sMean.as<double>();
       mb.dmv[l] = grad ? gp->sMisc.as<double>() : nullptr;
-      mb.McPad[l] = McPad;
-      mb.G[l] = G;
       mb.variance[l] = gp->variance;
     }
     TB_TRY(launch_ehvi(h, grad, mb, mc, c0, vals.out(c0), rq.want_argmax));
@@ -3132,12 +3096,9 @@ static int ehvi_run(tb_ehvi* h, EhviRequest& rq) {
     TB_TRY(grads.back(c0, mc));
     TB_TRY(vals.back(c0, mc));
   }
-  EvalRequest best;
-  if (rq.want_argmax) TB_TRY(argmax_read(g0, best));
+  if (rq.want_argmax) TB_TRY(argmax_end(g0, rq));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
-  rq.best_value = best.best_value;
-  rq.best_index = best.best_index;
   for (int l = 0; l < L; ++l) TB_TRY(profile_fold(h->m[l]));
   return 0;
 }
@@ -3200,53 +3161,44 @@ int tb_ehvi_set_cells(tb_ehvi* h, const double* lower, const double* upper, int6
   return 0;
 }
 
-int tb_ehvi_eval(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad) {
-  TB_CHECK(h && (M == 0 || (Xc && out)), "tb_ehvi_eval: null argument");
-  TB_CHECK(M >= 0, "tb_ehvi_eval: negative candidate count");
-  TB_TRY(tb::ehvi_check(h, "tb_ehvi_eval"));
-  tb::EhviRequest rq;
+// tb_ehvi_eval, and tb_ehvi_argmax when best_index is set
+static int ehvi_call(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad, void* best_value, int64_t* best_index,
+                     const char* who) {
+  TB_TRY(tb::ehvi_check(h, who));
+  tb::EvalRequest rq;
   rq.M = M;
+  rq.want_argmax = best_index != nullptr;
   tb::DtypeBridge br(h->m[0]);
   TB_TRY(br.in(Xc, M * h->D, &rq.Xc));
   TB_TRY(br.out(out, M, &rq.out_vals));
   TB_TRY(br.out(grad, M * h->D, &rq.out_grad));
   TB_TRY(tb::ehvi_run(h, rq));
+  if (best_index) argmax_result(rq, h->dtype, best_value, best_index);
   return br.finish();
+}
+
+int tb_ehvi_eval(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad) {
+  TB_CHECK(h && (M == 0 || (Xc && out)), "tb_ehvi_eval: null argument");
+  TB_CHECK(M >= 0, "tb_ehvi_eval: negative candidate count");
+  return ehvi_call(h, Xc, M, out, grad, nullptr, nullptr, "tb_ehvi_eval");
 }
 
 int tb_ehvi_argmax(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* best_value, int64_t* best_index) {
   TB_CHECK(h && Xc && best_value && best_index, "tb_ehvi_argmax: null argument");
   TB_CHECK(M > 0, "tb_ehvi_argmax: argmax over an empty candidate set");
-  TB_TRY(tb::ehvi_check(h, "tb_ehvi_argmax"));
-  tb::EhviRequest rq;
-  rq.M = M;
-  rq.want_argmax = true;
-  tb::DtypeBridge br(h->m[0]);
-  TB_TRY(br.in(Xc, M * h->D, &rq.Xc));
-  TB_TRY(br.out(out, M, &rq.out_vals));
-  TB_TRY(tb::ehvi_run(h, rq));
-  if (rq.best_index == INT64_MAX) {  // every value was NaN: tf.math.argmax still returns a valid index
-    rq.best_index = 0;
-    rq.best_value = std::nan("");
-  }
-  if (h->dtype == TB_F32) *(float*)best_value = (float)rq.best_value;
-  else *(double*)best_value = rq.best_value;
-  *best_index = rq.best_index;
-  return br.finish();
+  return ehvi_call(h, Xc, M, out, nullptr, best_value, best_index, "tb_ehvi_argmax");
 }
 
 int tb_ehvi_maximize(tb_ehvi* h, const double* lower, const double* upper, const double* starts, int64_t P, int maxcor,
                      int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
                      int64_t* nfev) {
   TB_CHECK(h && lower && upper, "tb_ehvi_maximize: null argument");
-  TB_CHECK(P >= 0 && P < ((int64_t)1 << 31), "tb_ehvi_maximize: number of starts out of range");
-  TB_CHECK(P == 0 || (starts && x_out && f_out && success && nfev), "tb_ehvi_maximize: null argument");
-  TB_TRY(tb::check_lbfgs_options("tb_ehvi_maximize", maxcor, maxiter, maxls, gtol, ftol));
+  TB_TRY(tb::check_starts("tb_ehvi_maximize", P, starts, x_out, f_out, success, nfev, maxcor, maxiter, maxls, gtol, ftol));
   TB_TRY(tb::ehvi_check(h, "tb_ehvi_maximize"));
   if (P == 0) return 0;
   TB_CUDA(cudaSetDevice(h->device));
   auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad) -> int {
-    tb::EhviRequest rq;
+    tb::EvalRequest rq;
     rq.Xc = xt;
     rq.M = n;
     rq.out_vals = vals;
