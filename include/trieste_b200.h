@@ -264,6 +264,13 @@ int tb_ehvi_destroy(tb_ehvi* h);
 /* the cells' bounds lower, upper [K, L] (fp64, host or device) as prepare_default_non_dominated_partition_bounds returns
  * them, in the objectives' minimisation orientation; K >= 1. */
 int tb_ehvi_set_cells(tb_ehvi* h, const double* lower, const double* upper, int64_t K);
+/* HIPPO's penalty (acquisition/function/multi_objective.py:664-758): every later evaluation, argmax and maximisation
+ * returns EHVI(x) * prod_p (2/pi) atan(d_p(x)), d_p(x) = sqrt(sum_l ((mean_l(x) - pending_mean[p, l]) / sqrt(pending_var[p, l]))^2),
+ * with its gradient.  pending_mean, pending_var [P, L] (fp64, host or device); P = 0 (null pointers allowed) removes the
+ * penalty, which a new object does not have.  Setting the state the object already holds copies nothing and does not
+ * synchronise (a device array is read back for the comparison).  TB_ERR_INVALID for P < 0, null arrays with P > 0, or a
+ * negative or NaN variance; the penalty held before then stays. */
+int tb_ehvi_set_penalty(tb_ehvi* h, const double* pending_mean, const double* pending_var, int P);
 /* Xc [M, D] -> out [M]; grad (nullable) [M, D].  The members' dtype, host or device pointers.  TB_ERR_INVALID if the cells
  * are not set or a member's posterior cache is not built. */
 int tb_ehvi_eval(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad);

@@ -67,6 +67,7 @@ SIGNATURES = {
     "tb_ehvi_create": (_i32, [C.POINTER(_vp), C.POINTER(_vp), _i32]),
     "tb_ehvi_destroy": (_i32, [_vp]),
     "tb_ehvi_set_cells": (_i32, [_vp, _vp, _vp, _i64]),
+    "tb_ehvi_set_penalty": (_i32, [_vp, _vp, _vp, _i32]),
     "tb_ehvi_eval": (_i32, [_vp, _vp, _i64, _vp, _vp]),
     "tb_ehvi_argmax": (_i32, [_vp, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
     "tb_ehvi_maximize": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),

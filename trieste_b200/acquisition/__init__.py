@@ -38,7 +38,13 @@ from .greedy_batch import (  # noqa: F401
     local_penalizer,
     soft_local_penalizer,
 )
-from .multi_objective import ExpectedHypervolumeImprovement, expected_hv_improvement  # noqa: F401
+from .multi_objective import (  # noqa: F401
+    HIPPO,
+    ExpectedHypervolumeImprovement,
+    expected_hv_improvement,
+    hippo_penalized_ehvi,
+    hippo_penalizer,
+)
 from .interface import (  # noqa: F401
     AcquisitionFunctionBuilder,
     GreedyAcquisitionFunctionBuilder,

@@ -15,6 +15,14 @@
 // d prod_l g_kl / d g_kl is the product of the other factors (prefix x suffix, no division: g may be 0).  The clipped
 // branch of max(., 0) passes no gradient; at equality the gradient goes to the difference, as tf.maximum sends it to its
 // first argument when x >= y.  dm/dmean = -1, ds/dvar = 1 / (2 s), and 0 where the variance is clipped.
+//
+// With PEN, HIPPO's penalty (trieste multi_objective.py:664-758) multiplies the value: for pending points p with stack
+// moments (mu_pl, sigma_pl) and the candidate's member means mean_l,
+//   d_p = sqrt(sum_l ((mean_l - mu_pl) / sigma_pl)^2),   w_p = (2/pi) atan(d_p),   pen = prod_p w_p,
+// the pending points streamed through the cell tiles' shared memory after the cells.  pen and G_l = d pen / d mean_l are
+// built in one pass in index order, G_l <- G_l w_p + pen w'_p dd_p/dmean_l and then pen <- pen w_p, with
+// w'_p = (2/pi) / (1 + d_p^2) and dd_p/dmean_l = (mean_l - mu_pl) / (sigma_pl^2 d_p), taken as 0 at d_p = 0: no division
+// by a factor that may be 0.  Then d/dmean_l = pen dEHVI/dmean_l + EHVI G_l and d/dvar_l = pen dEHVI/dvar_l.
 #pragma once
 #include "batch_ei.cuh"
 
@@ -23,6 +31,7 @@ namespace tb {
 constexpr int EHVI_LMAX = 8;
 constexpr int EHVI_TILE = 64;  // cells per shared-memory tile
 constexpr double EHVI_CLIP = 1e10;  // multi_objective.py:215
+constexpr double HIPPO_WARP = 0.63661977236758134308;  // 2 / pi, multi_objective.py:755
 
 // the chunk outputs of the L member handles, as the tail reads them
 struct EhviMembers {
@@ -32,6 +41,13 @@ struct EhviMembers {
   int64_t McPad[EHVI_LMAX];
   int G[EHVI_LMAX];
   double variance[EHVI_LMAX];
+};
+
+// HIPPO's penalty state: the pending points' stack moments, P >= 1 when a PEN kernel reads it
+struct EhviPenalty {
+  const double* mean;  // [P][L]
+  const double* sd;    // [P][L], sqrt of the stack's variances
+  int P;
 };
 
 // g(a, b) of one cell and objective, and with GRAD its derivatives in m and s
@@ -57,10 +73,10 @@ __device__ __forceinline__ double ehvi_factor(double a, double b, double m, doub
 }
 
 // cells: lower [K][L] then upper [K][L].  Candidate t's value to out_vals[t] (nullable); with blk_best the block's first-max
-// (NaN never wins) of (value, idx0 + t).
-template <int L, bool GRAD>
+// (NaN never wins) of (value, idx0 + t).  pen is read only with PEN.
+template <int L, bool GRAD, bool PEN>
 __global__ void __launch_bounds__(256)
-ehvi_kernel(const EhviMembers mb, const double* __restrict__ cells, int64_t K, int64_t Mc, int64_t idx0,
+ehvi_kernel(const EhviMembers mb, const EhviPenalty pen, const double* __restrict__ cells, int64_t K, int64_t Mc, int64_t idx0,
             double* __restrict__ out_vals, double* __restrict__ blk_best, int64_t* __restrict__ blk_idx) {
   __shared__ double sa[EHVI_TILE * L], sb[EHVI_TILE * L];
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -110,16 +126,54 @@ ehvi_kernel(const EhviMembers mb, const double* __restrict__ cells, int64_t K, i
       }
     }
   }
+  double pv = 1.0, G[L];  // penalty and its partials in the member means
+  if (PEN) {
+#pragma unroll
+    for (int l = 0; l < L; ++l) G[l] = 0.0;
+    for (int p0 = 0; p0 < pen.P; p0 += EHVI_TILE) {
+      const int np = pen.P - p0 < EHVI_TILE ? pen.P - p0 : EHVI_TILE;
+      __syncthreads();
+      for (int i = threadIdx.x; i < np * L; i += blockDim.x) {
+        sa[i] = pen.mean[(int64_t)p0 * L + i];
+        sb[i] = pen.sd[(int64_t)p0 * L + i];
+      }
+      __syncthreads();
+      if (!live) continue;
+      for (int p = 0; p < np; ++p) {
+        double r[L], d2 = 0.0;
+#pragma unroll
+        for (int l = 0; l < L; ++l) {
+          r[l] = (-m[l] - sa[p * L + l]) / sb[p * L + l];
+          d2 = fma(r[l], r[l], d2);
+        }
+        const double d = sqrt(d2);
+        const double w = HIPPO_WARP * atan(d);
+        if (GRAD) {
+          const double c = d > 0.0 ? pv * (HIPPO_WARP / (1.0 + d2)) / d : 0.0;
+#pragma unroll
+          for (int l = 0; l < L; ++l) G[l] = fma(G[l], w, c * (r[l] / sb[p * L + l]));
+        }
+        pv *= w;
+      }
+    }
+  }
   double bv = -INFINITY;
   int64_t bi = INT64_MAX;
   if (live) {
     if (GRAD) {
 #pragma unroll
       for (int l = 0; l < L; ++l) {
-        mb.dmv[l][t] = -am[l];
-        mb.dmv[l][Mc + t] = clipped[l] ? 0.0 : as[l] / (2.0 * s[l]);
+        const double dvar = clipped[l] ? 0.0 : as[l] / (2.0 * s[l]);
+        if (PEN) {
+          mb.dmv[l][t] = fma(pv, -am[l], val * G[l]);
+          mb.dmv[l][Mc + t] = pv * dvar;
+        } else {
+          mb.dmv[l][t] = -am[l];
+          mb.dmv[l][Mc + t] = dvar;
+        }
       }
     }
+    if (PEN) val *= pv;
     if (out_vals) out_vals[t] = val;
     if (val == val) {
       bv = val;

@@ -2982,6 +2982,9 @@ struct tb_ehvi {
   int L = 0, D = 0, device = 0, dtype = TB_F64;
   int64_t K = 0;          // cells; 0: not set
   tb::DevBuf dCells;      // lower [K][L] then upper [K][L]
+  int P = 0;              // HIPPO pending points (tb_ehvi_set_penalty); 0: no penalty
+  tb::DevBuf dPen;        // their means [P][L] then standard deviations [P][L]
+  std::vector<double> hPen;  // the means and variances [2][P][L] as last set, to recognise an unchanged push
   tb::DevBuf sXc, sVals, sGrad, sGradL;  // staged candidates, values, gradient, and the members' gradients [L][mc][D]
   std::vector<cudaEvent_t> ev;           // ev[l] orders member l's stream against the first member's (ev[0]: the other way)
 };
@@ -2989,13 +2992,19 @@ struct tb_ehvi {
 namespace tb {
 
 template <int L>
-static void launch_ehvi_l(bool grad, const EhviMembers& mb, const double* cells, int64_t K, int64_t mc, int64_t c0, double* vals,
-                          double* bb, int64_t* bi, cudaStream_t st) {
+static void launch_ehvi_l(bool grad, const EhviMembers& mb, const EhviPenalty& pen, const double* cells, int64_t K, int64_t mc,
+                          int64_t c0, double* vals, double* bb, int64_t* bi, cudaStream_t st) {
   const unsigned blocks = (unsigned)((mc + 255) / 256);
-  if (grad)
-    ehvi_kernel<L, true><<<blocks, 256, 0, st>>>(mb, cells, K, mc, c0, vals, bb, bi);
-  else
-    ehvi_kernel<L, false><<<blocks, 256, 0, st>>>(mb, cells, K, mc, c0, vals, bb, bi);
+  if (pen.P > 0) {
+    if (grad)
+      ehvi_kernel<L, true, true><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+    else
+      ehvi_kernel<L, false, true><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+  } else if (grad) {
+    ehvi_kernel<L, true, false><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+  } else {
+    ehvi_kernel<L, false, false><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+  }
 }
 
 static int launch_ehvi(tb_ehvi* h, bool grad, const EhviMembers& mb, int64_t mc, int64_t c0, double* vals, bool argmax) {
@@ -3003,14 +3012,16 @@ static int launch_ehvi(tb_ehvi* h, bool grad, const EhviMembers& mb, int64_t mc,
   double* bb = argmax ? g0->sBlkBest.as<double>() : nullptr;
   int64_t* bi = argmax ? g0->sBlkIdx.as<int64_t>() : nullptr;
   const double* cells = h->dCells.as<double>();
+  const double* pd = h->P > 0 ? h->dPen.as<double>() : nullptr;
+  const EhviPenalty pen{pd, pd ? pd + (size_t)h->P * h->L : nullptr, h->P};
   switch (h->L) {
-    case 2: launch_ehvi_l<2>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 3: launch_ehvi_l<3>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 4: launch_ehvi_l<4>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 5: launch_ehvi_l<5>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 6: launch_ehvi_l<6>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 7: launch_ehvi_l<7>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    default: launch_ehvi_l<8>(grad, mb, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 2: launch_ehvi_l<2>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 3: launch_ehvi_l<3>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 4: launch_ehvi_l<4>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 5: launch_ehvi_l<5>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 6: launch_ehvi_l<6>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 7: launch_ehvi_l<7>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    default: launch_ehvi_l<8>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
   }
   TB_LAUNCHED();
   TB_CUDA(cudaGetLastError());
@@ -3158,6 +3169,47 @@ int tb_ehvi_set_cells(tb_ehvi* h, const double* lower, const double* upper, int6
   TB_CUDA(cudaMemcpyAsync(h->dCells.as<double>() + n, upper, sizeof(double) * n, cudaMemcpyDefault, st));
   TB_CUDA(cudaStreamSynchronize(st));
   h->K = K;
+  return 0;
+}
+
+int tb_ehvi_set_penalty(tb_ehvi* h, const double* pending_mean, const double* pending_var, int P) {
+  TB_CHECK(h, "tb_ehvi_set_penalty: null handle");
+  TB_CHECK(P >= 0, "tb_ehvi_set_penalty: negative number of pending points");
+  if (P == 0) {
+    h->P = 0;
+    h->hPen.clear();
+    return 0;
+  }
+  TB_CHECK(pending_mean && pending_var, "tb_ehvi_set_penalty: null argument");
+  const size_t n = (size_t)P * h->L;
+  const bool dev = tb::is_device_ptr(pending_mean) || tb::is_device_ptr(pending_var);
+  std::vector<double> in;
+  const double *mean = pending_mean, *var = pending_var;
+  if (dev) {  // device arrays are read back: the variances are checked on the host
+    TB_CUDA(cudaSetDevice(h->device));
+    in.resize(2 * n);
+    TB_CUDA(cudaMemcpy(in.data(), pending_mean, sizeof(double) * n, cudaMemcpyDefault));
+    TB_CUDA(cudaMemcpy(in.data() + n, pending_var, sizeof(double) * n, cudaMemcpyDefault));
+    mean = in.data();
+    var = in.data() + n;
+  }
+  // the state the object already holds (the penalised function pushes before every launch): no copy, no synchronise
+  if (h->P == P && std::equal(mean, mean + n, h->hPen.begin()) && std::equal(var, var + n, h->hPen.begin() + n)) return 0;
+  for (size_t i = 0; i < n; ++i)
+    TB_CHECK(var[i] >= 0.0, "tb_ehvi_set_penalty: the pending variances must be non-negative, got " + std::to_string(var[i]));
+  std::vector<double> held(mean, mean + n);
+  held.insert(held.end(), var, var + n);
+  std::vector<double> up(mean, mean + n);
+  for (size_t i = 0; i < n; ++i) up.push_back(std::sqrt(var[i]));
+  TB_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = h->m[0]->stream;
+  h->P = 0;  // a failed upload leaves no penalty
+  h->hPen.clear();
+  TB_TRY(h->dPen.reserve(sizeof(double) * 2 * n));
+  TB_CUDA(cudaMemcpyAsync(h->dPen.p, up.data(), sizeof(double) * 2 * n, cudaMemcpyHostToDevice, st));
+  TB_CUDA(cudaStreamSynchronize(st));
+  h->hPen.swap(held);
+  h->P = P;
   return 0;
 }
 
