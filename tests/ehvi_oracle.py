@@ -61,14 +61,36 @@ def ehvi_factors(mean, var, lower, upper):
     return np.maximum(diff, 0.0) + nu, gm, gs, s
 
 
+def _in_blocks(f, arrays, K, L):
+    """f over row blocks of the [M, ...] arrays, its outputs concatenated: the [M, K, L] intermediates stay near 32 MB
+    each, whatever the cell and candidate counts"""
+    rows = max(1, (1 << 22) // max(1, K * L))
+    M = len(arrays[0])
+    if M <= rows:
+        return f(*arrays)
+    parts = [f(*(a[i:i + rows] for a in arrays)) for i in range(0, M, rows)]
+    if isinstance(parts[0], tuple):
+        return tuple(np.concatenate(p) for p in zip(*parts))
+    return np.concatenate(parts)
+
+
 def ehvi(mean, var, lower, upper):
     """the product-of-sums form: sum_k prod_l g_kl -> [M]"""
-    g = ehvi_factors(mean, var, lower, upper)[0]
-    return np.prod(g, axis=-1).sum(axis=-1)
+    def one(mean, var):
+        return np.prod(ehvi_factors(mean, var, lower, upper)[0], axis=-1).sum(axis=-1)
+
+    return _in_blocks(one, (np.asarray(mean), np.asarray(var)), *np.shape(lower))
 
 
 def ehvi_partials(mean, var, lower, upper, var_clipped=None):
     """d EHVI / d mean and d EHVI / d var, each [M, L]; zero in var where the variance was clipped"""
+    arrays = (np.asarray(mean), np.asarray(var))
+    if var_clipped is not None:
+        arrays += (np.broadcast_to(var_clipped, arrays[0].shape),)
+    return _in_blocks(lambda *a: _partials(*a[:2], lower, upper, *a[2:]), arrays, *np.shape(lower))
+
+
+def _partials(mean, var, lower, upper, var_clipped=None):
     g, gm, gs, s = ehvi_factors(mean, var, lower, upper)
     L = g.shape[-1]
     others = np.stack([np.prod(np.delete(g, l, axis=-1), axis=-1) for l in range(L)], axis=-1)  # [M, K, L]

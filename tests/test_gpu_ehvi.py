@@ -22,6 +22,10 @@ OBJECTIVES = [
     lambda x: o.ackley(x).reshape(-1, 1),
     lambda x: o.random_fourier_objective(x, seed=3),
     lambda x: o.random_fourier_objective(x, seed=5),
+    lambda x: o.random_fourier_objective(x, seed=7),
+    lambda x: o.random_fourier_objective(x, seed=11),
+    lambda x: o.random_fourier_objective(x, seed=13),
+    lambda x: o.random_fourier_objective(x, seed=17),
 ]
 
 
@@ -37,7 +41,9 @@ def _cells(oms):
     from trieste_b200.acquisition.multi_objective import (Pareto, get_reference_point,
                                                           prepare_default_non_dominated_partition_bounds)
 
-    Y = np.concatenate([om.y.reshape(-1, 1) for om in oms], axis=1)[:40]  # a front of tens to hundreds of cells
+    # a front of tens to hundreds of cells; from five objectives on the cell count grows steeply with the front, so four
+    # points give a few hundred to a few thousand
+    Y = np.concatenate([om.y.reshape(-1, 1) for om in oms], axis=1)[:40 if len(oms) <= 4 else 4]
     front = Pareto(Y).front
     return prepare_default_non_dominated_partition_bounds(get_reference_point(front), front)
 
@@ -53,8 +59,12 @@ def _allowance(oms, engines, mean, var, lower, upper):
     return 1e-14 + 10.0 * np.abs(dvar) @ eps
 
 
+MIXED8 = ["int8", "fp64", "int8x21"] * 2 + ["int8", "fp64"]
 CASES = [["int8"] * 2, ["int8x21"] * 2, ["fp64"] * 2, ["int8"] * 3, ["int8x21"] * 3, ["fp64"] * 3, ["int8"] * 4,
-         ["fp64"] * 4, ["int8", "fp64", "int8x21"]]
+         ["fp64"] * 4, ["int8", "fp64", "int8x21"], ["int8"] * 5, ["fp64"] * 6, ["int8x21"] * 7, ["int8"] * 8, ["fp64"] * 8,
+         MIXED8]
+# one stack per objective count from five to eight, for the paths that run every kernel instantiation
+WIDE = [["int8"] * 5, ["fp64"] * 6, ["int8x21"] * 7, MIXED8]
 
 
 @pytest.mark.parametrize("engines", CASES, ids=["-".join(c) for c in CASES])
@@ -79,7 +89,7 @@ def test_values_match_oracle(engines):
     assert np.any(ref > 0)
 
 
-@pytest.mark.parametrize("engines", [["int8"] * 2, ["fp64"] * 3, ["int8x21"] * 4, ["int8", "fp64", "int8x21"]],
+@pytest.mark.parametrize("engines", [["int8"] * 2, ["fp64"] * 3, ["int8x21"] * 4, ["int8", "fp64", "int8x21"]] + WIDE,
                          ids=lambda c: "-".join(c))
 def test_gradient_matches_oracle(engines):
     from trieste_b200.acquisition import expected_hv_improvement
@@ -96,7 +106,7 @@ def test_gradient_matches_oracle(engines):
     np.testing.assert_allclose(grad[:, 0, :], ref, rtol=1e-6, atol=1e-7 * scale)
 
 
-@pytest.mark.parametrize("engines", [["int8"] * 2, ["fp64"] * 3], ids=lambda c: "-".join(c))
+@pytest.mark.parametrize("engines", [["int8"] * 2, ["fp64"] * 3, ["int8"] * 5, MIXED8], ids=lambda c: "-".join(c))
 @pytest.mark.parametrize("device_arrays", [False, True])
 def test_fused_argmax_is_first_max_of_values(engines, device_arrays):
     from trieste_b200.acquisition import expected_hv_improvement
@@ -124,7 +134,7 @@ def test_fused_argmax_is_first_max_of_values(engines, device_arrays):
     assert best == vals[idx]
 
 
-@pytest.mark.parametrize("engines", [["int8"] * 2, ["fp64"] * 3], ids=lambda c: "-".join(c))
+@pytest.mark.parametrize("engines", [["int8"] * 2, ["fp64"] * 3, ["int8"] * 5, MIXED8], ids=lambda c: "-".join(c))
 def test_device_lbfgs_reaches_scipy_values(engines):
     from trieste_b200.acquisition import expected_hv_improvement
 

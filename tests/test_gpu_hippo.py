@@ -14,7 +14,7 @@ import pytest
 from oracle import gp_oracle as o
 from tests import ehvi_oracle as eo
 from tests import hippo_oracle as ho
-from tests.test_gpu_ehvi import ENGINE_VAR_EPS, _cells, _kernel_count, _oracle_moments, _stack
+from tests.test_gpu_ehvi import ENGINE_VAR_EPS, MIXED8, WIDE, _cells, _kernel_count, _oracle_moments, _stack
 from tests.util import candidates
 
 pytestmark = pytest.mark.gpu
@@ -22,6 +22,8 @@ pytestmark = pytest.mark.gpu
 CASES = [["int8"] * 2, ["int8x21"] * 2, ["fp64"] * 2, ["int8"] * 3, ["int8x21"] * 3, ["fp64"] * 3, ["int8"] * 4,
          ["fp64"] * 4, ["int8", "fp64", "int8x21"]]
 TILE = 64  # pending points per shared-memory tile of the kernel
+# five to eight objectives, with one pending point and with more than a tile of them
+WIDE_CASES = [(e, P) for e in WIDE + [["int8"] * 8] for P in (1, TILE + 6)]
 
 
 def _penalised(stack, lower, upper, P, seed=7):
@@ -39,8 +41,9 @@ def _allowance(oms, engines, mean, var, lower, upper, pmean, pvar):
     return 1e-14 + 10.0 * (np.abs(dvar) @ veps + np.abs(dmu) @ meps)
 
 
-@pytest.mark.parametrize("P", [1, 4, TILE + 6])
-@pytest.mark.parametrize("engines", CASES, ids=["-".join(c) for c in CASES])
+@pytest.mark.parametrize("engines, P", [(e, P) for P in (1, 4, TILE + 6) for e in CASES] + WIDE_CASES,
+                         ids=[f"{'-'.join(e)}-{P}" for P in (1, 4, TILE + 6) for e in CASES] +
+                             [f"{'-'.join(e)}-{P}" for e, P in WIDE_CASES])
 def test_values_match_oracle(engines, P):
     oms, nms, stack = _stack(engines)
     lower, upper = _cells(oms)
@@ -62,9 +65,11 @@ def test_values_match_oracle(engines, P):
     assert np.all(got <= base(X[:, None, :])[:, 0])  # the penalty is at most 1
 
 
-@pytest.mark.parametrize("engines", [["int8"] * 2, ["fp64"] * 3, ["int8x21"] * 4, ["int8", "fp64", "int8x21"]],
-                         ids=lambda c: "-".join(c))
-@pytest.mark.parametrize("P", [1, 5, TILE + 6])
+GRAD_CASES = [(e, P) for e in [["int8"] * 2, ["fp64"] * 3, ["int8x21"] * 4, ["int8", "fp64", "int8x21"]]
+              for P in (1, 5, TILE + 6)] + WIDE_CASES
+
+
+@pytest.mark.parametrize("engines, P", GRAD_CASES, ids=[f"{P}-{'-'.join(e)}" for e, P in GRAD_CASES])
 def test_gradient_matches_oracle(engines, P):
     oms, nms, stack = _stack(engines)
     lower, upper = _cells(oms)

@@ -34,8 +34,10 @@ class _TwoOutputs:
 
 
 def _cells(L, seed):
+    """the partition of a random front: six points up to four objectives, four from five on (hundreds to thousands of
+    cells)"""
     rng = np.random.default_rng(seed)
-    front = Pareto(rng.uniform(0.0, 1.0, size=(6, L))).front
+    front = Pareto(rng.uniform(0.0, 1.0, size=(6 if L <= 4 else 4, L))).front
     return prepare_default_non_dominated_partition_bounds(get_reference_point(front), front)
 
 
@@ -44,7 +46,7 @@ def _moments(M, L, seed):
     return rng.uniform(-0.5, 1.5, size=(M, L)), rng.uniform(0.01, 0.5, size=(M, L))
 
 
-@pytest.mark.parametrize("L, P", [(2, 1), (2, 4), (3, 3), (4, 7)])
+@pytest.mark.parametrize("L, P", [(2, 1), (2, 4), (3, 3), (4, 7), (5, 2), (6, 5), (7, 1), (8, 9)])
 def test_penalty_partials_match_central_differences(L, P):
     mean, _ = _moments(60, L, L + P)
     pmean, pvar = _moments(P, L, 100 + P)
@@ -59,7 +61,7 @@ def test_penalty_partials_match_central_differences(L, P):
     assert ho.penalty(mean[:1], pmean, pvar)[0] > 0
 
 
-@pytest.mark.parametrize("L, P", [(2, 1), (3, 2), (4, 5)])
+@pytest.mark.parametrize("L, P", [(2, 1), (3, 2), (4, 5), (5, 3), (6, 1), (7, 2), (8, 4)])
 def test_penalised_partials_match_central_differences(L, P):
     lower, upper = _cells(L, L)
     mean, var = _moments(50, L, 3 + L)
@@ -140,7 +142,7 @@ def test_penaliser_call_matches_the_oracle_with_several_outputs():
     np.testing.assert_allclose(hp(x)[:, 0], ho.penalty(model.predict(x[:, 0])[0], pmean[:2], pvar[:2]), rtol=1e-14)
 
 
-@pytest.mark.parametrize("L", [2, 3])
+@pytest.mark.parametrize("L", [2, 3, 5, 8])
 def test_product_agrees_with_the_reference_log_form(L):
     lower, upper = _cells(L, 9)
     mean, var = _moments(200, L, 2)

@@ -36,10 +36,6 @@ def _dominated_volume_brute(front, ref):
     return total
 
 
-def _overlap(lo1, up1, lo2, up2):
-    return np.prod(np.clip(np.minimum(up1, up2) - np.maximum(lo1, lo2), 0.0, None))
-
-
 def test_pareto_and_reference_point_errors():
     with pytest.raises(ValueError):
         Pareto(np.zeros((3,)))
@@ -63,7 +59,8 @@ def test_reference_point_is_worst_front_point_plus_twice_range_over_size():
 
 
 # ---- partitions ----
-@pytest.mark.parametrize("L, n", [(2, 7), (3, 6), (4, 5)])
+# from five objectives on, fronts of 3-5 points keep the cell count in the hundreds to thousands
+@pytest.mark.parametrize("L, n", [(2, 7), (3, 6), (4, 5), (5, 5), (6, 4), (7, 4), (8, 3)])
 @pytest.mark.parametrize("seed", [0, 1])
 def test_partition_cells_are_disjoint_and_complete(L, n, seed):
     front = _front(n, L, seed)
@@ -71,9 +68,9 @@ def test_partition_cells_are_disjoint_and_complete(L, n, seed):
     anti = front.min(0) - 0.7
     lower, upper = prepare_default_non_dominated_partition_bounds(ref, front, anti)
     assert np.all(lower <= upper)
-    for i in range(len(lower)):
-        for j in range(i + 1, len(lower)):
-            assert _overlap(lower[i], upper[i], lower[j], upper[j]) < 1e-12
+    for i in range(len(lower) - 1):  # cell i against every later cell
+        ext = np.minimum(upper[i], upper[i + 1:]) - np.maximum(lower[i], lower[i + 1:])
+        assert np.all(np.prod(np.clip(ext, 0.0, None), axis=1) < 1e-12), i
     cells = np.sum(np.prod(upper - lower, axis=1))
     dominated = _dominated_volume_brute(front, ref)
     assert cells + dominated == pytest.approx(np.prod(ref - anti), rel=1e-12)
@@ -82,7 +79,7 @@ def test_partition_cells_are_disjoint_and_complete(L, n, seed):
         assert not np.any(np.all(front <= lo + 1e-12, axis=1) & np.all(lo + 1e-12 < ref))
 
 
-@pytest.mark.parametrize("L, n", [(2, 6), (3, 6), (4, 5)])
+@pytest.mark.parametrize("L, n", [(2, 6), (3, 6), (4, 5), (5, 5), (6, 4), (7, 4), (8, 4)])
 def test_hypervolume_indicator_matches_inclusion_exclusion(L, n):
     front = _front(n, L, 3)
     ref = front.max(0) + 0.2
@@ -125,19 +122,20 @@ def _moments(M, L, seed, scale=1.0):
     return rng.uniform(-0.5, 1.5, size=(M, L)), scale * rng.uniform(0.01, 0.5, size=(M, L))
 
 
-@pytest.mark.parametrize("L", [2, 3, 4])
+@pytest.mark.parametrize("L", [2, 3, 4, 5, 6, 7, 8])
 def test_oracle_product_of_sums_equals_literal_form(L):
-    front = _front(6, L, 5)
+    # the literal form costs 2^L products per cell: from five objectives on, fronts of four points and fewer candidates
+    front = _front(6 if L <= 4 else 4, L, 5)
     lower, upper = prepare_default_non_dominated_partition_bounds(get_reference_point(front), front)
-    mean, var = _moments(200, L, L)
+    mean, var = _moments(200 if L <= 4 else 48 if L <= 6 else 8, L, L)
     lit, pos = eo.ehvi_literal(mean, var, lower, upper), eo.ehvi(mean, var, lower, upper)
     np.testing.assert_allclose(pos, lit, rtol=1e-13, atol=1e-300)
     assert np.all(pos > 0)
 
 
-@pytest.mark.parametrize("L", [2, 3, 4])
+@pytest.mark.parametrize("L", [2, 3, 4, 5, 6, 7, 8])
 def test_oracle_partials_match_central_differences(L):
-    front = _front(5, L, 7)
+    front = _front(5 if L <= 5 else 4, L, 7)
     lower, upper = prepare_default_non_dominated_partition_bounds(get_reference_point(front), front)
     mean, var = _moments(50, L, 11)
     dmu, dvar = eo.ehvi_partials(mean, var, lower, upper)
