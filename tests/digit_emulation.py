@@ -1,4 +1,4 @@
-"""CPU emulation of the single-pass digit engine (trieste_b200/csrc/ozaki5.cuh, ozaki.cuh, int8_engines.cu) — TEST INFRASTRUCTURE.
+"""CPU emulation of the int8 digit engine (trieste_b200/csrc/ozaki5.cuh, ozaki.cuh, int8_engines.cu) — TEST INFRASTRUCTURE.
 
 The int8 tensor-core engine evaluates the fp64 product ``A = Linv · K*`` as exact integer digit GEMMs.  Everything it does is
 integer arithmetic on balanced base-256 digits plus a handful of fp64 operations in the epilogue, so NumPy can replay it

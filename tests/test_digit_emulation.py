@@ -29,7 +29,7 @@ def _model(kind, N, D, noise_frac, seed=0):
 
 def test_balanced_digits_are_exact_and_match_the_byte_trick():
     rng = np.random.default_rng(0)
-    for S in (3, 4, 5):
+    for S in (3, 4, 5, 6):
         lim = int(0.498 * 2 ** (8 * S))
         v = rng.integers(-lim, lim, size=5000)
         d = de.balanced_digits(v, S)
@@ -61,9 +61,9 @@ def test_fifteen_products_meet_the_bar_and_the_estimate_covers_them(kind):
     assert mx < BAR / 3, (kind, mx)
     assert est <= 3e-10, (kind, est)  # the mode is admitted for the default noise level ...
     assert mx <= 3.0 * est and est <= 100.0 * mx, (kind, mx, est)  # ... by an estimate of the right size
-    # 21 products of round 1 (6 digits, p + q <= 7, power-of-two scales with two spare bits, uncentred K*): two orders tighter
-    mx21, _, n21 = de.variance_error(Linv, Ks, var, SA=6, SB=6, R=7, tight=False, centre=False)
-    assert n21 == 21 and mx21 < mx / 10
+    # the 21 products of the six-digit mode (the same tight scales and centred K*, pairs p + q <= 7): two orders tighter
+    mx21, _, n21 = de.variance_error(Linv, Ks, var, SA=6, SB=6, R=7)
+    assert n21 == 21 and mx21 < mx / 100
 
 
 def test_what_tight_scales_and_the_centred_kstar_buy():
@@ -80,7 +80,7 @@ def test_what_tight_scales_and_the_centred_kstar_buy():
 
 def test_low_noise_model_is_refused_by_the_estimate():
     # an RBF model with noise σ_f²/1e5 has rows of Linv up to ~300/σ_f: the 15-product error approaches the bar and the
-    # a-priori estimate (which only sees the row scales) must keep such a handle on the 21-product kernels
+    # a-priori estimate (which only sees the row scales) must keep such a handle on 6 digits (21 products)
     N = 400
     Linv, Ks, var = _model("rbf", N, 6, 1e-5)
     est = de.apriori_estimate(var, de.tight_row_scales(Linv)[0].max(), N, 5)

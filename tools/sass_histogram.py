@@ -12,7 +12,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "trieste_b200", "libtrieste_b200.so")
-WANT = ["dg::digit_gemm_kernel", "oz5::kstar_digits_kernel<3, 10, 5>", "oz::kstar_digits_kernel<3, 10>", "tb::trigemm_kernel<false, 0>",
+WANT = ["dg::digit_gemm_kernel", "oz5::kstar_digits_kernel<3, 10, 5>", "oz5::kstar_digits_kernel<3, 10, 6>", "tb::trigemm_kernel<false, 0>",
         "tb::tail_kernel", "tc_mean_bounds_kernel<3, 10>", "rff_eval_kernel<6, 8>", "joint_kernel<3, 1>", "lbfgs_step_kernel", "kdot_kernel<3, 6, 4>", "grad_kernel<3, 10, 1>", "grad_kernel<3, 10, 8>",
         "fac::chol_syrk_kernel", "fac::kinv_kernel"]
 KEY = ["IGMMA", "HGMMA", "UBLKCP", "UTMALDG", "SYNCS", "DMMA", "HMMA", "IMMA", "DFMA", "DADD", "DMUL", "MUFU", "F2F", "I2F", "F2I",

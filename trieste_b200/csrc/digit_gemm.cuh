@@ -1,4 +1,4 @@
-// The digit GEMM shared by the INT8 engines (ozaki.cuh: 6 digits, ozaki5.cuh: 3 - 5 digits), on Hopper warpgroup MMA.
+// The digit GEMM of the INT8 engine (ozaki.cuh, ozaki5.cuh: 3 - 6 digits), on Hopper warpgroup MMA.
 //
 // Operands are int8 digit planes pre-packed in the no-swizzle K-major core-matrix layout (8 rows x 16 bytes per core matrix,
 // K-adjacent core matrices LBO apart, 8-row groups SBO apart), so one pipeline stage is a handful of contiguous 1-D bulk-TMA

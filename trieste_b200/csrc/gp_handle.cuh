@@ -56,23 +56,24 @@ struct DevBuf {
 // two are equal.
 constexpr uint64_t STALE = ~(uint64_t)0;
 
-// One left operand of the digit GEMM (Linv or the dense K^-1): digit planes in the GEMM's stage layout, per-row scales, and
-// per-row sums (the single-pass engine's centring term; empty for the 21-product engine).
+// One left operand of the digit GEMM (Linv or the dense K^-1): per-row scales and per-row sums (the centring term), and digit
+// planes cut against them in the GEMM's stage layout at two plane counts: the admitted split's (4 or 5) and 6.
 struct DigitOperand {
-  DevBuf digits, scale, sum;
-  int planes = 0;        // digit planes stored per stage; 0: the single-pass engine was not admitted for this operand
-  uint64_t gen = STALE;  // cache_gen the operand was built from
+  DevBuf scale, sum, digits, digits6;
+  int planes = 0;         // planes of `digits`; 0: the a-priori estimate refused the operand
+  uint64_t gen = STALE;   // cache_gen the row stats, the admission and `digits` were built from
+  uint64_t gen6 = STALE;  // cache_gen `digits6` was cut from
 };
 
-// The int8 engines' state (int8_engines.cu owns it): both engines' Linv and K^-1 operands stay alive together, so one handle
-// can run single-pass values and 21-product gradients when the V estimate refuses the single-pass split.
+// The int8 engine's state (int8_engines.cu owns it).  Both cuts of Linv and of K^-1 stay alive together, so one handle can run
+// values at 5 digits and gradients at 6 when the V estimate refuses 5.
 struct DigitState {
-  DigitOperand linv21, kinv21;  // 21-product engine: 6 planes, power-of-two row scales
-  DigitOperand linv, kinv;      // single-pass engine: tight row scales and row sums; linv.gen also stamps the admission below
-  DevBuf X2;                    // squared row norms of the scaled training inputs (centred K* generation)
-  bool full = false;            // tb_gp_set_engine(2): always the 21-product engine
-  int mode = 0;                 // digits the single-pass variance GEMM computes with (0: not admitted)
-  double est = 0.0;             // a-priori estimate of max |Δvar| / σ_f² in that mode
+  DigitOperand linv, kinv;  // linv.gen also stamps the admission below
+  DevBuf X2;                // squared row norms of the scaled training inputs (centred K* generation)
+  bool full = false;        // tb_gp_set_engine(2): always 6 digits
+  int mode = 0;             // digits the variance GEMM computes with on the admitted split (0: not admitted)
+  double est = 0.0;         // a-priori estimate of max |Δvar| / σ_f² in that mode
+  int S = 0;                // digit planes of the K* tiles and left operands of the current call (int8_select)
 };
 
 inline bool is_device_ptr(const void* p) {
@@ -192,11 +193,11 @@ struct tb_gp {
   tb::DevBuf dLinvTP;           // packed upper panels of Linv^T (lazy; gradient path)
   uint64_t upper_gen = tb::STALE;
   int engine = 1;  // 0 = fp64 DMMA, 1 = int8 tensor cores (default; same stated tolerances, ~3x faster)
-  // dense K^-1 (lower triangle, ld = N) of the int8 engines' gradient path: an append grows it by rank m (tb_gp_append_data)
+  // dense K^-1 (lower triangle, ld = N) of the int8 engine's gradient path: an append grows it by rank m (tb_gp_append_data)
   // instead of rebuilding it in O(N^3)
   tb::DevBuf dKinv, dKinvSpare;
   uint64_t kinv_gen = tb::STALE;
-  tb::DigitState digits;       // the int8 engines' digit operands (int8_engines.cu)
+  tb::DigitState digits;       // the int8 engine's digit operands (int8_engines.cu)
   tb::DevBuf sMeanPart;        // per-split mean partials of the k-split K* generation (few candidate tiles)
   tb::DevBuf dWork, dInfo;      // cusolver workspace / info flag
   tb::DevBuf dDinv;             // inverses of the diagonal blocks of L (hand-written factorisation)

@@ -1,17 +1,20 @@
-// Single-pass digit GEMM of the INT8 engine: fewer digit products, one pass.
+// The int8 digit engine: centred K* generation and the digit count of a call.
 //
-// Same error-free splitting and digit cutters as ozaki.cuh, re-budgeted against the 1e-9·σ_f² variance bar:
-//   * operands are scaled TIGHTLY (|x̂| <= 0.4975, arbitrary fp64 scale per row of Linv instead of a power of two with two
-//     spare bits) and K* is CENTRED: K* = h + K̃ with h = σ_f²/2, |K̃| <= h, so the sign bit of the top digit carries
-//     information;  A = Linv·K̃ + h·rowsum(Linv), the second term is a per-row constant added in the epilogue;
-//   * with those 3-4 extra bits, S = 5 balanced base-256 digits and the pairs p + q <= S + 1 (15 products instead of 21)
-//     keep max |Δvar| at ~1e-10·σ_f² (emulated; the host picks this mode from an a-priori bound computed from the row scales
-//     and falls back to the 6-digit / 21-product kernel otherwise);
-//   * all S levels r = 2..S+1 are accumulated at once: ONE pass per row-block and column chunk, one epilogue;
-//   * fp32 models use S = 3 (6 products): ~5e-6·σ_f² against the 1e-4·σ_f² fp32 bar.
+// Operands are cut by ozaki.cuh's digit cutters against TIGHT scales (|x̂| <= 0.4975, an arbitrary fp64 scale per row of Linv),
+// and K* is CENTRED: K* = h + K̃ with h = σ_f²/2, |K̃| <= h, so the sign bit of the top digit carries information;
+// A = Linv·K̃ + h·rowsum(Linv), the second term is a per-row constant added in the epilogue.  With S balanced base-256 digits
+// the pairs p + q <= S + 1 are kept, and all S levels r = 2..S+1 are accumulated at once: ONE pass per row-block and column
+// chunk, one epilogue.  The host (int8_engines.cu) picks S from an a-priori bound computed from the row scales:
+//   * S = 5 (15 products) keeps max |Δvar| at ~1e-10·σ_f² (emulated) on fp64 handles;
+//   * fp32 models compute with S = 3 or 4 leading planes of a 4-digit split (6 / 10 products): ~5e-6·σ_f² against the
+//     1e-4·σ_f² fp32 bar;
+//   * handles the bound refuses (and tb_gp_set_engine(2)) run S = 6 (21 products; fp32 handles compute with its 4 leading
+//     planes).
 // The K* digit tiles are NT candidates wide (192 for S = 5, 128 otherwise); the GEMM (digit_gemm.cuh) works on them in
-// column chunks of 64 candidates, whose S levels of int32 accumulators fit the registers of two consumer warpgroups.
+// column chunks of 64 candidates (32 for S = 6), whose S levels of int32 accumulators fit the registers of two consumer
+// warpgroups.
 #pragma once
+#include "kernel_fn.cuh"
 #include "ozaki.cuh"
 
 namespace tb {
@@ -24,7 +27,9 @@ using oz::LBO;
 using oz::SBO;
 using oz::two_pow_8S;
 
-template <int S> __host__ __device__ constexpr double dig_koff() { return S == 5 ? 551911719040.0 : S == 4 ? 2155905152.0 : 8421504.0; }  // 0x8080808080 / 0x80808080 / 0x808080
+template <int S> __host__ __device__ constexpr double dig_koff() {  // 0x808080808080 / 0x8080808080 / 0x80808080 / 0x808080
+  return S == 6 ? 141289400074368.0 : S == 5 ? 551911719040.0 : S == 4 ? 2155905152.0 : 8421504.0;
+}
 
 // X2[k] = |Xs[k]|^2 for the rows that exist (Xs is [rows_have][DP], zero padded), 0 beyond
 __global__ void row_norms_kernel(const double* __restrict__ Xs, int64_t rows_have, int DP, int64_t rows, double* __restrict__ X2) {
@@ -47,9 +52,10 @@ __global__ void row_norms_kernel(const double* __restrict__ Xs, int64_t rows_hav
 // that the k-stages can be split far finer than the mean's chain allows, and mean_replay_kernel rebuilds the chain of any split.
 // ------------------------------------------------------------------------------------------------
 constexpr int KGEN_WARPS = 8;
-// (KVAL launches are a few CTAs per SM at most: 128 registers, 255 for D > 12; no spills)
+// S <= 5: 64 registers / 32 warps per SM (80 / 24 for D > 12).  S = 6 spills at 64 and 80 registers: 128, 255 for D > 10,
+// and no spills.  KVAL launches are a few CTAs per SM at most: 128 registers, 255 for D > 12; no spills.
 template <int KIND, int DP, int S, bool KVAL = false>
-__global__ void __launch_bounds__(KGEN_WARPS * 32, KVAL ? (DP <= 12 ? 2 : 1) : DP <= 12 ? 4 : 3)  // 64 registers / 32 warps per SM (80 / 24 for D > 12: no spills)
+__global__ void __launch_bounds__(KGEN_WARPS * 32, KVAL ? (DP <= 12 ? 2 : 1) : S == 6 ? (DP <= 10 ? 2 : 1) : DP <= 12 ? 4 : 3)
 kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2, const double* __restrict__ alpha,
                     const double* __restrict__ Xc, const double* __restrict__ inv_ls, int N, int nst, int D, int64_t M, double variance,
                     double inv_bscale_2p, double dig_c, double mean_const, const __grid_constant__ fm::Consts fc, int ntiles,
@@ -163,7 +169,7 @@ kstar_digits_kernel(const double* __restrict__ Xs, const double* __restrict__ X2
         macc = fma(kval, al_s[buf][kv], macc);
       }
       const double tb = fma(kval, inv_bscale_2p, dig_c);
-      const uint32_t wl = (uint32_t)__double2loint(tb) ^ 0x80808080u, wh = (uint32_t)__double2hiint(tb) ^ 0x80u;
+      const uint32_t wl = (uint32_t)__double2loint(tb) ^ 0x80808080u, wh = (uint32_t)__double2hiint(tb) ^ (S == 6 ? 0x8080u : 0x80u);
       oz::scatter_rt<S>(pk, j, wl, wh);
     }
     if (tile_id < ntiles) {

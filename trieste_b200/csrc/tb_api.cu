@@ -224,8 +224,8 @@ __global__ void colmajor_lower_to_rowmajor_kernel(const double* __restrict__ A, 
 // =================================================================================================
 // dtype bridge.  TB_F32 handles (fp32 models, e.g. BASELINE config 5) take and return float arrays: whole inputs are widened
 // to device doubles and outputs narrowed back.  Their posterior cache is fp64.  select_engine runs their candidate GEMMs on
-// the int8 engines with fewer digits than an fp64 handle gets: the single-pass engine with the fewest digits int8_select
-// admits (3 digits / 6 products, 4 / 10 or 5 / 15), else the 4 leading planes (10 products) of the 21-product engine.
+// the int8 engine with fewer digits than an fp64 handle gets: the fewest digits int8_select admits (3 digits / 6 products,
+// 4 / 10 or 5 / 15), else the 4 leading planes (10 products) of the 6-digit split.
 // Above N = 16384 and on engine 0 they run the fp64 DMMA kernels, as fp64 handles do.
 // =================================================================================================
 __global__ void widen_kernel(const float* __restrict__ in, int64_t n, double* __restrict__ out) {
@@ -914,7 +914,7 @@ static int launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const 
   return 0;
 }
 
-// The dense K^-1 whose digit tiles the int8 engines' gradient path multiplies with the K* digits (V = K^-1 K*, one dense digit
+// The dense K^-1 whose digit tiles the int8 engine's gradient path multiplies with the K* digits (V = K^-1 K*, one dense digit
 // GEMM): Linv^T Linv (lower triangle, ld = N), O(N^3) on the DMMA pipe (cuSOLVER potri on the cross-check path), lazily once
 // per full cache refresh; appends grow it in O(m N^2) (finish_cache / fac::kinv_grow_kernel)
 static int ensure_kinv_dense(tb_gp* gp) {
@@ -1174,14 +1174,12 @@ static int launch_mean_bounds(tb_gp* gp, cudaStream_t st, const double* Xc, int6
 // =================================================================================================
 enum class Engine {
   F64,   // native fp64 DMMA kernels (kernels_f64.cuh)
-  OZ21,  // 6-digit int8 engine, 21 digit products (ozaki.cuh, int8_engines.cu)
-  OZ15,  // single-pass int8 engine (ozaki5.cuh, int8_engines.cu): 15 digit products on fp64 handles, 6 or 10 on fp32 ones
+  INT8,  // int8 digit engine (ozaki5.cuh, int8_engines.cu): 15 or 21 digit products on fp64 handles, 6, 10 or 15 on fp32 ones
 };
 
 // The engine of a call, after the lazy builds it needs.  need_v: the call also needs V = K^-1 K* (gradients).  The int8
-// engines' int32 accumulators are exact up to K = N = 16384; larger models and engine 0 run the fp64 kernels.  The
-// single-pass engine runs when its a-priori error estimates admit the handle (int8_select); otherwise the 21-product engine
-// does.
+// engine's int32 accumulators are exact up to K = N = 16384; larger models and engine 0 run the fp64 kernels.  The int8
+// engine's digit count (gp->digits.S) comes from its a-priori error estimates (int8_select).
 static int select_engine(tb_gp* gp, bool need_v, Engine* eng) {
   if (!(gp->engine == 1 && gp->N <= 16384)) {
     if (need_v) TB_TRY(ensure_upper_panels(gp));
@@ -1189,19 +1187,18 @@ static int select_engine(tb_gp* gp, bool need_v, Engine* eng) {
     return 0;
   }
   if (need_v) TB_TRY(ensure_kinv_dense(gp));
-  bool single_pass;
-  TB_TRY(int8_select(gp, need_v, &single_pass));
-  *eng = single_pass ? Engine::OZ15 : Engine::OZ21;
+  TB_TRY(int8_select(gp, need_v));
+  *eng = Engine::INT8;
   return 0;
 }
 
 // candidates per K* tile, and the K* scratch bytes per tile
-static int eng_tile_width(const tb_gp* gp, Engine e) { return e == Engine::F64 ? BT : int8_tile_width(gp, e == Engine::OZ15); }
+static int eng_tile_width(const tb_gp* gp, Engine e) { return e == Engine::F64 ? BT : int8_tile_width(gp); }
 static size_t eng_tile_bytes(const tb_gp* gp, Engine e) {
-  return e == Engine::F64 ? (size_t)gp->nkc * PANEL * sizeof(double) : int8_tile_bytes(gp, e == Engine::OZ15);
+  return e == Engine::F64 ? (size_t)gp->nkc * PANEL * sizeof(double) : int8_tile_bytes(gp);
 }
 
-// Row-block groups per candidate tile of the Linv GEMMs.  int8 engines: ~4 row-blocks per CTA amortise the CTA prologue
+// Row-block groups per candidate tile of the Linv GEMMs.  int8 engine: ~4 row-blocks per CTA amortise the CTA prologue
 // while the co-resident CTAs share few enough candidate tiles for the K* digits to stay in L2; small batches get more
 // groups (>= 2 items per SM).  fp64 engine: one group from a full wave of tiles on.
 static int eng_groups(const tb_gp* gp, Engine e, int tiles) {
@@ -1211,19 +1208,19 @@ static int eng_groups(const tb_gp* gp, Engine e, int tiles) {
 }
 
 // K* of mc device candidates into gp->sKs (fp64 panels or digit tiles), their posterior means into gp->sMean.
-// split: the int8 engines' k-split (nullptr: the one int8_kstar_split gives for this many tiles); wide: int8_kstar's
+// split: the int8 engine's k-split (nullptr: the one int8_kstar_split gives for this many tiles); wide: int8_kstar's
 static int eng_kstar(tb_gp* gp, Engine e, const double* xc, int64_t mc, int tiles, const KSplit* split = nullptr, bool wide = false) {
   double* mean = gp->sMean.as<double>();
   if (e == Engine::F64) return launch_kstar(gp, xc, mc, tiles, gp->sKs.as<double>(), mean);
-  return int8_kstar(gp, e == Engine::OZ15, xc, mc, tiles, gp->sKs.as<int8_t>(), mean, split, wide);
+  return int8_kstar(gp, xc, mc, tiles, gp->sKs.as<int8_t>(), mean, split, wide);
 }
 
 // Variance GEMM: sums of squares of A = Linv K* over G row-block groups into gp->sPartial.  fp64 engine with packed_a: A
-// also goes to gp->sA as packed panels, the operand of its V GEMM.  kper > 0 (int8 engines): split-K (int8_split_kper).
+// also goes to gp->sA as packed panels, the operand of its V GEMM.  kper > 0 (int8 engine): split-K (int8_split_kper).
 static int eng_variance(tb_gp* gp, Engine e, int tiles, int G, int64_t McPad, bool packed_a, int kper = 0) {
   cudaStream_t st = gp->stream;
   double* partial = gp->sPartial.as<double>();
-  if (e != Engine::F64) return int8_variance(gp, e == Engine::OZ15, gp->sKs.as<int8_t>(), tiles, G, McPad, partial, kper);
+  if (e != Engine::F64) return int8_variance(gp, gp->sKs.as<int8_t>(), tiles, G, McPad, partial, kper);
   if (packed_a)
     trigemm_kernel<false, EPI_SUMSQ_PACKED><<<dim3(tiles, G), TG_THREADS, TG_SMEM, st>>>(
         gp->dLinvP.as<double>(), gp->sKs.as<double>(), gp->NB, gp->nkc, G, McPad, partial, gp->sA.as<double>(), nullptr, 0);
@@ -1239,7 +1236,7 @@ static int eng_variance(tb_gp* gp, Engine e, int tiles, int G, int64_t McPad, bo
 static int eng_store_a(tb_gp* gp, Engine e, int tiles, int64_t McPad, double* out) {
   const int64_t lda = (int64_t)gp->NB * BM;
   const int G = eng_groups(gp, e, tiles);
-  if (e != Engine::F64) return int8_store(gp, e == Engine::OZ15, false, gp->sKs.as<int8_t>(), tiles, G, McPad, out, lda);
+  if (e != Engine::F64) return int8_store(gp, false, gp->sKs.as<int8_t>(), tiles, G, McPad, out, lda);
   trigemm_kernel<false, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, gp->stream>>>(gp->dLinvP.as<double>(), gp->sKs.as<double>(),
                                                                                         gp->NB, gp->nkc, G, McPad, nullptr, nullptr, out, lda);
   TB_LAUNCHED();
@@ -1248,17 +1245,17 @@ static int eng_store_a(tb_gp* gp, Engine e, int tiles, int64_t McPad, double* ou
 }
 
 // V = K^-1 K* stored plain into gp->sV ([candidate][NB*128]).  fp64 engine: Linv^T A over the packed A that eng_variance left
-// in gp->sA; int8 engines: the digit tiles of the dense K^-1 times the same K* digits.  The 21-product engine's V GEMM has
-// its own row-block groups: at most ~8 row-blocks each.
+// in gp->sA; int8 engine: the digit tiles of the dense K^-1 times the same K* digits.  With 6 digits the V GEMM has its own
+// row-block groups: at most ~8 row-blocks each.
 static int eng_store_v(tb_gp* gp, Engine e, int tiles, int64_t McPad) {
   const int64_t ldv = (int64_t)gp->NB * BM;
   double* V = gp->sV.as<double>();
-  if (e == Engine::OZ21) {
-    const int G = std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)));
-    return int8_store(gp, false, true, gp->sKs.as<int8_t>(), tiles, G, McPad, V, ldv);
+  if (e == Engine::INT8) {
+    const int G = gp->digits.S == 6 ? std::max(1, std::min(gp->NB, std::max((gp->NB + 7) / 8, (2 * NUM_SMS + tiles - 1) / tiles)))
+                                    : eng_groups(gp, e, tiles);
+    return int8_store(gp, true, gp->sKs.as<int8_t>(), tiles, G, McPad, V, ldv);
   }
   const int G = eng_groups(gp, e, tiles);
-  if (e == Engine::OZ15) return int8_store(gp, true, true, gp->sKs.as<int8_t>(), tiles, G, McPad, V, ldv);
   trigemm_kernel<true, EPI_PLAIN><<<dim3(tiles, G), TG_THREADS, TG_SMEM, gp->stream>>>(gp->dLinvTP.as<double>(), gp->sA.as<double>(), gp->NB,
                                                                                        gp->NB * (BM / BK), G, McPad, nullptr, nullptr, V, ldv);
   TB_LAUNCHED();
@@ -1338,7 +1335,7 @@ struct EvalOut {
 // the variance sums of squares (gp->sPartial) and, with grad, V = K^-1 K* (gp->sV).  Gfix: the call's row-block groups (0:
 // eng_groups of this chunk); *G and *McPad return the groups and the candidates padded to whole tiles, the layout of
 // gp->sPartial.  The screened argmax passes the k-split of the chunk its candidates come from, and spread: when they are too
-// few tiles for the row-block groups to fill the SMs, the int8 engines spread them wider (split-K variance GEMM, wide K*
+// few tiles for the row-block groups to fill the SMs, the int8 engine spreads them wider (split-K variance GEMM, wide K*
 // generation) with the same results.
 static int member_step(tb_gp* gp, Engine e, const double* xc, int64_t n, int Gfix, bool grad, int* G, int64_t* McPad,
                        const KSplit* split = nullptr, bool spread = false) {
@@ -1346,7 +1343,7 @@ static int member_step(tb_gp* gp, Engine e, const double* xc, int64_t n, int Gfi
   const int tiles = (int)((n + nt - 1) / nt);
   *G = Gfix ? Gfix : eng_groups(gp, e, tiles);
   *McPad = (int64_t)tiles * nt;
-  const int kper = spread && e != Engine::F64 ? int8_split_kper(gp, e == Engine::OZ15, tiles, *G) : 0;
+  const int kper = spread && e != Engine::F64 ? int8_split_kper(gp, tiles, *G) : 0;
   TB_TRY(eng_kstar(gp, e, xc, n, tiles, split, kper > 0));
   TB_TRY(profiled_gemm(gp, (double)*McPad * (double)gp->N * (double)gp->N,
                        [&] { return eng_variance(gp, e, tiles, *G, *McPad, grad, kper); }));
@@ -1404,8 +1401,7 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, Engine e, int64_t c
   unsigned long long* count = reinterpret_cast<unsigned long long*>(probe_v + 2);
   // the unscreened loop's chunks: whole ones over [0, split), the last over [split, M); only the last can have another k-split
   const int64_t split = ((M - 1) / chunk_cap) * chunk_cap;
-  const KSplit ks_full = int8_kstar_split(gp, e == Engine::OZ15, (int)(chunk_cap / nt)),
-               ks_last = int8_kstar_split(gp, e == Engine::OZ15, (int)((M - split + nt - 1) / nt));
+  const KSplit ks_full = int8_kstar_split(gp, (int)(chunk_cap / nt)), ks_last = int8_kstar_split(gp, (int)((M - split + nt - 1) / nt));
   const bool same_split = ks_full.ksplit == ks_last.ksplit && ks_full.kc_per == ks_last.kc_per;
   // 1. bound pass
   const double var_ub = std::fmax(gp->variance, 1e-12);
@@ -1449,13 +1445,13 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, Engine e, int64_t c
 
 // Chunk geometry of a call over the n handles gps with engines eng (one for run_eval, the members for ehvi_run): candidates
 // per chunk (chunk_cap, the smallest of the handles' own) and each handle's row-block groups G[l], fixed for the call when
-// G[l] > 0, else eng_groups of each chunk.  The screened argmax and the k-split of the single-pass engine reproduce these
+// G[l] > 0, else eng_groups of each chunk.  The screened argmax and the k-split of the int8 engine reproduce these
 // chunks, so they must not drift; with one handle chunk_cap is a whole number of its tiles.  A handle's own chunk size:
-//   int8 engines, values: K* digit scratch within 1,280 MB, whole pairs of waves (or one wave), at most 8 waves; G of the
-//                         first chunk for the whole call
-//   single-pass engine, gradients: K* digits or V (NB*128 doubles per candidate), whichever is larger, within 1,280 MB,
-//                         whole waves
-//   fp64 engine, and the 21-product engine's gradients: chunk_tiles
+//   int8 engine, values: K* digit scratch within 1,280 MB, whole pairs of waves (or one wave), at most 8 waves; G of the
+//                        first chunk for the whole call
+//   int8 engine, gradients below 6 digits: K* digits or V (NB*128 doubles per candidate), whichever is larger, within
+//                        1,280 MB, whole waves
+//   fp64 engine, and the int8 engine's gradients at 6 digits: chunk_tiles
 // A handle whose own chunk size is the common one therefore sums each candidate's variance exactly as its tb_gp_predict does;
 // the others agree with it to rounding.
 struct ChunkPlan {
@@ -1475,7 +1471,7 @@ static ChunkPlan plan_chunks(tb_gp* const* gps, const Engine* eng, int n, bool g
       if (max_tiles >= 2 * NUM_SMS) max_tiles = (max_tiles / (2 * NUM_SMS)) * (2 * NUM_SMS);
       else if (max_tiles >= NUM_SMS) max_tiles = NUM_SMS;
       max_tiles = std::min<int64_t>(max_tiles, 8 * NUM_SMS);
-    } else if (e == Engine::OZ15) {
+    } else if (e == Engine::INT8 && gp->digits.S != 6) {
       const size_t v_bytes = (size_t)nt * gp->NB * BM * sizeof(double);
       max_tiles = std::max<int64_t>(1, (int64_t)(budget / std::max(eng_tile_bytes(gp, e), v_bytes)));
       if (max_tiles >= NUM_SMS) max_tiles = (max_tiles / NUM_SMS) * NUM_SMS;

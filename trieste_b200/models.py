@@ -160,7 +160,7 @@ class GaussianProcessRegression:
         if engine not in ("fp64", "int8", "int8x21"):
             raise ValueError(f"engine must be 'fp64', 'int8' or 'int8x21', got {engine!r}")
         # "int8" picks the number of digit products (15 or 21; fp32 models 6 or 10) from the a-priori error estimate of the
-        # cache; "int8x21" pins the full 21-product kernels
+        # cache; "int8x21" pins six digits (21 products)
         _lib.check(_lib.lib().tb_gp_set_engine(self._h, {"fp64": 0, "int8": 1, "int8x21": 2}[engine]))
         self._engine = engine
 
