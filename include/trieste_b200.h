@@ -61,7 +61,14 @@ enum tb_acq {
   TB_ACQ_GIBBON_REPULSION = 8, /* gibbon_repulsion_term.__call__, entropy.py:580-618: w·½(log(yvar − ‖L_B⁻¹c(x)‖²) − log yvar)
                                   over the pending points set by tb_acq_set_gibbon_repulsion; yvar = var + σ²;
                                   needs no min-value samples */
-  TB_ACQ_GIBBON = 9            /* GibbonAcquisition.__call__, entropy.py:435-436: repulsion + quality */
+  TB_ACQ_GIBBON = 9,           /* GibbonAcquisition.__call__, entropy.py:435-436: repulsion + quality */
+  TB_ACQ_FEASIBILITY_BICHON = 10, /* bichon_ranjan_criterion(delta = 1), active_learning.py:227-234: G_1 * sqrt(var),
+                                     t = (param - mean)/sqrt(var); param = the threshold T, alpha set by tb_acq_set_feasibility */
+  TB_ACQ_FEASIBILITY_RANJAN = 11, /* bichon_ranjan_criterion(delta = 2), active_learning.py:235-243: G_2 * var */
+  TB_ACQ_BALD = 12,               /* bayesian_active_learning_by_disagreement.__call__, active_learning.py:498-513:
+                                     h(Phi(mean / sqrt(v + 1))) - E, v = max(var, param); param = the jitter (> 0) */
+  TB_ACQ_PREDICTIVE_VARIANCE = 13 /* predictive_variance at q = 1, active_learning.py:98-108: exp(logdet([[var + param]]))
+                                     = var + param; param = the jitter (q > 1: tb_acq_predictive_variance) */
 };
 /* OR-ed into `acq` of tb_acq_eval / tb_acq_argmax / tb_acq_maximize: the value (and gradient) is multiplied by the local
  * penalty set by tb_acq_set_penalization (PenalizedAcquisition, acquisition/function/greedy_batch.py:250-269). */
@@ -142,6 +149,11 @@ int tb_acq_set_penalization(tb_gp* gp, int kind, const double* pending, int P, c
  * TB_ERR_NUMERIC if B + σ²I is not positive definite. */
 int tb_acq_set_gibbon_repulsion(tb_gp* gp, const double* pending, int m, double weight);
 
+/* ExpectedFeasibility.__init__ (active_learning.py:121-140): the neighbourhood parameter alpha of the two feasibility kinds,
+ * held by the handle for every later TB_ACQ_FEASIBILITY_BICHON / _RANJAN launch (which refuse to run before it is set).
+ * TB_ERR_INVALID for alpha <= 0 or non-finite alpha; the alpha held before then stays. */
+int tb_acq_set_feasibility(tb_gp* gp, double alpha);
+
 /* the posterior mean and its gradient, what LocalPenalization's Lipschitz estimate differentiates
  * (greedy_batch.py:207-217): Xc [M,D] → mean [M] = k(x, X) α + m and grad [M,D] = its derivative in x.  No variance: one
  * kernel launch per 65,536 points, no GEMM.  Handle dtype, host or device pointers. */
@@ -187,6 +199,14 @@ int tb_acq_batch_ei(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w
  * gradient assembly as tb_acq_batch_mc_ei_grad.  out [B], grad [B,q,D]. */
 int tb_acq_batch_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const double* w, int S, double eta, void* out,
                          void* grad);
+
+/* predictive_variance.acquisition (active_learning.py:98-108): exp(logdet(cov + jitter)) of the joint posterior of each
+ * q-batch.  As in the reference the scalar jitter is added to EVERY entry of cov (cov + jitter 1 1^T, not cov + jitter I);
+ * the log-determinant is 2 sum log diag chol.  Xc [B,q,D] → out [B]; grad (nullable) [B,q,D] = d out / d Xc (the reverse
+ * pass with Sigma_bar = det(M) M^-1, M = cov + jitter 1 1^T, assembled as for tb_acq_batch_mc_ei_grad).  Handle dtype,
+ * host or device pointers.  1 <= q <= 32 (the reference has no bound); TB_ERR_NUMERIC if M of a batch is not positive
+ * definite. */
+int tb_acq_predictive_variance(tb_gp* gp, const void* Xc, int64_t B, int q, double jitter, void* out, void* grad);
 
 /* MultivariateNormalCDF.__call__ (acquisition/function/utils.py:109-199): P(X ≤ x) for X ~ N(mean, cov + jitter I) by
  * Genz's recursion over the S Sobol points w [Q−1,S] (column-contiguous; may be null for Q = 1).  x, mean [B,Q],

@@ -19,6 +19,7 @@ TB_F64, TB_F32 = 0, 1
 KERNEL_IDS = {"rbf": 0, "matern12": 1, "matern32": 2, "matern52": 3}
 ACQ_EI, ACQ_LOG_EI, ACQ_NEG_LCB, ACQ_LCB, ACQ_PBT, ACQ_AEI, ACQ_MES = 0, 1, 2, 3, 4, 5, 6
 ACQ_GIBBON_QUALITY, ACQ_GIBBON_REPULSION, ACQ_GIBBON = 7, 8, 9
+ACQ_FEASIBILITY_BICHON, ACQ_FEASIBILITY_RANJAN, ACQ_BALD, ACQ_PREDICTIVE_VARIANCE = 10, 11, 12, 13
 ACQ_PENALIZED = 0x100  # OR-ed into the acquisition kind: multiply by the handle's local penalty
 PEN_SOFT, PEN_HARD = 1, 2
 
@@ -44,12 +45,14 @@ SIGNATURES = {
     "tb_acq_set_min_value_samples": (_i32, [_vp, C.POINTER(_f64), _i32]),
     "tb_acq_set_penalization": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp]),
     "tb_acq_set_gibbon_repulsion": (_i32, [_vp, _vp, _i32, _f64]),
+    "tb_acq_set_feasibility": (_i32, [_vp, _f64]),
     "tb_gp_mean_gradient": (_i32, [_vp, _vp, _i64, _vp, _vp]),
     "tb_acq_maximize": (_i32, [_vp, _i32, _f64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
     "tb_acq_batch_mc_ei": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _f64, _vp]),
     "tb_acq_batch_mc_ei_grad": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _f64, _vp, _vp]),
     "tb_acq_batch_ei": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _vp]),
     "tb_acq_batch_ei_grad": (_i32, [_vp, _vp, _i64, _i32, _vp, _i32, _f64, _vp, _vp]),
+    "tb_acq_predictive_variance": (_i32, [_vp, _vp, _i64, _i32, _f64, _vp, _vp]),
     "tb_mvn_cdf": (_i32, [_i32, _vp, _vp, _vp, _i64, _i32, _vp, _i32, _f64, _vp]),
     "tb_gp_covariance_between_points": (_i32, [_vp, _vp, _i64, _vp, _i64, _vp]),
     "tb_gp_sample_joint": (_i32, [_vp, _vp, _i64, _vp, _i32, _f64, _vp]),

@@ -1,3 +1,11 @@
+from .active_learning import (  # noqa: F401
+    BayesianActiveLearningByDisagreement,
+    ExpectedFeasibility,
+    PredictiveVariance,
+    bayesian_active_learning_by_disagreement,
+    bichon_ranjan_criterion,
+    predictive_variance,
+)
 from .continuous_thompson_sampling import (  # noqa: F401
     GreedyContinuousThompsonSampling,
     ParallelContinuousThompsonSampling,

@@ -216,6 +216,7 @@ struct tb_gp {
   std::vector<double> gibP;
   int gibM = 0, gibMp = 0, gibD = 0;
   double gibW = 0.0;
+  double feasAlpha = 0.0;               // alpha of the feasibility kinds (tb_acq_set_feasibility); 0 = not set
   uint64_t cache_gen = 0;               // bumped whenever the posterior cache is (re)built
   uint64_t gib_gen = tb::STALE;         // cache_gen the derived GIBBON state was built for
   tb::DevBuf dGibPs, dGibLinv, dGibWhat;

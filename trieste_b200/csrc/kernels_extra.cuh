@@ -664,7 +664,9 @@ acq_partials_kernel(const double* __restrict__ partial, int G, int64_t McPad, co
   double dm, dv;
   if (acq == TB_ACQ_MES) {
     mes_partials(samp, nsamp, mean[t], fmax(raw, 1e-12), clipped, dm, dv);
-  } else if (acq >= TB_ACQ_GIBBON_QUALITY) {
+  } else if (active_learning_kind(acq)) {
+    active_learning_partials(acq, param, aux, mean[t], fmax(raw, 1e-12), clipped, dm, dv);
+  } else if (gibbon_kind(acq)) {
     const double var = fmax(raw, 1e-12);
     dm = 0.0;
     dv = 0.0;

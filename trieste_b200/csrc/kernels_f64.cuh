@@ -354,6 +354,81 @@ __device__ __forceinline__ void acq_partials(int acq, double param, double aux, 
   dvar = clipped ? 0.0 : 1.0 / (2.0 * var * one_zR);
 }
 
+// ---- the kinds with a tail of their own beside acq_value (which the screened EI bound pass also inlines)
+__host__ __device__ __forceinline__ bool gibbon_kind(int acq) {
+  return acq == TB_ACQ_GIBBON_QUALITY || acq == TB_ACQ_GIBBON_REPULSION || acq == TB_ACQ_GIBBON;
+}
+__host__ __device__ __forceinline__ bool feasibility_kind(int acq) {
+  return acq == TB_ACQ_FEASIBILITY_BICHON || acq == TB_ACQ_FEASIBILITY_RANJAN;
+}
+__host__ __device__ __forceinline__ bool active_learning_kind(int acq) {
+  return feasibility_kind(acq) || acq == TB_ACQ_BALD || acq == TB_ACQ_PREDICTIVE_VARIANCE;
+}
+
+// ---- active learning (active_learning.py), values in the reference's operation order:
+//   feasibility (:220-245): s = sqrt(var), t = (T - mean)/s, t+- = t +- alpha; param = T, aux = alpha
+//     Bichon  G1 = alpha (Phi(t+) - Phi(t-)) - t (2 Phi(t) - Phi(t+) - Phi(t-)) - (2 phi(t) - phi(t+) - phi(t-)),  G1 s
+//     Ranjan  G2 = (alpha^2 - 1 - t^2)(Phi(t+) - Phi(t-)) - 2 t (phi(t+) - phi(t-)) + t+ phi(t+) - t- phi(t-),     G2 var
+//   BALD (:504-513): v = max(var, j), p = Phi(mean / sqrt(v + 1)), E = sqrt(C2)/sqrt(v + C2) exp(-mean^2 / (2 (v + C2))),
+//     C2 = pi log 2 / 2:  -p log(p + j) - (1 - p) log(1 - p + j) - E; param = j
+//   predictive variance at q = 1 (:108): var + param
+constexpr double BALD_C2 = 1.0887930451518010;  // pi log(2) / 2
+__device__ __forceinline__ double npdf(double x) { return exp(-0.5 * x * x) * 0.3989422804014327; }
+__device__ __forceinline__ double active_learning_value(int acq, double param, double aux, double mean, double var) {
+  if (acq == TB_ACQ_PREDICTIVE_VARIANCE) return var + param;
+  if (acq == TB_ACQ_BALD) {
+    const double v = fmax(var, param);
+    const double p = ndtr_tfp(mean / sqrt(v + 1.0));
+    const double ef = (sqrt(BALD_C2) / sqrt(v + BALD_C2)) * exp(-(mean * mean) / (2.0 * (v + BALD_C2)));
+    return -p * log(p + param) - (1.0 - p) * log(1.0 - p + param) - ef;
+  }
+  const double s = sqrt(var), a = aux;
+  const double t = (param - mean) / s, tp = t + a, tm = t - a;
+  const double cp = ndtr_tfp(tp), cm = ndtr_tfp(tm), pp = npdf(tp), pm = npdf(tm);
+  if (acq == TB_ACQ_FEASIBILITY_BICHON)
+    return (a * (cp - cm) - t * (2.0 * ndtr_tfp(t) - cp - cm) - (2.0 * npdf(t) - pp - pm)) * s;
+  return ((a * a - 1.0 - t * t) * (cp - cm) - 2.0 * t * (pp - pm) + tp * pp - tm * pm) * var;
+}
+// d/dmean and d/dvar of the above (A = Phi(t+) - Phi(t-), B = phi(t+) - phi(t-)):
+//   Bichon  dmean = 2 Phi(t) - Phi(t+) - Phi(t-),  dvar = (alpha A - (2 phi(t) - phi(t+) - phi(t-))) / (2 s)
+//   Ranjan  dmean = 2 s (t A + B),                 dvar = G2 + t (t A + B)
+//   BALD    h' = -log(p + j) - p/(p + j) + log(1 - p + j) + (1 - p)/(1 - p + j), u = mean / sqrt(v + 1):
+//           dmean = h' phi(u) / sqrt(v + 1) + E mean / (v + C2),
+//           dvar  = -h' phi(u) u / (2 (v + 1)) - E (mean^2 / (2 (v + C2)^2) - 1 / (2 (v + C2))), 0 where var < j
+//   predictive variance: dmean = 0, dvar = 1
+// and dvar = 0 where the tail clipped the variance
+__device__ __forceinline__ void active_learning_partials(int acq, double param, double aux, double mean, double var,
+                                                         bool clipped, double& dmu, double& dvar) {
+  if (acq == TB_ACQ_PREDICTIVE_VARIANCE) {
+    dmu = 0.0;
+    dvar = clipped ? 0.0 : 1.0;
+    return;
+  }
+  if (acq == TB_ACQ_BALD) {
+    const double v = fmax(var, param), sv = sqrt(v + 1.0), vc = v + BALD_C2;
+    const double u = mean / sv, p = ndtr_tfp(u), fu = npdf(u);
+    const double ef = (sqrt(BALD_C2) / sqrt(vc)) * exp(-(mean * mean) / (2.0 * vc));
+    const double dh = -log(p + param) - p / (p + param) + log(1.0 - p + param) + (1.0 - p) / (1.0 - p + param);
+    dmu = dh * fu / sv + ef * mean / vc;
+    dvar = (clipped || var < param) ? 0.0
+                                    : -dh * fu * u / (2.0 * (v + 1.0)) - ef * (mean * mean / (2.0 * vc * vc) - 1.0 / (2.0 * vc));
+    return;
+  }
+  const double s = sqrt(var), a = aux;
+  const double t = (param - mean) / s, tp = t + a, tm = t - a;
+  const double cp = ndtr_tfp(tp), cm = ndtr_tfp(tm), pp = npdf(tp), pm = npdf(tm);
+  const double A = cp - cm;
+  if (acq == TB_ACQ_FEASIBILITY_BICHON) {
+    dmu = 2.0 * ndtr_tfp(t) - cp - cm;
+    dvar = clipped ? 0.0 : (a * A - (2.0 * npdf(t) - pp - pm)) / (2.0 * s);
+    return;
+  }
+  const double B = pp - pm, tab = t * A + B;
+  const double g2 = (a * a - 1.0 - t * t) * A - 2.0 * t * B + tp * pp - tm * pm;
+  dmu = 2.0 * s * tab;
+  dvar = clipped ? 0.0 : g2 + t * tab;
+}
+
 struct BestPair {
   double v;
   int64_t i;
@@ -552,9 +627,10 @@ tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const doub
     if (out_var) out_var[t] = var;
     if (acq >= 0) {
       double v = (acq == TB_ACQ_MES) ? mes_value(samp, nsamp, mu, var)
-                 : (acq >= TB_ACQ_GIBBON_QUALITY)
+                 : gibbon_kind(acq)
                      ? gibbon_value(acq, samp, nsamp, mu, var, aux, pen.gib_uu ? pen.gib_uu[t] : 0.0, pen.gib_w)
-                     : acq_value(acq, param, aux, mu, var);
+                 : active_learning_kind(acq) ? active_learning_value(acq, param, aux, mu, var)
+                                             : acq_value(acq, param, aux, mu, var);
       if (PEN) {
         vb = v;
       } else {

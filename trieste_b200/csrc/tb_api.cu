@@ -4,6 +4,7 @@
 #include "kernels_extra.cuh"
 #include "prescreen.cuh"
 #include "batch_ei.cuh"
+#include "active_learning.cuh"
 #include "ehvi.cuh"
 #include "int8_engines.h"
 #include <chrono>
@@ -829,6 +830,9 @@ static int launch_grad(tb_gp* gp, const double* xc, int64_t mc, double* grad_dev
 
 static inline bool gibbon_repulsion_kind(int acq) { return acq == TB_ACQ_GIBBON_REPULSION || acq == TB_ACQ_GIBBON; }
 
+// the tails' second parameter: the feasibility kinds' alpha (tb_acq_set_feasibility), else the likelihood noise variance
+static inline double tail_aux(const tb_gp* gp, int acq) { return feasibility_kind(acq) ? gp->feasAlpha : gp->noise; }
+
 // GIBBON cross term of one chunk (ensure_gibbon has run): |u|^2 into sGib[0, mc); with keep_u also u into sGib[2 mc, ...) for
 // gibbon_grad_kernel.  One launch whatever m.
 static int launch_gibbon_cross(tb_gp* gp, cudaStream_t st, const double* xc, int64_t mc, bool keep_u) {
@@ -869,7 +873,7 @@ static int launch_partials(tb_gp* gp, cudaStream_t st, int acq, double param, co
   if (gib) TB_TRY(launch_gibbon_cross(gp, st, xc, mc, true));
   double* g = gib ? gp->sGib.as<double>() : nullptr;
   acq_partials_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, st>>>(partial, G, McPad, mean, mc, gp->variance, acq, param,
-                                                                    gp->noise, gp->dMes.as<double>(), gp->mesS, cmu, cmu + mc,
+                                                                    tail_aux(gp, acq), gp->dMes.as<double>(), gp->mesS, cmu, cmu + mc,
                                                                     g, gp->gibW, g ? g + mc : nullptr);
   TB_LAUNCHED();
   return 0;
@@ -904,10 +908,10 @@ static int launch_tail(tb_gp* gp, cudaStream_t st, const EvalRequest& rq, const 
     pen.P = gp->penP;
     pen.D = gp->D;
     pen.kind = gp->penKind;
-    tail_kernel<true><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, gp->noise,
+    tail_kernel<true><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, tail_aux(gp, rq.acq),
                                               gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, idx_map, pen);
   } else {
-    tail_kernel<false><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, gp->noise,
+    tail_kernel<false><<<blocks, 256, 0, st>>>(partial, G, McPad, mean, mc, c0, gp->variance, rq.acq, rq.param, tail_aux(gp, rq.acq),
                                                gp->dMes.as<double>(), gp->mesS, d_vals, d_mean, d_var, bb, bi, idx_map, pen);
   }
   TB_LAUNCHED();
@@ -1713,8 +1717,8 @@ int tb_gp_mean_gradient(tb_gp* gp, const void* Xc, int64_t M, void* mean, void* 
 static int check_acq(tb_gp* gp, int& acq, double param, bool& pen, const char* who) {
   pen = (acq & TB_ACQ_PENALIZED) != 0;
   acq &= ~TB_ACQ_PENALIZED;
-  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_GIBBON, std::string(who) + ": unknown acquisition kind");
-  TB_CHECK(!(pen && acq >= TB_ACQ_GIBBON_QUALITY),
+  TB_CHECK(acq >= TB_ACQ_EI && acq <= TB_ACQ_PREDICTIVE_VARIANCE, std::string(who) + ": unknown acquisition kind");
+  TB_CHECK(!(pen && gibbon_kind(acq)),
            std::string(who) + ": the GIBBON kinds do not compose with TB_ACQ_PENALIZED (the repulsion term is their batch term)");
   if (pen)
     TB_CHECK(gp->penP > 0 && gp->penD == gp->D,
@@ -1722,7 +1726,10 @@ static int check_acq(tb_gp* gp, int& acq, double param, bool& pen, const char* w
   if (acq == TB_ACQ_LCB || acq == TB_ACQ_NEG_LCB)
     TB_CHECK(param >= 0.0, "Standard deviation scaling parameter beta must not be negative");
   if (acq == TB_ACQ_MES) TB_CHECK(gp->mesS > 0, "min-value entropy search: set the min-value samples first (tb_acq_set_min_value_samples)");
-  if (acq < TB_ACQ_GIBBON_QUALITY) return 0;
+  if (feasibility_kind(acq))
+    TB_CHECK(gp->feasAlpha > 0.0, std::string(who) + ": the feasibility criteria need alpha first (tb_acq_set_feasibility)");
+  if (acq == TB_ACQ_BALD) TB_CHECK(param > 0.0, "Jitter must be positive.");
+  if (!gibbon_kind(acq)) return 0;
   if (acq != TB_ACQ_GIBBON_REPULSION)
     TB_CHECK(gp->mesS > 0, std::string(who) + ": GIBBON's quality term needs the min-value samples first (tb_acq_set_min_value_samples)");
   if (acq != TB_ACQ_GIBBON_QUALITY) {
@@ -1825,6 +1832,13 @@ int tb_acq_set_gibbon_repulsion(tb_gp* gp, const double* pending, int m, double 
   return rc;
 }
 
+int tb_acq_set_feasibility(tb_gp* gp, double alpha) {
+  TB_CHECK(gp, "tb_acq_set_feasibility: null handle");
+  TB_CHECK(std::isfinite(alpha) && alpha > 0.0, "Parameter alpha must be positive.");
+  gp->feasAlpha = alpha;
+  return 0;
+}
+
 int tb_gp_profile(tb_gp* gp, int enable) {
   TB_CHECK(gp, "tb_gp_profile: null handle");
   gp->profile = enable != 0;
@@ -1920,11 +1934,12 @@ enum class BatchTail {
   Samples,  // mean + chol(cov + jitter I) eps, eps [q, S] normal base samples (sampler.py:277-278)
   McEi,     // batch Monte-Carlo EI (function.py:1181-1186) over eps [q, S] normal base samples
   BatchEi,  // batch EI of Chevalier & Ginsbourger (function.py:1747-1805) over the Sobol points w [q-1, S]
+  PredVar,  // exp(logdet(cov + jitter 1 1^T)) of active learning's predictive variance (active_learning.py:98-108)
 };
 
 struct BatchRequest {
   BatchTail tail;
-  bool grad = false;  // also d out_val / d Xc (McEi, BatchEi)
+  bool grad = false;  // also d out_val / d Xc (McEi, BatchEi, PredVar)
   const double* Xc = nullptr;  // [B, q, D]
   int64_t B;
   int q;
@@ -1992,18 +2007,18 @@ static int launch_qei_cross(tb_gp* gp, const double* xc, int64_t npts, int q, co
 
 // Every q-batch call, chunk by chunk of whole batches: K* -> A = Linv K* (stored plain) -> with a gradient, V = K^-1 K*
 // -> per-batch mean / cov (joint_kernel, which also computes the Samples tail and the McEi value) -> the other tails:
-// bei_kernel for the BatchEi value; for a gradient the tail's reverse kernel (value, G_mu, Sigma_bar: qei_backward_kernel
-// or bei_backward_kernel) -> per-batch mix V~ = Sigma_bar V (qei_mix_kernel) -> grad_kernel (the training-point sums) ->
-// qei_cross_kernel (the K(x_b, x_b) term).
+// bei_kernel for the BatchEi value, pv_kernel for the PredVar value; for a gradient the tail's reverse kernel (value, G_mu,
+// Sigma_bar: qei_backward_kernel, bei_backward_kernel or pv_kernel<true>) -> per-batch mix V~ = Sigma_bar V (qei_mix_kernel)
+// -> grad_kernel (the training-point sums) -> qei_cross_kernel (the K(x_b, x_b) term).
 static int run_batch(tb_gp* gp, const BatchRequest& rq) {
   if (rq.B == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
   cudaStream_t st = gp->stream;
   const int D = gp->D, q = rq.q, S = rq.S;
   const int64_t lda = (int64_t)gp->NB * BM;
-  const bool bei = rq.tail == BatchTail::BatchEi;
+  const bool bei = rq.tail == BatchTail::BatchEi, pv = rq.tail == BatchTail::PredVar;
   const int mode = rq.tail == BatchTail::Samples ? JOINT_SAMPLE : rq.tail == BatchTail::McEi && !rq.grad ? JOINT_QEI : JOINT_PREDICT;
-  const bool post_dev = bei || rq.grad;  // joint_kernel leaves mean / cov in bmu / bcov for a tail kernel
+  const bool post_dev = bei || pv || rq.grad;  // joint_kernel leaves mean / cov in bmu / bcov for a tail kernel
   Engine e;
   TB_TRY(select_engine(gp, rq.grad, &e));
   const int nt = eng_tile_width(gp, e);  // candidates per tile
@@ -2062,6 +2077,12 @@ static int run_batch(tb_gp* gp, const BatchRequest& rq) {
       TB_CUDA(cudaFuncSetAttribute(bei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
     else
       TB_CUDA(cudaFuncSetAttribute(bei_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
+  } else if (pv) {
+    tail_smem = (size_t)PV_WARPS * pv_warp_doubles(q, rq.grad) * sizeof(double);
+    if (rq.grad)
+      TB_CUDA(cudaFuncSetAttribute(pv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
+    else
+      TB_CUDA(cudaFuncSetAttribute(pv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
   } else if (rq.grad) {
     tail_smem = (size_t)QEIG_WARPS * (3 * q * q + 2 * q) * sizeof(double);
     TB_CUDA(cudaFuncSetAttribute(qei_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem));
@@ -2092,12 +2113,22 @@ static int run_batch(tb_gp* gp, const BatchRequest& rq) {
       TB_LAUNCHED();
       TB_CUDA(cudaGetLastError());
     }
+    if (pv) {
+      const unsigned blocks = (unsigned)((nbc + PV_WARPS - 1) / PV_WARPS);
+      double* cmu = rq.grad ? gp->sMisc.as<double>() : nullptr;
+      if (rq.grad)
+        pv_kernel<true><<<blocks, PV_WARPS * 32, tail_smem, st>>>(cv, nbc, q, rq.jitter, dval, cmu, cmu + mc, bsbar.as<double>(), err);
+      else
+        pv_kernel<false><<<blocks, PV_WARPS * 32, tail_smem, st>>>(cv, nbc, q, rq.jitter, dval, nullptr, nullptr, nullptr, err);
+      TB_LAUNCHED();
+      TB_CUDA(cudaGetLastError());
+    }
     if (rq.grad) {
       double* cmu = gp->sMisc.as<double>();
       if (bei)
         bei_backward_kernel<<<(unsigned)nbc, bei_warps * 32, tail_smem, st>>>(mu, cv, q, eps_dev, S, rq.eta, dval, cmu, cmu + mc,
                                                                               bsbar.as<double>(), err);
-      else
+      else if (!pv)
         qei_backward_kernel<<<(unsigned)((nbc + QEIG_WARPS - 1) / QEIG_WARPS), QEIG_WARPS * 32, tail_smem, st>>>(
             mu, cv, nbc, q, eps_dev, S, rq.eta, rq.jitter, dval, cmu, cmu + mc, bsbar.as<double>(), err);
       TB_LAUNCHED();
@@ -2114,8 +2145,10 @@ static int run_batch(tb_gp* gp, const BatchRequest& rq) {
   TB_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
-  TB_CHECK_CODE(herr == 0, "Cholesky decomposition was not successful. The input might not be valid "
-                      "(covariance + jitter*I of a query batch is not positive definite)", tb::ERR_NUMERIC);
+  TB_CHECK_CODE(herr == 0, pv ? "Cholesky decomposition was not successful. The input might not be valid "
+                                "(covariance + jitter of a query batch is not positive definite)"
+                              : "Cholesky decomposition was not successful. The input might not be valid "
+                                "(covariance + jitter*I of a query batch is not positive definite)", tb::ERR_NUMERIC);
   return 0;
 }
 
@@ -2885,6 +2918,19 @@ int tb_acq_batch_mc_ei_grad(tb_gp* gp, const void* Xc, int64_t B, int q, const v
   tb::DtypeBridge br(gp);
   TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
   TB_TRY(br.in(eps, (int64_t)q * S, &rq.eps));
+  TB_TRY(br.out(out, B, &rq.out_val));
+  TB_TRY(br.out(grad, B * q * gp->D, &rq.out_grad));
+  TB_TRY(tb::run_batch(gp, rq));
+  return br.finish();
+}
+
+int tb_acq_predictive_variance(tb_gp* gp, const void* Xc, int64_t B, int q, double jitter, void* out, void* grad) {
+  TB_CHECK(gp && (B == 0 || (Xc && out)), "tb_acq_predictive_variance: null argument");
+  TB_TRY(tb::check_batch(gp, B, q, false, 0, nullptr, 0.0));
+  tb::BatchRequest rq(tb::BatchTail::PredVar, B, q, 0, 0.0, jitter);
+  rq.grad = grad != nullptr;
+  tb::DtypeBridge br(gp);
+  TB_TRY(br.in(Xc, B * q * gp->D, &rq.Xc));
   TB_TRY(br.out(out, B, &rq.out_val));
   TB_TRY(br.out(grad, B * q * gp->D, &rq.out_grad));
   TB_TRY(tb::run_batch(gp, rq));
