@@ -270,6 +270,25 @@ int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const d
 int tb_rff_maximize_boxes(tb_rff* r, const double* lower, const double* upper, int nbox, const double* starts, int64_t R,
                           int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
                           int32_t* success, int64_t* nfev);
+/* BatchTrustRegionBox with local models (rule.py:1364-1435: the base rule deep-copied per region, each region's function
+ * maximised inside its region by _perform_parallel_continuous_optimization, optimizer.py:566-745), all regions in ONE device
+ * L-BFGS: problem p = r * S + s of the starts [R, S, D] maximises acq[s] with param[s] under models[s] inside the box s of
+ * lower / upper [S, D].  Each round evaluates every model's active problems on that model's stream, the models side by side,
+ * with one host synchronise per round.  Results are bit for bit those of S tb_acq_maximize calls, model s from the starts
+ * [R, s, D].  The models share one device, dtype and D, have their posterior caches built, pass tb_acq_maximize's acquisition
+ * checks and are distinct handles (their min-value samples, penalty and alpha are their own).  x_out [R, S, D], f_out, success,
+ * nfev [R, S] as tb_acq_maximize.  R * S < 2^31. */
+int tb_acq_maximize_models(tb_gp* const* models, const int* acq, const double* param, int S, const double* lower,
+                           const double* upper, const double* starts, int64_t R, int maxcor, int maxiter, int maxls, double gtol,
+                           double ftol, double* x_out, double* f_out, int32_t* success, int64_t* nfev);
+/* The same for ParallelContinuousThompsonSampling with local models (rule.py:1364-1435): S trajectory handles of k = nb
+ * trajectories each (every r[s]->nb == k), V = k * S columns; start (i, v) of the starts [R, V, D] maximises -f of trajectory
+ * v / S of r[v % S] inside box v % S of lower / upper [S, D], the round robin of a TaggedMultiSearchSpace (optimizer.py:859-890).
+ * Bit for bit the results of tb_rff_maximize_boxes(r[s], box s) from the starts [R, k, D] of the columns v = j * S + s.
+ * x_out [R, V, D], f_out [R, V] (= -f at x_out), success, nfev as tb_rff_maximize.  R * V < 2^31. */
+int tb_rff_maximize_models(tb_rff* const* r, int S, const double* lower, const double* upper, const double* starts, int64_t R,
+                           int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
+                           int32_t* success, int64_t* nfev);
 /* (K(X,X) + noise I)^-1 B = Linv^T (Linv B) through the cached triangular inverse: B, out [nrhs][N] (each right-hand side contiguous);
  * the v-weights of a decoupled trajectory (sampler.py:716, gpflux compute_A_inv_b).  fp64, host or device. */
 int tb_gp_kinv_apply(tb_gp* gp, const double* B, int nrhs, double* out);

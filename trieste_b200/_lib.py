@@ -67,6 +67,8 @@ SIGNATURES = {
     "tb_rff_eval_paired": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp]),
     "tb_rff_maximize": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
     "tb_rff_maximize_boxes": (_i32, [_vp, _vp, _vp, _i32, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
+    "tb_acq_maximize_models": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
+    "tb_rff_maximize_models": (_i32, [_vp, _i32, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
     "tb_ehvi_create": (_i32, [C.POINTER(_vp), C.POINTER(_vp), _i32]),
     "tb_ehvi_destroy": (_i32, [_vp]),
     "tb_ehvi_set_cells": (_i32, [_vp, _vp, _vp, _i64]),

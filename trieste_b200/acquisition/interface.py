@@ -6,6 +6,7 @@ the *same* function object from ``update`` (tests assert identity, test_function
 """
 from __future__ import annotations
 
+import copy
 from abc import ABC, abstractmethod
 from typing import Callable, Generic, Mapping, Optional, TypeVar
 
@@ -52,6 +53,9 @@ class SingleModelAcquisitionBuilder(Generic[M_contra], ABC):
             def __repr__(self) -> str:
                 return f"{single!r} using tag {tag!r}"
 
+            def __deepcopy__(self, memo):  # a copy wraps a copy of the builder and its state (one per trust region)
+                return copy.deepcopy(single, memo).using(tag)
+
         return _Anon()
 
     @abstractmethod
@@ -96,6 +100,9 @@ class SingleModelGreedyAcquisitionBuilder(Generic[M_contra], ABC):
             def __repr__(self) -> str:
                 return f"{single!r} using tag {tag!r}"
 
+            def __deepcopy__(self, memo):  # a copy wraps a copy of the builder and its state (one per trust region)
+                return copy.deepcopy(single, memo).using(tag)
+
         return _Anon()
 
     @abstractmethod
@@ -126,5 +133,8 @@ class SingleModelVectorizedAcquisitionBuilder(SingleModelAcquisitionBuilder[M_co
 
             def __repr__(self) -> str:
                 return f"{single!r} using tag {tag!r}"
+
+            def __deepcopy__(self, memo):  # a copy wraps a copy of the builder and its state (one per trust region)
+                return copy.deepcopy(single, memo).using(tag)
 
         return _Anon()

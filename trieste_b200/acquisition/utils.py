@@ -1,5 +1,6 @@
-"""``split_acquisition_function`` / ``split_acquisition_function_calls`` / ``select_nth_output`` — mirrors
-trieste/acquisition/utils.py:31-123 — and ``MultivariateNormalCDF`` (acquisition/function/utils.py:29-199).
+"""``split_acquisition_function`` / ``split_acquisition_function_calls`` / ``select_nth_output`` and the local-model helpers
+``copy_to_local_models`` / ``with_local_datasets`` — mirrors trieste/acquisition/utils.py:31-204 — and
+``MultivariateNormalCDF`` (acquisition/function/utils.py:29-199).
 
 In the reference these wrappers bound the memory of one TensorFlow evaluation by cutting the leading (candidate) axis into
 blocks.  Here the fused kernels already stream any batch through bounded scratch (``run_eval`` chunks at
@@ -7,10 +8,13 @@ blocks.  Here the fused kernels already stream any batch through bounded scratch
 optimisers keep working, with the reference's splitting rule and error behaviour."""
 from __future__ import annotations
 
+import copy
 import functools
 import math
 
 import numpy as np
+
+from .interface import OBJECTIVE
 
 
 def _concat(parts):
@@ -57,6 +61,42 @@ def split_acquisition_function_calls(optimizer, split_size: int):
         return optimizer(search_space, (taf, n) if isinstance(f, tuple) else taf)
 
     return split_optimizer
+
+
+def copy_to_local_models(global_model, num_local_models: int, key=OBJECTIVE):
+    """utils.py:146-160: ``num_local_models`` deep copies of ``global_model`` under ``LocalizedTag(key, i)``.  A copy of a
+    ``GaussianProcessRegression`` owns its own device handle, data and posterior cache."""
+    from ..utils import LocalizedTag
+
+    return {LocalizedTag(key, i): copy.deepcopy(global_model) for i in range(num_local_models)}
+
+
+def with_local_datasets(datasets, num_local_datasets: int, local_dataset_indices=None):
+    """utils.py:163-204: ``datasets`` plus, for every global tag without them, ``num_local_datasets`` local datasets under
+    ``LocalizedTag(tag, i)``: the whole global dataset, or its rows ``local_dataset_indices[i]``."""
+    from ..data import Dataset
+    from ..utils import LocalizedTag
+
+    if local_dataset_indices is not None and len(local_dataset_indices) != num_local_datasets:
+        raise ValueError(
+            f"local_dataset_indices should have {num_local_datasets} entries, has {len(local_dataset_indices)}"
+        )
+    updated_datasets = {}
+    for tag in datasets:
+        updated_datasets[tag] = datasets[tag]
+        ltag = LocalizedTag.from_tag(tag)
+        if not ltag.is_local:
+            for i in range(num_local_datasets):
+                target_ltag = LocalizedTag(ltag.global_tag, i)
+                if target_ltag not in datasets:
+                    if local_dataset_indices is None:
+                        updated_datasets[target_ltag] = datasets[tag]
+                    else:
+                        rows = np.asarray(local_dataset_indices[i], dtype=np.int64)
+                        updated_datasets[target_ltag] = Dataset(
+                            np.asarray(datasets[tag].query_points)[rows], np.asarray(datasets[tag].observations)[rows]
+                        )
+    return updated_datasets
 
 
 def select_nth_output(x, output_dim: int = 0):

@@ -174,41 +174,56 @@ lbfgs_step_kernel(State s, Options o, int n_active, const int* __restrict__ idx,
   if (lane == 0) s.status[p] = status;
 }
 
-// deterministic compaction of the active problems (single CTA, block scan) + gather of their trial points
+// deterministic compaction of the active problems (single CTA, block scan) + gather of their trial points.  The active problems
+// are ordered by group g = p % G, increasing p within a group; count[g] receives the number of active problems of group g (with
+// G = 1, count[0] is the number of active problems and idx lists them in increasing order).
 __global__ void __launch_bounds__(1024)
-lbfgs_compact_kernel(const int* __restrict__ status, long long P, int* __restrict__ idx, int* __restrict__ count) {
+lbfgs_compact_kernel(const int* __restrict__ status, long long P, int G, int* __restrict__ idx, int* __restrict__ count) {
   __shared__ int warp_tot[32];
   __shared__ int base;
   if (threadIdx.x == 0) base = 0;
   __syncthreads();
-  for (long long c0 = 0; c0 < P; c0 += blockDim.x) {
-    const long long p = c0 + threadIdx.x;
-    const int a = (p < P && status[p] == ST_ACTIVE) ? 1 : 0;
-    int v = a;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int n = __shfl_up_sync(0xffffffffu, v, o);
-      if ((threadIdx.x & 31) >= o) v += n;
-    }
-    if ((threadIdx.x & 31) == 31) warp_tot[threadIdx.x >> 5] = v;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      int t = warp_tot[threadIdx.x];
+  int prev = 0;  // thread 0: active problems of the groups before g
+  for (int g = 0; g < G; ++g) {
+    const long long nG = (P - g + G - 1) / G;  // problems g, g + G, ...
+    for (long long c0 = 0; c0 < nG; c0 += blockDim.x) {
+      const long long j = c0 + threadIdx.x, p = g + j * G;
+      const int a = (j < nG && status[p] == ST_ACTIVE) ? 1 : 0;
+      int v = a;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
-        const int n = __shfl_up_sync(0xffffffffu, t, o);
-        if (threadIdx.x >= o) t += n;
+        const int n = __shfl_up_sync(0xffffffffu, v, o);
+        if ((threadIdx.x & 31) >= o) v += n;
       }
-      warp_tot[threadIdx.x] = t;  // inclusive totals of the warps
+      if ((threadIdx.x & 31) == 31) warp_tot[threadIdx.x >> 5] = v;
+      __syncthreads();
+      if (threadIdx.x < 32) {
+        int t = warp_tot[threadIdx.x];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int n = __shfl_up_sync(0xffffffffu, t, o);
+          if (threadIdx.x >= o) t += n;
+        }
+        warp_tot[threadIdx.x] = t;  // inclusive totals of the warps
+      }
+      __syncthreads();
+      const int before = ((threadIdx.x >> 5) > 0 ? warp_tot[(threadIdx.x >> 5) - 1] : 0) + v - a;
+      if (a) idx[base + before] = (int)p;
+      __syncthreads();
+      if (threadIdx.x == 0) base += warp_tot[31];
+      __syncthreads();
     }
-    __syncthreads();
-    const int before = ((threadIdx.x >> 5) > 0 ? warp_tot[(threadIdx.x >> 5) - 1] : 0) + v - a;
-    if (a) idx[base + before] = (int)p;
-    __syncthreads();
-    if (threadIdx.x == 0) base += warp_tot[31];
-    __syncthreads();
+    if (threadIdx.x == 0) {
+      count[g] = base - prev;
+      prev = base;
+    }
   }
-  if (threadIdx.x == 0) *count = base;
+}
+
+// trajectory of each compacted problem of tb_rff_maximize_models: problem p = i * V + v runs trajectory v / S of its handle
+__global__ void lbfgs_traj_index_kernel(const int* __restrict__ idx, int n, int V, int S, int* __restrict__ traj) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n) traj[t] = (idx[t] % V) / S;
 }
 
 __global__ void lbfgs_gather_kernel(const double* __restrict__ xtrial, const int* __restrict__ idx, int n_active, int D,

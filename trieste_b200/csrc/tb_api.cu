@@ -742,6 +742,7 @@ struct EvalRequest {
   double* out_grad = nullptr;  // [M, D] (nullable)
   bool want_argmax = false;
   bool pen = false;  // TB_ACQ_PENALIZED: multiply by the handle's local penalty (tb_acq_set_penalization)
+  bool sync = true;  // false: run_eval returns with its work queued on the handle's stream (device outputs only, no argmax)
   double best_value = 0.0;
   int64_t best_index = -1;
 };
@@ -1560,6 +1561,7 @@ static int run_eval(tb_gp* gp, EvalRequest& rq) {
     TB_TRY(var.back(c0, mc));
   }
   if (rq.want_argmax) TB_TRY(argmax_end(gp, rq));
+  if (!rq.sync) return 0;  // the caller synchronises, then folds the profile
   TB_CUDA(cudaStreamSynchronize(st));
   TB_CUDA(cudaGetLastError());
   return profile_fold(gp);
@@ -2736,11 +2738,13 @@ static int check_starts(const std::string& who, int64_t P, const double* starts,
 }
 
 // The multi-start L-BFGS round loop shared by every device maximiser: P (>= 1) problems in D dimensions on the stream st, problem
-// p inside box p % nbox of lower/upper [nbox, D]; each
-// round asks eval(xt [n, D], idx [n], n, vals [n], grad [n, D]) for the values and gradients of the function to MAXIMISE at the
-// trial points of the n active problems (all device arrays; idx holds their problem indices), then runs one step of each.
+// p inside box p % nbox of lower/upper [nbox, D] and in group p % G; each
+// round asks eval(xt [n, D], idx [n], n, vals [n], grad [n, D], group_n [G]) for the values and gradients of the function to
+// MAXIMISE at the trial points of the n active problems (all device arrays; idx holds their problem indices, ordered by group,
+// and the host array group_n the number of them in each group), then runs one step of each.  The device-to-host read of the
+// group counts is the round's one host synchronise.
 template <class Eval>
-static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* lower, const double* upper, int nbox,
+static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* lower, const double* upper, int nbox, int G,
                      const double* starts, int64_t P, int maxcor, int maxiter, int maxls, double gtol, double ftol, Eval&& eval, double* x_out,
                      double* f_out, int32_t* success, int64_t* nfev) {
   const int m = maxcor;
@@ -2752,7 +2756,7 @@ static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* low
   TB_TRY(bS.reserve(8 * PD * m)); TB_TRY(bY.reserve(8 * PD * m)); TB_TRY(brho.reserve(8 * (size_t)P * m));
   TB_TRY(bint.reserve(sizeof(int) * 6 * (size_t)P)); TB_TRY(bnfev.reserve(8 * (size_t)P));
   TB_TRY(bidx.reserve(sizeof(int) * (size_t)P)); TB_TRY(bxt.reserve(8 * PD)); TB_TRY(bval.reserve(8 * (size_t)P));
-  TB_TRY(bgrad.reserve(8 * PD)); TB_TRY(bbox.reserve(8 * 2 * (size_t)nbox * D)); TB_TRY(bcount.reserve(sizeof(int)));
+  TB_TRY(bgrad.reserve(8 * PD)); TB_TRY(bbox.reserve(8 * 2 * (size_t)nbox * D)); TB_TRY(bcount.reserve(sizeof(int) * (size_t)G));
   tb::lb::State s;
   s.x = bx.as<double>(); s.f = bf.as<double>(); s.g = bg.as<double>(); s.d = bd.as<double>(); s.t = bt.as<double>();
   s.S = bS.as<double>(); s.Y = bY.as<double>(); s.rho = brho.as<double>(); s.gam = bgam.as<double>();
@@ -2772,11 +2776,14 @@ static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* low
   TB_LAUNCHED();
   tb::lb::Options o{D, m, maxiter, maxls, nbox, gtol, ftol};
   int n_active = 0;
+  std::vector<int> group_n(G, 0);
   auto compact = [&]() -> int {
-    tb::lb::lbfgs_compact_kernel<<<1, 1024, 0, st>>>(s.status, P, bidx.as<int>(), bcount.as<int>());
+    tb::lb::lbfgs_compact_kernel<<<1, 1024, 0, st>>>(s.status, P, G, bidx.as<int>(), bcount.as<int>());
     TB_LAUNCHED();
-    TB_CUDA(cudaMemcpyAsync(&n_active, bcount.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    TB_CUDA(cudaMemcpyAsync(group_n.data(), bcount.p, sizeof(int) * (size_t)G, cudaMemcpyDeviceToHost, st));
     TB_CUDA(cudaStreamSynchronize(st));
+    n_active = 0;
+    for (int g = 0; g < G; ++g) n_active += group_n[g];
     if (n_active > 0) {
       tb::lb::lbfgs_gather_kernel<<<(unsigned)(((size_t)n_active * D + 255) / 256), 256, 0, st>>>(s.xtrial, bidx.as<int>(), n_active, D,
                                                                                                  bxt.as<double>());
@@ -2792,7 +2799,7 @@ static int lbfgs_run(const char* name, cudaStream_t st, int D, const double* low
   for (int64_t round = 0; n_active > 0 && round < max_rounds; ++round) {
     const auto t_round = std::chrono::steady_clock::now();
     const int n_round = n_active;
-    TB_TRY(eval(bxt.as<double>(), bidx.as<int>(), n_active, bval.as<double>(), bgrad.as<double>()));
+    TB_TRY(eval(bxt.as<double>(), bidx.as<int>(), n_active, bval.as<double>(), bgrad.as<double>(), group_n.data()));
     tb::lb::lbfgs_step_kernel<<<(unsigned)((n_active + 7) / 8), 256, 0, st>>>(s, o, n_active, bidx.as<int>(), bxt.as<double>(),
                                                                              bval.as<double>(), bgrad.as<double>(), dlo, dup);
     TB_LAUNCHED();
@@ -2834,7 +2841,7 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
   TB_TRY(check_acq(gp, acq, param, pen, "tb_acq_maximize"));
   if (P == 0) return 0;
   TB_CUDA(cudaSetDevice(gp->device));
-  auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad) -> int {
+  auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad, const int*) -> int {
     tb::EvalRequest rq;
     rq.acq = acq;
     rq.pen = pen;
@@ -2845,7 +2852,7 @@ int tb_acq_maximize(tb_gp* gp, int acq, double param, const double* lower, const
     rq.out_grad = grad;
     return tb::run_eval(gp, rq);
   };
-  return tb::lbfgs_run("tb_acq_maximize", gp->stream, gp->D, lower, upper, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
+  return tb::lbfgs_run("tb_acq_maximize", gp->stream, gp->D, lower, upper, 1, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
                        x_out, f_out, success, nfev);
 }
 
@@ -2863,14 +2870,14 @@ int tb_rff_maximize_boxes(tb_rff* r, const double* lower, const double* upper, i
   const int D = r->D;
   // problem p = (i, b) of the [R, nb, D] starts runs on trajectory p % nb inside box p % nbox = b % nbox (nbox divides nb); the
   // step kernel maximises, so the values and gradients handed to it are those of -f_b
-  auto eval = [&](const double* xt, const int* idx, int n, double* vals, double* grad) -> int {
+  auto eval = [&](const double* xt, const int* idx, int n, double* vals, double* grad, const int*) -> int {
     for (int64_t c0 = 0; c0 < n; c0 += tb::RFF_PAIRED_CHUNK) {
       const int64_t mc = std::min<int64_t>(tb::RFF_PAIRED_CHUNK, n - c0);
       TB_TRY(tb::launch_rff_paired(r, xt + c0 * D, mc, 0, idx + c0, -1.0, vals + c0, grad + c0 * D));
     }
     return 0;
   };
-  return tb::lbfgs_run("tb_rff_maximize", r->stream, D, lower, upper, nbox, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
+  return tb::lbfgs_run("tb_rff_maximize", r->stream, D, lower, upper, nbox, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval,
                        x_out, f_out, success, nfev);
 }
 
@@ -2878,6 +2885,150 @@ int tb_rff_maximize(tb_rff* r, const double* lower, const double* upper, const d
                     int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
                     int64_t* nfev) {
   return tb_rff_maximize_boxes(r, lower, upper, 1, starts, R, maxcor, maxiter, maxls, gtol, ftol, x_out, f_out, success, nfev);
+}
+
+}  // extern "C"
+
+namespace tb {
+// ordering events that destroy themselves
+struct Events {
+  std::vector<cudaEvent_t> e;
+  Events() = default;
+  Events(const Events&) = delete;
+  Events& operator=(const Events&) = delete;
+  ~Events() {
+    for (cudaEvent_t x : e)
+      if (x) cudaEventDestroy(x);
+  }
+  int create(int n) {
+    e.assign(n, nullptr);
+    for (cudaEvent_t& x : e) TB_CUDA(cudaEventCreateWithFlags(&x, cudaEventDisableTiming));
+    return 0;
+  }
+};
+
+// One evaluation round of a maximiser over S handles (lbfgs_run with G = S): group s, the group_n[s] compacted problems at
+// offset o, is queued by run(s, o, group_n[s]) on streams[s].  Every stream waits for st before its group and st waits for it
+// after (the ehvi_run pattern), so the groups overlap on the device and the round keeps lbfgs_run's single host synchronise.
+// ev holds S + 1 events.
+template <class Run>
+static int fork_join(cudaStream_t st, const cudaStream_t* streams, int S, const int* group_n, Events& ev, Run&& run) {
+  TB_CUDA(cudaEventRecord(ev.e[0], st));
+  int64_t o = 0;
+  for (int s = 0; s < S; ++s) {
+    if (group_n[s] == 0) continue;
+    const bool own = streams[s] != st;
+    if (own) TB_CUDA(cudaStreamWaitEvent(streams[s], ev.e[0], 0));
+    TB_TRY(run(s, o, group_n[s]));
+    if (own) {
+      TB_CUDA(cudaEventRecord(ev.e[s + 1], streams[s]));
+      TB_CUDA(cudaStreamWaitEvent(st, ev.e[s + 1], 0));
+    }
+    o += group_n[s];
+  }
+  return 0;
+}
+}  // namespace tb
+
+extern "C" {
+
+int tb_acq_maximize_models(tb_gp* const* models, const int* acq, const double* param, int S, const double* lower,
+                           const double* upper, const double* starts, int64_t R, int maxcor, int maxiter, int maxls, double gtol,
+                           double ftol, double* x_out, double* f_out, int32_t* success, int64_t* nfev) {
+  const std::string who = "tb_acq_maximize_models";
+  TB_CHECK(models && acq && param && lower && upper, who + ": null argument");
+  TB_CHECK(S >= 1, who + ": the number of models must be at least 1, got " + std::to_string(S));
+  std::vector<int> kind(acq, acq + S);
+  std::vector<char> pen(S, 0);
+  for (int s = 0; s < S; ++s) {
+    tb_gp* gp = models[s];
+    TB_CHECK(gp, who + ": null model handle " + std::to_string(s));
+    // handle state (min-value samples, local penalty, feasibility alpha) belongs to one function: no handle twice
+    for (int j = 0; j < s; ++j) TB_CHECK(models[j] != gp, who + ": the same model handle appears twice");
+    TB_CHECK(gp->device == models[0]->device, who + ": the models must be on one device");
+    TB_CHECK(gp->dtype == models[0]->dtype, who + ": the models must have one dtype");
+    TB_CHECK(gp->D == models[0]->D, who + ": the models must have one input dimension");
+    TB_CHECK(gp->cache_valid, who + ": posterior cache of model " + std::to_string(s) +
+                                  " is not built: call tb_gp_update_posterior_cache first");
+    bool p = false;
+    TB_TRY(check_acq(gp, kind[s], param[s], p, who.c_str()));
+    pen[s] = p;
+  }
+  TB_CHECK(R >= 0 && R < ((int64_t)1 << 31) / S, who + ": number of starts out of range");
+  const int64_t P = R * S;
+  TB_TRY(tb::check_starts(who, P, starts, x_out, f_out, success, nfev, maxcor, maxiter, maxls, gtol, ftol));
+  if (P == 0) return 0;
+  TB_CUDA(cudaSetDevice(models[0]->device));
+  const int D = models[0]->D;
+  std::vector<cudaStream_t> streams(S);
+  for (int s = 0; s < S; ++s) streams[s] = models[s]->stream;
+  tb::Events ev;
+  TB_TRY(ev.create(S + 1));
+  // problem p = r * S + s: model s, box s, group s; each group's rounds see exactly the points tb_acq_maximize on model s alone
+  // would evaluate from the starts [R, s, D]
+  auto eval = [&](const double* xt, const int*, int, double* vals, double* grad, const int* group_n) -> int {
+    return tb::fork_join(streams[0], streams.data(), S, group_n, ev, [&](int s, int64_t o, int n) -> int {
+      tb::EvalRequest rq;
+      rq.acq = kind[s];
+      rq.pen = pen[s] != 0;
+      rq.param = param[s];
+      rq.Xc = xt + o * D;
+      rq.M = n;
+      rq.out_vals = vals + o;
+      rq.out_grad = grad + o * D;
+      rq.sync = false;
+      return tb::run_eval(models[s], rq);
+    });
+  };
+  TB_TRY(tb::lbfgs_run(who.c_str(), streams[0], D, lower, upper, S, S, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval, x_out,
+                       f_out, success, nfev));
+  for (int s = 0; s < S; ++s) TB_TRY(tb::profile_fold(models[s]));  // lbfgs_run's last synchronise joined every stream
+  return 0;
+}
+
+int tb_rff_maximize_models(tb_rff* const* r, int S, const double* lower, const double* upper, const double* starts, int64_t R,
+                           int maxcor, int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out,
+                           int32_t* success, int64_t* nfev) {
+  const std::string who = "tb_rff_maximize_models";
+  TB_CHECK(r && lower && upper, who + ": null argument");
+  TB_CHECK(S >= 1, who + ": the number of trajectory handles must be at least 1, got " + std::to_string(S));
+  for (int s = 0; s < S; ++s) {
+    TB_CHECK(r[s], who + ": null trajectory handle " + std::to_string(s));
+    for (int j = 0; j < s; ++j) TB_CHECK(r[j] != r[s], who + ": the same trajectory handle appears twice");
+    TB_TRY(tb::check_rff_paired(r[s], who.c_str()));
+    TB_CHECK(r[s]->device == r[0]->device, who + ": the trajectory handles must be on one device");
+    TB_CHECK(r[s]->D == r[0]->D, who + ": the trajectory handles must have one input dimension");
+    TB_CHECK(r[s]->nb == r[0]->nb, who + ": every handle must hold the same number of trajectories, got " +
+                                       std::to_string(r[s]->nb) + " and " + std::to_string(r[0]->nb));
+  }
+  const int k = r[0]->nb, V = k * S;
+  TB_CHECK(R >= 0 && R < ((int64_t)1 << 31) / V, who + ": number of starts out of range");
+  const int64_t P = R * V;
+  TB_TRY(tb::check_starts(who, P, starts, x_out, f_out, success, nfev, maxcor, maxiter, maxls, gtol, ftol));
+  if (P == 0) return 0;
+  TB_CUDA(cudaSetDevice(r[0]->device));
+  const int D = r[0]->D;
+  std::vector<cudaStream_t> streams(S);
+  for (int s = 0; s < S; ++s) streams[s] = r[s]->stream;
+  tb::Events ev;
+  TB_TRY(ev.create(S + 1));
+  tb::DevBuf btraj;
+  TB_TRY(btraj.reserve(sizeof(int) * (size_t)P));
+  int* traj = btraj.as<int>();
+  // problem p = i * V + v: trajectory v / S of handle v % S, box v % S, group v % S = p % S
+  auto eval = [&](const double* xt, const int* idx, int n, double* vals, double* grad, const int* group_n) -> int {
+    tb::lb::lbfgs_traj_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, streams[0]>>>(idx, n, V, S, traj);
+    TB_LAUNCHED();
+    return tb::fork_join(streams[0], streams.data(), S, group_n, ev, [&](int s, int64_t o, int ns) -> int {
+      for (int64_t c0 = 0; c0 < ns; c0 += tb::RFF_PAIRED_CHUNK) {
+        const int64_t mc = std::min<int64_t>(tb::RFF_PAIRED_CHUNK, ns - c0);
+        TB_TRY(tb::launch_rff_paired(r[s], xt + (o + c0) * D, mc, 0, traj + o + c0, -1.0, vals + o + c0, grad + (o + c0) * D));
+      }
+      return 0;
+    });
+  };
+  return tb::lbfgs_run(who.c_str(), streams[0], D, lower, upper, S, S, starts, P, maxcor, maxiter, maxls, gtol, ftol, eval, x_out,
+                       f_out, success, nfev);
 }
 
 int tb_gp_covariance_between_points(tb_gp* gp, const void* X1, int64_t M1, const void* X2, int64_t M2, void* out) {
@@ -3291,7 +3442,7 @@ int tb_ehvi_maximize(tb_ehvi* h, const double* lower, const double* upper, const
   TB_TRY(tb::ehvi_check(h, "tb_ehvi_maximize"));
   if (P == 0) return 0;
   TB_CUDA(cudaSetDevice(h->device));
-  auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad) -> int {
+  auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad, const int*) -> int {
     tb::EvalRequest rq;
     rq.Xc = xt;
     rq.M = n;
@@ -3299,7 +3450,7 @@ int tb_ehvi_maximize(tb_ehvi* h, const double* lower, const double* upper, const
     rq.out_grad = grad;
     return tb::ehvi_run(h, rq);
   };
-  return tb::lbfgs_run("tb_ehvi_maximize", h->m[0]->stream, h->D, lower, upper, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol,
+  return tb::lbfgs_run("tb_ehvi_maximize", h->m[0]->stream, h->D, lower, upper, 1, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol,
                        eval, x_out, f_out, success, nfev);
 }
 

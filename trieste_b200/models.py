@@ -10,6 +10,7 @@ meaning and output shape.  All arithmetic runs on the GPU behind the C-ABI; arra
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import math
 from typing import Optional, Tuple
@@ -115,6 +116,16 @@ class GaussianProcessRegression:
             except Exception:  # pragma: no cover
                 pass
             self._h = None
+
+    def __deepcopy__(self, memo):
+        """A model with its own device handle, data, hyper-parameters, engine and posterior cache (``copy_to_local_models``
+        conditions each copy on its own local data)."""
+        new = GaussianProcessRegression(copy.deepcopy(self._spec, memo), self._device, self._num_rff_features,
+                                        self._use_decoupled_sampler)
+        memo[id(self)] = new
+        if hasattr(self, "_engine"):
+            new.set_engine(self._engine)
+        return new
 
     @property
     def handle(self) -> C.c_void_p:

@@ -1,11 +1,13 @@
 """Acquisition rules — mirrors trieste/acquisition/rule.py (``EfficientGlobalOptimization`` :209-399,
 ``DiscreteThompsonSampling`` :879-994, and the box trust regions: ``SingleObjectiveTrustRegionBox`` / ``TREGOBox`` /
 ``TURBOBox`` :1569-2218 with ``BatchTrustRegionBox`` :1261-1566, 1863-1920).  Rules are per-BO-step orchestration on the
-host; each region's acquisition runs through the same device paths as a plain ``Box``.  Local models and datasets
-(``LocalizedTag``), discrete, product and categorical regions and the asynchronous rules are out of scope."""
+host; each region's acquisition runs through the same device paths as a plain ``Box``.  Regions may have local models and
+datasets (``LocalizedTag``, rule.py:1099-1232, 1364-1435, 1501-1566); discrete, product and categorical regions and the
+asynchronous rules are out of scope."""
 from __future__ import annotations
 
 import copy
+from collections import Counter
 from typing import Mapping, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -23,6 +25,7 @@ from .acquisition.optimizer import automatic_optimizer_selector, batchify_joint,
 from .acquisition.sampler import ExactThompsonSampler, ThompsonSamplerFromTrajectory  # noqa: F401
 from .data import Dataset
 from .space import Box, SearchSpace, TaggedMultiSearchSpace
+from .utils import LocalizedTag
 
 
 class EfficientGlobalOptimization:
@@ -39,6 +42,7 @@ class EfficientGlobalOptimization:
             optimizer = automatic_optimizer_selector
         if isinstance(builder, (SingleModelAcquisitionBuilder, SingleModelGreedyAcquisitionBuilder)):
             builder = builder.using(OBJECTIVE)
+        base_optimizer = optimizer  # before batchify: BatchTrustRegionBox's batched local-model route vectorises it itself
         if num_query_points > 1:  # rule.py:291-301
             if isinstance(builder, VectorizedAcquisitionFunctionBuilder):
                 optimizer = batchify_vectorize(optimizer, num_query_points)  # batch elements optimised independently
@@ -46,6 +50,7 @@ class EfficientGlobalOptimization:
                 optimizer = batchify_joint(optimizer, num_query_points)  # ... jointly over space ** q
             # a GreedyAcquisitionFunctionBuilder collects the batch sequentially in acquire()
         self._builder = builder
+        self._base_optimizer = base_optimizer
         self._optimizer = optimizer
         self._num_query_points = num_query_points
         self._acquisition_function = None
@@ -119,7 +124,7 @@ class DiscreteThompsonSampling:
 # box trust regions (rule.py:1039-1236, 1569-2218)
 # ---------------------------------------------------------------------------------------------------
 def _objective_dataset(datasets: Optional[Mapping[str, Dataset]]) -> Dataset:
-    if datasets is None or len(datasets) != 1 or next(iter(datasets)) != OBJECTIVE:
+    if datasets is None or len(datasets) != 1 or LocalizedTag.from_tag(next(iter(datasets))).global_tag != OBJECTIVE:
         raise ValueError("a single OBJECTIVE dataset must be provided")
     return next(iter(datasets.values()))
 
@@ -152,6 +157,45 @@ class UpdatableTrustRegionBox(Box):
         lower = np.maximum(self.global_search_space.lower, self.location - eps)
         upper = np.minimum(self.global_search_space.upper, self.location + eps)
         return lower, upper
+
+    def _get_tags(self, tags):
+        """rule.py:1099-1114: (global parts of this region's local tags, global tags without a local tag here)."""
+        local_gtags, global_tags = set(), set()
+        for tag in tags:
+            ltag = LocalizedTag.from_tag(tag)
+            if not ltag.is_local:
+                global_tags.add(tag)
+            elif ltag.local_index == self.region_index:
+                local_gtags.add(ltag.global_tag)
+        return local_gtags, global_tags - local_gtags
+
+    def select_in_region(self, mapping):
+        """rule.py:1177-1206: the items of this region — for each tag its local item of this region's index, else the
+        global one (only the global items without an index); None when there are none."""
+        if mapping is None:
+            _mapping = {}
+        elif self.region_index is None:
+            _mapping = {tag: item for tag, item in mapping.items() if not LocalizedTag.from_tag(tag).is_local}
+        else:
+            local_gtags, global_tags = self._get_tags(set(mapping))
+            _mapping = {}
+            for tag in local_gtags:
+                ltag = LocalizedTag(tag, self.region_index)
+                _mapping[ltag] = mapping[ltag]
+            for tag in global_tags:
+                _mapping[tag] = mapping[tag]
+        return _mapping if _mapping else None
+
+    def get_datasets_filter_mask(self, datasets):
+        """rule.py:1208-1232: for each of this region's local datasets, the mask of its points inside the region."""
+        assert self.region_index is not None, "the region_index should be set for filtering local datasets"
+        if datasets is None:
+            return None
+        return {
+            tag: self.contains(np.asarray(dataset.query_points))
+            for tag, dataset in datasets.items()
+            if LocalizedTag.from_tag(tag).local_index == self.region_index
+        }
 
 
 class SingleObjectiveTrustRegionBox(UpdatableTrustRegionBox):
@@ -197,7 +241,7 @@ class SingleObjectiveTrustRegionBox(UpdatableTrustRegionBox):
         self._initialized = True
 
     def update(self, models=None, datasets: Optional[Mapping[str, Dataset]] = None) -> None:
-        x_min, y_min = self.get_dataset_min(datasets)
+        x_min, y_min = self.get_dataset_min(self.select_in_region(datasets))
         tr_volume = np.prod(self.upper - self.lower)
         self._step_is_success = bool(y_min < self._y_min - self._kappa * tr_volume)
         self.eps = self.eps / self._beta if self._step_is_success else self.eps * self._beta
@@ -257,6 +301,17 @@ class TREGOBox(SingleObjectiveTrustRegionBox):
         dataset = _objective_dataset(datasets)
         return self.get_values_min(dataset.query_points, dataset.observations, in_region_only=False)
 
+    def get_datasets_filter_mask(self, datasets):
+        """rule.py:2003-2020: TREGO keeps its whole local dataset."""
+        assert self.region_index is not None, "the region_index should be set for filtering local datasets"
+        if datasets is None:
+            return None
+        return {
+            tag: np.ones(np.asarray(dataset.query_points).shape[:-1], dtype=bool)
+            for tag, dataset in datasets.items()
+            if LocalizedTag.from_tag(tag).local_index == self.region_index
+        }
+
 
 class TURBOBox(UpdatableTrustRegionBox):
     """rule.py:2038-2218 (TuRBO, Eriksson et al. 2019): a box of side ``L`` centred on the best observation, stretched
@@ -298,7 +353,7 @@ class TURBOBox(UpdatableTrustRegionBox):
                 f"{self.success_tolerance!r}, {self.failure_tolerance!r}, {self.region_index!r})")
 
     def _set_tr_width(self, models=None) -> None:
-        if models is None or len(models) != 1 or next(iter(models)) != OBJECTIVE:
+        if models is None or len(models) != 1 or LocalizedTag.from_tag(next(iter(models))).global_tag != OBJECTIVE:
             raise ValueError("a single OBJECTIVE model must be provided")
         model = next(iter(models.values()))
         D = self.global_search_space.dimension
@@ -310,15 +365,15 @@ class TURBOBox(UpdatableTrustRegionBox):
         self.upper = np.minimum(self.global_search_space.upper, self.location + self.tr_width / 2.0)
 
     def initialize(self, models=None, datasets: Optional[Mapping[str, Dataset]] = None) -> None:
-        x_min, self.y_min = self.get_dataset_min(datasets)
+        x_min, self.y_min = self.get_dataset_min(self.select_in_region(datasets))
         self.location = x_min
         self.L, self.failure_counter, self.success_counter = self.L_init, 0, 0
-        self._set_tr_width(models)
+        self._set_tr_width(self.select_in_region(models))
         self._update_domain()
         self._initialized = True
 
     def update(self, models=None, datasets: Optional[Mapping[str, Dataset]] = None) -> None:
-        x_min, y_min = self.get_dataset_min(datasets)
+        x_min, y_min = self.get_dataset_min(self.select_in_region(datasets))
         self.location = x_min
         step_is_success = y_min < self.y_min - 1e-10
         self.y_min = y_min
@@ -333,7 +388,7 @@ class TURBOBox(UpdatableTrustRegionBox):
         self.L = min(self.L, self.L_max)
         if self.L < self.L_min:  # too small: start again
             self.L, self.failure_counter, self.success_counter = self.L_init, 0, 0
-        self._set_tr_width(models)
+        self._set_tr_width(self.select_in_region(models))
         self._update_domain()
 
     def get_dataset_min(self, datasets: Optional[Mapping[str, Dataset]]) -> Tuple[np.ndarray, float]:
@@ -355,12 +410,21 @@ def get_unique_points_mask(points: np.ndarray, tolerance: float = 1e-6) -> np.nd
 class BatchTrustRegionBox:
     """rule.py:1261-1566, 1863-1920: one query batch per trust region, the regions updated from the data between steps.
 
-    The rule keeps its regions: the first ``acquire`` initialises them (the reference's first ``filter_datasets``);
-    every later call first updates them from the datasets it receives — re-initialising regions that have shrunk below
-    their minimum size or share a centre with an earlier region — and then acquires.  With an
-    ``EfficientGlobalOptimization`` base rule the acquisition runs once over a ``TaggedMultiSearchSpace`` of the
-    regions, column v of a vectorised function searching region v mod S; any other base rule is deep-copied once per
-    region and run inside it.  ``acquire`` returns the [q, S, D] points flattened to [q * S, D]."""
+    The rule keeps its regions.  With global models and datasets only, the first ``acquire`` initialises them (the
+    reference's first ``filter_datasets``) and every later call first updates them from the datasets it receives —
+    re-initialising regions that have shrunk below their minimum size or share a centre with an earlier region — and then
+    acquires.  With local datasets (``LocalizedTag``, see ``with_local_datasets``) ``filter_datasets`` updates the regions
+    and ``acquire`` only acquires, as in the reference.
+
+    With an ``EfficientGlobalOptimization`` base rule and global models the acquisition runs once over a
+    ``TaggedMultiSearchSpace`` of the regions, column v of a vectorised function searching region v mod S.  Otherwise the
+    base rule is deep-copied once per region and each copy acquires inside its region with that region's models and
+    datasets under their global tags.  With local models, an ``EfficientGlobalOptimization`` base rule whose builder is
+    not greedy and region functions that all maximise on the device (a fused single-query function on a model of its
+    own, or the negated trajectories of ``ParallelContinuousThompsonSampling``), the regions' functions are stacked into
+    one function over V = k * S columns and the base optimiser runs once over the regions, every region's L-BFGS in one
+    device call (``tb_acq_maximize_models`` / ``tb_rff_maximize_models``).  ``acquire`` returns the [q, S, D] points
+    flattened to [q * S, D]."""
 
     def __init__(self, init_subspaces: Union[None, UpdatableTrustRegionBox, Sequence[UpdatableTrustRegionBox]] = None,
                  rule=None):
@@ -376,6 +440,7 @@ class BatchTrustRegionBox:
         self._rule = rule
         self._rules = None  # one deep copy of the base rule per region, when the base rule is run per region
         self._subspaces: Optional[Tuple[UpdatableTrustRegionBox, ...]] = None  # the current regions
+        self._filtered = {}  # the local datasets of the last filter_datasets
 
     def __repr__(self) -> str:
         return f"BatchTrustRegionBox({self._init_subspaces!r}, {self._rule!r})"
@@ -424,6 +489,38 @@ class BatchTrustRegionBox:
                 subspace.update(models, datasets)
         self.maybe_initialize_subspaces(self._subspaces, models, datasets)
 
+    def filter_datasets(self, models, datasets):
+        """rule.py:1501-1566: update the regions from ``datasets`` (as ``update_subspaces``), then keep the points of each
+        local dataset that lie inside its own region (TREGO keeps them all); global datasets pass through unchanged.
+
+        Deviation: a local dataset that filtering would leave empty (a region re-initialised away from all of its
+        points) keeps the dataset it had after the previous filtering — the first time, the one it was given — so its
+        model stays as it is.  The reference conditions that region's GPR on no data and searches it under the prior;
+        the device GPR needs at least one point."""
+        self.update_subspaces(models, datasets)
+        used_masks = {
+            tag: np.zeros(np.asarray(dataset.query_points).shape[:-1], dtype=bool)
+            for tag, dataset in datasets.items()
+            if LocalizedTag.from_tag(tag).is_local
+        }
+        for subspace in self._subspaces:
+            in_region_masks = subspace.get_datasets_filter_mask(datasets)
+            for tag, in_region in (in_region_masks or {}).items():
+                used_masks[tag] = used_masks[tag] | np.asarray(in_region, dtype=bool)
+        filtered = {}
+        for tag, used_mask in used_masks.items():
+            dataset = datasets[tag]
+            if used_mask.any():
+                filtered[tag] = Dataset(np.asarray(dataset.query_points)[used_mask],
+                                        np.asarray(dataset.observations)[used_mask])
+            else:
+                filtered[tag] = self._filtered.get(tag, dataset)
+        self._filtered = dict(filtered)
+        for tag, dataset in datasets.items():
+            if not LocalizedTag.from_tag(tag).is_local:
+                filtered[tag] = dataset
+        return filtered
+
     def acquire(self, search_space: SearchSpace, models: Mapping[str, object],
                 datasets: Optional[Mapping[str, Dataset]] = None) -> np.ndarray:
         for subspace in self._init_subspaces or ():
@@ -441,14 +538,160 @@ class BatchTrustRegionBox:
                 self._rule = DiscreteThompsonSampling(min(100 * search_space.dimension, 5000), 1)
             else:
                 self._rule = EfficientGlobalOptimization()
-        if self._rules is None and not isinstance(self._rule, EfficientGlobalOptimization):
+        num_local_models = Counter(
+            LocalizedTag.from_tag(tag).global_tag for tag in models if LocalizedTag.from_tag(tag).is_local
+        )
+        num_local_models_vals = set(num_local_models.values())
+        if len(num_local_models_vals) > 1:
+            raise ValueError(f"The number of local models should be the same for all tags, got {num_local_models}")
+        _num_local_models = sum(num_local_models_vals)
+        num_subspaces = len(self._tags)
+        if _num_local_models not in (0, num_subspaces):
+            raise ValueError(
+                f"When using local models, the number of subspaces {num_subspaces} should be equal to the number of "
+                f"local models {_num_local_models}"
+            )
+        if self._rules is None and not (_num_local_models == 0 and isinstance(self._rule, EfficientGlobalOptimization)):
             self._rules = [copy.deepcopy(self._rule) for _ in self._tags]
-        self.update_subspaces(models, datasets)
+        local_data = any(LocalizedTag.from_tag(tag).is_local for tag in (datasets or {}))
+        if not (local_data or _num_local_models) or self._subspaces is None:
+            self.update_subspaces(models, datasets)  # with local data, filter_datasets has updated the regions
         subspaces = self._subspaces
         if self._rules is not None:
-            points = np.stack([rule.acquire(subspace, models, datasets) for subspace, rule in zip(subspaces, self._rules)],
-                              axis=1)
+            per_region = [
+                (_global_tags(subspace.select_in_region(models)), _global_tags(subspace.select_in_region(datasets)))
+                for subspace in subspaces
+            ]
+            if _num_local_models and isinstance(self._rule, EfficientGlobalOptimization) and not isinstance(
+                self._rule._builder, GreedyAcquisitionFunctionBuilder
+            ):
+                points = self._acquire_local_ego(subspaces, per_region)
+            else:
+                points = np.stack([rule.acquire(subspace, m, d) for subspace, rule, (m, d)
+                                   in zip(subspaces, self._rules, per_region)], axis=1)
         else:
-            points = self._rule.acquire(TaggedMultiSearchSpace(subspaces, self._tags), models, datasets)
+            global_datasets = None if datasets is None else {
+                tag: dataset for tag, dataset in datasets.items() if not LocalizedTag.from_tag(tag).is_local
+            }
+            points = self._rule.acquire(TaggedMultiSearchSpace(subspaces, self._tags), models, global_datasets)
         points = np.asarray(points).reshape(-1, len(subspaces), points.shape[-1])  # [q, S, D]
         return points.reshape(-1, points.shape[-1])
+
+    def _acquire_local_ego(self, subspaces, per_region) -> np.ndarray:
+        """EfficientGlobalOptimization.acquire of every region's copy (a builder that is not greedy), with the
+        maximisation batched over the regions when their functions allow it (``_RegionStack``).  Returns [q, S, D]."""
+        functions = []
+        for rule, (models, datasets) in zip(self._rules, per_region):
+            if rule._acquisition_function is None:
+                rule._acquisition_function = rule._builder.prepare_acquisition_function(models, datasets=datasets)
+            else:
+                rule._acquisition_function = rule._builder.update_acquisition_function(
+                    rule._acquisition_function, models, datasets=datasets
+                )
+            functions.append(rule._acquisition_function)
+        k = self._rule._num_query_points
+        stack = _RegionStack.of(functions, k)
+        if stack is None:
+            return np.stack([rule._optimizer(subspace, fn) for subspace, rule, fn in zip(subspaces, self._rules, functions)],
+                            axis=1)
+        S = len(subspaces)
+        points = self._rule._base_optimizer(TaggedMultiSearchSpace(subspaces, self._tags), (stack, k * S))  # [k * S, D]
+        return np.asarray(points).reshape(k, S, -1)
+
+
+def _global_tags(mapping):
+    """rule.py:1422-1432: a region's items under their global tags (single-model builders expect OBJECTIVE)."""
+    if mapping is None:
+        return None
+    return {LocalizedTag.from_tag(tag).global_tag: item for tag, item in mapping.items()}
+
+
+class _RegionStack:
+    """S regions' acquisition functions as one function vectorised over V = k * S columns: column v is column v // S of
+    region v % S's function, searched inside region v % S (the round robin of a ``TaggedMultiSearchSpace``).  Values and
+    gradients call each region's function on its own columns.  ``maximize_from`` runs every region's multi-start L-BFGS in
+    one device call: ``tb_acq_maximize_models`` for fused single-query functions (k = 1) on S distinct model handles,
+    ``tb_rff_maximize_models`` for the negated trajectories of S distinct trajectory handles of k trajectories each."""
+
+    def __init__(self, functions, k: int, kind: str):
+        self._fns = list(functions)
+        self._S = len(self._fns)
+        self._k = k
+        self._kind = kind
+
+    @staticmethod
+    def of(functions, k: int):
+        """The stack of ``functions``, or None when some function cannot be maximised this way."""
+        from .acquisition.function import _FusedSingleQuery
+
+        if k == 1 and all(isinstance(f, _FusedSingleQuery)
+                          and type(f)._native_maximize is _FusedSingleQuery._native_maximize for f in functions):
+            handles = {f._model.handle.value for f in functions}
+            if len(handles) == len(functions) and len({f._model.dtype for f in functions}) == 1:
+                return _RegionStack(functions, k, "acq")
+        if all(hasattr(f, "minimize_from") and hasattr(f, "maximize_from") for f in functions):
+            if len({f._h.value for f in functions}) == len(functions):
+                return _RegionStack(functions, k, "rff")
+        return None
+
+    def _columns(self, x, s):
+        return x[..., s::self._S, :]
+
+    def __call__(self, x):
+        x = np.asarray(x)
+        out = np.empty(x.shape[:-1])
+        for s, f in enumerate(self._fns):
+            out[..., s::self._S] = np.asarray(f(self._columns(x, s))).reshape(out[..., s::self._S].shape)
+        return out
+
+    def value_and_gradient(self, x):
+        x = np.asarray(x)
+        vals, grads = np.empty(x.shape[:-1]), np.empty(x.shape)
+        for s, f in enumerate(self._fns):
+            v, g = f.value_and_gradient(self._columns(x, s))
+            vals[..., s::self._S] = np.asarray(v).reshape(vals[..., s::self._S].shape)
+            grads[..., s::self._S, :] = np.asarray(g).reshape(grads[..., s::self._S, :].shape)
+        return vals, grads
+
+    def maximize_from(self, starts, lower, upper, *, maxcor: int = 10, maxiter: int = 15000, maxls: int = 20,
+                      gtol: float = 1e-5, ftol: float = 2.220446049250313e-09):
+        """starts [R, V, D] ([P, D] when V = 1), one box [D] or the regions' boxes [S, D] -> (success, maximised values,
+        x, nfev) shaped like the starts without their last axis."""
+        import ctypes as C
+
+        from . import _lib
+
+        x0 = np.asarray(starts, dtype=np.float64)
+        flat = x0.ndim == 2
+        if flat:
+            x0 = x0[:, None, :]
+        x0 = np.ascontiguousarray(x0)
+        R, V, D = x0.shape
+        S = self._S
+        if V != self._k * S:
+            raise ValueError(f"starts must have {self._k * S} columns, got {V}")
+        lo, up = (np.ascontiguousarray(np.broadcast_to(np.atleast_2d(np.asarray(b, dtype=np.float64)), (S, D)))
+                  for b in (lower, upper))
+        x, f = np.empty((R, V, D)), np.empty((R, V))
+        ok, nfev = np.zeros((R, V), dtype=np.int32), np.zeros((R, V), dtype=np.int64)
+        tail = (int(maxcor), int(maxiter), int(maxls), float(gtol), float(ftol), x.ctypes.data, f.ctypes.data,
+                ok.ctypes.data, nfev.ctypes.data)
+        if self._kind == "acq":
+            for fn in self._fns:
+                fn._before_call()
+                fn._model._check_dim(x0)
+            handles = (C.c_void_p * S)(*[fn._model.handle.value for fn in self._fns])
+            acq = np.array([fn._acq for fn in self._fns], dtype=np.int32)
+            param = np.array([fn._param for fn in self._fns], dtype=np.float64)
+            _lib.check(_lib.lib().tb_acq_maximize_models(handles, acq.ctypes.data, param.ctypes.data, S, lo.ctypes.data,
+                                                         up.ctypes.data, x0.ctypes.data, R, *tail))
+        else:
+            for s, fn in enumerate(self._fns):
+                fn._model._check_dim(x0)
+                fn._batch(x0[:1, s::S])  # fixes the batch size k and draws the weights on first use
+            handles = (C.c_void_p * S)(*[fn._h.value for fn in self._fns])
+            _lib.check(_lib.lib().tb_rff_maximize_models(handles, S, lo.ctypes.data, up.ctypes.data, x0.ctypes.data, R,
+                                                         *tail))
+        if flat:
+            return ok[:, 0].astype(bool), f[:, 0], x[:, 0, :], nfev[:, 0]
+        return ok.astype(bool), f, x, nfev
