@@ -33,6 +33,7 @@ extern "C" {
 typedef struct tb_gp tb_gp;   /* exact-GPR posterior: owns device copies of X, Linv, alpha, hyper-params */
 typedef struct tb_rff tb_rff; /* random-Fourier-feature trajectory: owns W, b, theta */
 typedef struct tb_ehvi tb_ehvi; /* expected hypervolume improvement over L borrowed tb_gp handles: owns the partition cells */
+typedef struct tb_reduce tb_reduce; /* sum / product / softplus of single-query acquisitions over n borrowed tb_gp handles */
 
 enum tb_status {
   TB_OK = 0,
@@ -319,6 +320,35 @@ int tb_ehvi_argmax(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* best_
 int tb_ehvi_maximize(tb_ehvi* h, const double* lower, const double* upper, const double* starts, int64_t P, int maxcor,
                      int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
                      int64_t* nfev);
+
+/* ---- reducers over single-query acquisitions of several GPs -----------------------------------
+ * Sum / Product / MakePositive (acquisition/combination.py, function/function.py:1914-1990) over T terms, each a fused
+ * single-query kind on one of n distinct borrowed handles: value = v_0 + ... + v_{T-1}, v_0 * ... * v_{T-1} (in term order,
+ * as tf.add_n / tf.reduce_prod over the children) or log(1 + exp(v_0)) (T = 1).  Each distinct handle runs its predict once
+ * per chunk, however many terms use it.  tb_reduce_create borrows the handles (they must outlive the object): 1 <= n <= 8,
+ * distinct handles with data, on one device, with one dtype and one input dimension D; TB_ERR_INVALID otherwise. */
+enum tb_reduce_op { TB_REDUCE_SUM = 0, TB_REDUCE_PRODUCT = 1, TB_REDUCE_SOFTPLUS = 2 };
+int tb_reduce_create(tb_reduce** out, tb_gp* const* models, int n);
+int tb_reduce_destroy(tb_reduce* h);
+/* the terms of every later call: op (tb_reduce_op), 1 <= T <= 8 (T == 1 for the softplus); term t is kind acq[t] with
+ * parameter param[t] on handle member[t] (0 <= member[t] < n).  The kinds are EI, log-EI, PBT, NegLCB, LCB, AEI, MES, the
+ * two feasibility kinds, BALD and predictive variance; the feasibility kinds take alpha[t] > 0 (finite) as their alpha, the
+ * other kinds ignore alpha[t] (alpha may be null when no term is a feasibility kind).  AEI reads its handle's noise, MES
+ * its handle's min-value samples (tb_acq_set_min_value_samples) at each call.  Setting the terms the object already holds
+ * does nothing.  TB_ERR_INVALID for a bad op, T, member index, kind (GIBBON, penalised and unknown kinds are refused) or
+ * parameter; the terms held before then stay. */
+int tb_reduce_set_terms(tb_reduce* h, int op, int T, const int* member, const int* acq, const double* param,
+                        const double* alpha);
+/* Xc [M, D] -> out [M]; grad (nullable) [M, D].  The members' dtype, host or device pointers.  TB_ERR_INVALID, before
+ * anything is launched, if the terms are not set, a member's posterior cache is not built, or an MES term's handle has
+ * no min-value samples. */
+int tb_reduce_eval(tb_reduce* h, const void* Xc, int64_t M, void* out, void* grad);
+/* tb_acq_argmax's contract for the reduction: first-max index and value over Xc [M, D] (NaN never wins); out [M] nullable. */
+int tb_reduce_argmax(tb_reduce* h, const void* Xc, int64_t M, void* out, void* best_value, int64_t* best_index);
+/* tb_acq_maximize's contract for the reduction: the device multi-start L-BFGS inside the box [lower, upper] ([D]). */
+int tb_reduce_maximize(tb_reduce* h, const double* lower, const double* upper, const double* starts, int64_t P, int maxcor,
+                       int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
+                       int64_t* nfev);
 
 /* ---- instrumentation (bench / tests) ---------------------------------------------------------
  * kernels launched by this library in this process since the last reset; device time (ms) of the

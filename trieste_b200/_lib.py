@@ -76,6 +76,12 @@ SIGNATURES = {
     "tb_ehvi_eval": (_i32, [_vp, _vp, _i64, _vp, _vp]),
     "tb_ehvi_argmax": (_i32, [_vp, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
     "tb_ehvi_maximize": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
+    "tb_reduce_create": (_i32, [C.POINTER(_vp), C.POINTER(_vp), _i32]),
+    "tb_reduce_destroy": (_i32, [_vp]),
+    "tb_reduce_set_terms": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "tb_reduce_eval": (_i32, [_vp, _vp, _i64, _vp, _vp]),
+    "tb_reduce_argmax": (_i32, [_vp, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
+    "tb_reduce_maximize": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _vp, _vp, _vp, _vp]),
     "tb_gp_kinv_apply": (_i32, [_vp, _vp, _i32, _vp]),
     "tb_launch_count": (_i64, []),
     "tb_launch_count_reset": (None, []),

@@ -6,6 +6,7 @@ from .active_learning import (  # noqa: F401
     bichon_ranjan_criterion,
     predictive_variance,
 )
+from .combination import Product, Reducer, Sum  # noqa: F401
 from .continuous_thompson_sampling import (  # noqa: F401
     GreedyContinuousThompsonSampling,
     ParallelContinuousThompsonSampling,
@@ -20,6 +21,7 @@ from .function import (  # noqa: F401
     GIBBON,
     GibbonAcquisition,
     LogExpectedImprovement,
+    MakePositive,
     MinValueEntropySearch,
     MonteCarloExpectedImprovement,
     MultipleOptimismNegativeLowerConfidenceBound,

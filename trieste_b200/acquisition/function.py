@@ -552,6 +552,36 @@ class NegativeLowerConfidenceBound(SingleModelAcquisitionBuilder):
         return function  # no dependence on data (function.py:361-372)
 
 
+class MakePositive(SingleModelAcquisitionBuilder):
+    """function.py:1914-1990: ``log(1 + exp(f))`` of the base builder's function f, so that every value is positive (as
+    local penalisation needs of its base function).  Over a fused single-query function it runs on the device as a
+    one-term reduction (acquisition/combination.py), with ``value_and_gradient``, ``fused_argmax`` and ``maximize_from``;
+    over any other function with ``value_and_gradient`` the gradient is sigmoid(f) times the base gradient."""
+
+    def __init__(self, base_acquisition_function_builder: SingleModelAcquisitionBuilder) -> None:
+        self._base_builder = base_acquisition_function_builder
+
+    def __repr__(self) -> str:
+        return f"MakePositive({self._base_builder})"
+
+    def _wrap(self):
+        from .combination import REDUCE_SOFTPLUS, _softplus, reduce_functions
+
+        return reduce_functions(REDUCE_SOFTPLUS, lambda inputs: _softplus(inputs[0]), (self._base_function,))
+
+    def prepare_acquisition_function(self, model, dataset: Optional[Dataset] = None):
+        self._base_function = self._base_builder.prepare_acquisition_function(model, dataset)
+        return self._wrap()
+
+    def update_acquisition_function(self, function, model, dataset: Optional[Dataset] = None):
+        """function.py:1967-1990: the same function when the base builder updated its function in place."""
+        up_fn = self._base_builder.update_acquisition_function(self._base_function, model, dataset)
+        if up_fn is self._base_function:
+            return function
+        self._base_function = up_fn
+        return self._wrap()
+
+
 class multiple_optimism_lower_confidence_bound(AcquisitionFunctionClass):
     """function.py:1857-1911 (MOLCB, Torossian et al. 2020): a VECTORISED function ``[..., B, D] -> [..., B]``; column b is
     the negated lower confidence bound ``-mean + beta_b sqrt(var)`` with ``beta_b = 5 d Phi^-1(0.5 + 0.5 b / (B + 1))``, b = 1..B,

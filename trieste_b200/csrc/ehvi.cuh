@@ -28,20 +28,10 @@
 
 namespace tb {
 
-constexpr int EHVI_LMAX = 8;
+constexpr int EHVI_LMAX = MEMBERS_MAX;
 constexpr int EHVI_TILE = 64;  // cells per shared-memory tile
 constexpr double EHVI_CLIP = 1e10;  // multi_objective.py:215
 constexpr double HIPPO_WARP = 0.63661977236758134308;  // 2 / pi, multi_objective.py:755
-
-// the chunk outputs of the L member handles, as the tail reads them
-struct EhviMembers {
-  const double* partial[EHVI_LMAX];  // variance sums of squares over G row-block groups, stride McPad
-  const double* mean[EHVI_LMAX];
-  double* dmv[EHVI_LMAX];  // gradient path: d/dmean [Mc] then d/dvar [Mc] (the member's sMisc); null without a gradient
-  int64_t McPad[EHVI_LMAX];
-  int G[EHVI_LMAX];
-  double variance[EHVI_LMAX];
-};
 
 // HIPPO's penalty state: the pending points' stack moments, P >= 1 when a PEN kernel reads it
 struct EhviPenalty {
@@ -76,7 +66,7 @@ __device__ __forceinline__ double ehvi_factor(double a, double b, double m, doub
 // (NaN never wins) of (value, idx0 + t).  pen is read only with PEN.
 template <int L, bool GRAD, bool PEN>
 __global__ void __launch_bounds__(256)
-ehvi_kernel(const EhviMembers mb, const EhviPenalty pen, const double* __restrict__ cells, int64_t K, int64_t Mc, int64_t idx0,
+ehvi_kernel(const ChunkMembers mb, const EhviPenalty pen, const double* __restrict__ cells, int64_t K, int64_t Mc, int64_t idx0,
             double* __restrict__ out_vals, double* __restrict__ blk_best, int64_t* __restrict__ blk_idx) {
   __shared__ double sa[EHVI_TILE * L], sb[EHVI_TILE * L];
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -182,16 +172,6 @@ ehvi_kernel(const EhviMembers mb, const EhviPenalty pen, const double* __restric
   }
   if (blk_best == nullptr) return;
   block_best_store(bv, bi, blk_best, blk_idx);
-}
-
-// out[i] = sum_l slices[l][i] in l order (the members' gradient assemblies of one chunk)
-__global__ void __launch_bounds__(256)
-ehvi_grad_sum_kernel(const double* __restrict__ slices, int L, int64_t n, double* __restrict__ out) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  double acc = slices[i];
-  for (int l = 1; l < L; ++l) acc += slices[(int64_t)l * n + i];
-  out[i] = acc;
 }
 
 }  // namespace tb

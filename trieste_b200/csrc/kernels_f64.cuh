@@ -562,6 +562,16 @@ __device__ __forceinline__ void penalty_factor(int kind, double dist, double rad
   }
 }
 
+// the value of one single-query kind at (mean, var), as the plain tail computes it (tail_kernel, reduce_kernel); the
+// GIBBON repulsion kinds read |u|^2 of candidate t from gib_uu
+__device__ __forceinline__ double kind_value(int acq, double param, double aux, const double* __restrict__ samp, int nsamp,
+                                             double mu, double var, const double* __restrict__ gib_uu, int64_t t, double gib_w) {
+  return (acq == TB_ACQ_MES) ? mes_value(samp, nsamp, mu, var)
+         : gibbon_kind(acq)  ? gibbon_value(acq, samp, nsamp, mu, var, aux, gib_uu ? gib_uu[t] : 0.0, gib_w)
+         : active_learning_kind(acq) ? active_learning_value(acq, param, aux, mu, var)
+                                     : acq_value(acq, param, aux, mu, var);
+}
+
 constexpr int PEN_TILE = 32;  // pending points per shared-memory tile of the penalised tail
 constexpr int PEN_DMAX = 32;  // largest input dimension (pick_dp)
 
@@ -607,6 +617,27 @@ __device__ __forceinline__ double chunk_raw_variance(const double* __restrict__ 
   return variance - ss;
 }
 
+// the chunk outputs of up to MEMBERS_MAX handles evaluated together (EHVI, reducers), as the combining kernels read them
+constexpr int MEMBERS_MAX = 8;
+struct ChunkMembers {
+  const double* partial[MEMBERS_MAX];  // variance sums of squares over G row-block groups, stride McPad
+  const double* mean[MEMBERS_MAX];
+  double* dmv[MEMBERS_MAX];  // gradient path: d/dmean [Mc] then d/dvar [Mc] (the member's sMisc); null without a gradient
+  int64_t McPad[MEMBERS_MAX];
+  int G[MEMBERS_MAX];
+  double variance[MEMBERS_MAX];
+};
+
+// out[i] = sum_l slices[l][i] in l order (the members' gradient assemblies of one chunk)
+__global__ void __launch_bounds__(256)
+member_grad_sum_kernel(const double* __restrict__ slices, int L, int64_t n, double* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double acc = slices[i];
+  for (int l = 1; l < L; ++l) acc += slices[(int64_t)l * n + i];
+  out[i] = acc;
+}
+
 // one thread per candidate of the chunk; block-level first-max argmax.  PEN: the value (and the gradient, when
 // pen.grad is set) is multiplied by the local penalty before the argmax.  The argmax index of candidate t is idx_map[t]
 // when idx_map is set (the compacted survivors of the screened argmax), else idx0 + t.
@@ -626,11 +657,7 @@ tail_kernel(const double* __restrict__ partial, int G, int64_t McPad, const doub
     if (out_mean) out_mean[t] = mu;
     if (out_var) out_var[t] = var;
     if (acq >= 0) {
-      double v = (acq == TB_ACQ_MES) ? mes_value(samp, nsamp, mu, var)
-                 : gibbon_kind(acq)
-                     ? gibbon_value(acq, samp, nsamp, mu, var, aux, pen.gib_uu ? pen.gib_uu[t] : 0.0, pen.gib_w)
-                 : active_learning_kind(acq) ? active_learning_value(acq, param, aux, mu, var)
-                                             : acq_value(acq, param, aux, mu, var);
+      double v = kind_value(acq, param, aux, samp, nsamp, mu, var, pen.gib_uu, t, pen.gib_w);
       if (PEN) {
         vb = v;
       } else {

@@ -6,8 +6,10 @@
 #include "batch_ei.cuh"
 #include "active_learning.cuh"
 #include "ehvi.cuh"
+#include "reduce.cuh"
 #include "int8_engines.h"
 #include <chrono>
+#include <memory>
 #include "factor.cuh"
 #include "lbfgs.cuh"
 
@@ -1461,7 +1463,7 @@ static int argmax_screened(tb_gp* gp, const EvalRequest& rq, Engine e, int64_t c
 // the others agree with it to rounding.
 struct ChunkPlan {
   int64_t chunk_cap = 0;
-  int G[EHVI_LMAX] = {};
+  int G[MEMBERS_MAX] = {};
 };
 static ChunkPlan plan_chunks(tb_gp* const* gps, const Engine* eng, int n, bool grad, int64_t M) {
   ChunkPlan p;
@@ -3168,84 +3170,76 @@ int tb_mvn_cdf(int device, const double* x, const double* mean, const double* co
 }  // extern "C"
 
 // =================================================================================================
-// expected hypervolume improvement over a stack of L handles (ehvi.cuh)
+// several handles per chunk: the members' predict on their own streams, one combining kernel (EHVI, reducers)
 // =================================================================================================
-struct tb_ehvi {
-  std::vector<tb_gp*> m;  // borrowed member handles, one per objective
-  int L = 0, D = 0, device = 0, dtype = TB_F64;
-  int64_t K = 0;          // cells; 0: not set
-  tb::DevBuf dCells;      // lower [K][L] then upper [K][L]
-  int P = 0;              // HIPPO pending points (tb_ehvi_set_penalty); 0: no penalty
-  tb::DevBuf dPen;        // their means [P][L] then standard deviations [P][L]
-  std::vector<double> hPen;  // the means and variances [2][P][L] as last set, to recognise an unchanged push
-  tb::DevBuf sXc, sVals, sGrad, sGradL;  // staged candidates, values, gradient, and the members' gradients [L][mc][D]
-  std::vector<cudaEvent_t> ev;           // ev[l] orders member l's stream against the first member's (ev[0]: the other way)
-};
-
 namespace tb {
 
-template <int L>
-static void launch_ehvi_l(bool grad, const EhviMembers& mb, const EhviPenalty& pen, const double* cells, int64_t K, int64_t mc,
-                          int64_t c0, double* vals, double* bb, int64_t* bi, cudaStream_t st) {
-  const unsigned blocks = (unsigned)((mc + 255) / 256);
-  if (pen.P > 0) {
-    if (grad)
-      ehvi_kernel<L, true, true><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
-    else
-      ehvi_kernel<L, false, true><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
-  } else if (grad) {
-    ehvi_kernel<L, true, false><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
-  } else {
-    ehvi_kernel<L, false, false><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+// the borrowed member handles of a function over several GPs, its staging buffers and the events of its chunk loop
+struct MemberSet {
+  std::vector<tb_gp*> m;  // borrowed, distinct
+  int L = 0, D = 0, device = 0, dtype = TB_F64;
+  DevBuf sXc, sVals, sGrad, sGradL;  // staged candidates, values, gradient, and the members' gradients [L][mc][D]
+  std::vector<cudaEvent_t> ev;       // ev[l] orders member l's stream against the first member's (ev[0]: the other way)
+  ~MemberSet() {
+    if (!ev.empty()) cudaSetDevice(device);
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
   }
-}
+};
 
-static int launch_ehvi(tb_ehvi* h, bool grad, const EhviMembers& mb, int64_t mc, int64_t c0, double* vals, bool argmax) {
-  tb_gp* g0 = h->m[0];
-  double* bb = argmax ? g0->sBlkBest.as<double>() : nullptr;
-  int64_t* bi = argmax ? g0->sBlkIdx.as<int64_t>() : nullptr;
-  const double* cells = h->dCells.as<double>();
-  const double* pd = h->P > 0 ? h->dPen.as<double>() : nullptr;
-  const EhviPenalty pen{pd, pd ? pd + (size_t)h->P * h->L : nullptr, h->P};
-  switch (h->L) {
-    case 2: launch_ehvi_l<2>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 3: launch_ehvi_l<3>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 4: launch_ehvi_l<4>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 5: launch_ehvi_l<5>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 6: launch_ehvi_l<6>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    case 7: launch_ehvi_l<7>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
-    default: launch_ehvi_l<8>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+// the checks of a create call on the L handles (the caller has checked L's range), then the events
+static int members_init(MemberSet* s, tb_gp* const* models, int L, const char* who) {
+  const std::string w(who);
+  for (int l = 0; l < L; ++l) {
+    TB_CHECK(models[l], w + ": null model handle");
+    TB_CHECK(models[l]->have_data, w + ": member " + std::to_string(l) + " has no data");
+    for (int j = 0; j < l; ++j) TB_CHECK(models[j] != models[l], w + ": the same model handle appears twice");
+    TB_CHECK(models[l]->device == models[0]->device, w + ": the members must be on one device");
+    TB_CHECK(models[l]->dtype == models[0]->dtype, w + ": the members must have one dtype");
+    TB_CHECK(models[l]->D == models[0]->D, w + ": the members must have one input dimension");
   }
-  TB_LAUNCHED();
-  TB_CUDA(cudaGetLastError());
+  TB_CUDA(cudaSetDevice(models[0]->device));
+  s->m.assign(models, models + L);
+  s->L = L;
+  s->D = models[0]->D;
+  s->device = models[0]->device;
+  s->dtype = models[0]->dtype;
+  s->ev.assign(L, nullptr);
+  for (int l = 0; l < L; ++l) {
+    if (cudaEventCreateWithFlags(&s->ev[l], cudaEventDisableTiming) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(w + ": cudaEventCreate failed", ERR_RUNTIME);
+    }
+  }
   return 0;
 }
 
-// what every EHVI evaluation needs of the object and its members, checked before anything is staged
-static int ehvi_check(const tb_ehvi* h, const char* who) {
-  TB_CHECK(h->K >= 1, std::string(who) + ": the partition cells are not set (tb_ehvi_set_cells)");
-  for (int l = 0; l < h->L; ++l) {
-    const tb_gp* gp = h->m[l];
+// what every evaluation needs of the members, checked before anything is staged
+static int members_check(const MemberSet* s, const char* who) {
+  for (int l = 0; l < s->L; ++l) {
+    const tb_gp* gp = s->m[l];
     TB_CHECK(gp->cache_valid, std::string(who) + ": posterior cache of member " + std::to_string(l) +
                                   " is not built: call tb_gp_update_posterior_cache first");
-    TB_CHECK(gp->D == h->D, std::string(who) + ": member " + std::to_string(l) + " has input dimension " + std::to_string(gp->D) +
-                                ", the stack " + std::to_string(h->D));
+    TB_CHECK(gp->D == s->D, std::string(who) + ": member " + std::to_string(l) + " has input dimension " + std::to_string(gp->D) +
+                                ", the stack " + std::to_string(s->D));
   }
   return 0;
 }
 
-// The EHVI chunk loop (rq.acq unused).  The candidates are staged once, on the first member's stream st; each chunk runs every
-// member's member_step on the member's own stream, then one EHVI kernel on st over all members' chunk outputs, then the
-// members' gradient assemblies and their fixed-order sum, then the argmax fold.  Events order the member streams against st
-// both ways; the host waits once, at the end.
-static int ehvi_run(tb_ehvi* h, EvalRequest& rq) {
+// The chunk loop over several members (rq.acq unused).  The candidates are staged once, on the first member's stream st;
+// each chunk runs every member's member_step on the member's own stream, then combine(mb, mc, c0, vals) on st over all
+// members' chunk outputs (it writes the values, each member's d/d(mean, var) with a gradient, and with rq.want_argmax the
+// block winners into the first member's sBlkBest / sBlkIdx), then the members' gradient assemblies and their fixed-order
+// sum, then the argmax fold.  Events order the member streams against st both ways; the host waits once, at the end.
+template <class Combine>
+static int members_run(MemberSet* h, EvalRequest& rq, Combine&& combine) {
   TB_CUDA(cudaSetDevice(h->device));
   const int L = h->L, D = h->D;
   tb_gp* g0 = h->m[0];
   cudaStream_t st = g0->stream;
   const bool grad = rq.out_grad != nullptr;
   if (rq.M == 0) return 0;
-  Engine eng[EHVI_LMAX];
+  Engine eng[MEMBERS_MAX];
   for (int l = 0; l < L; ++l) TB_TRY(select_engine(h->m[l], grad, &eng[l]));
   const ChunkPlan cp = plan_chunks(h->m.data(), eng, L, grad, rq.M);
   const int64_t chunk_cap = cp.chunk_cap;
@@ -3274,7 +3268,7 @@ static int ehvi_run(tb_ehvi* h, EvalRequest& rq) {
     const double* xc;
     TB_TRY(xin.in(c0, mc, &xc));
     TB_TRY(fan_out());
-    EhviMembers mb{};
+    ChunkMembers mb{};
     for (int l = 0; l < L; ++l) {
       tb_gp* gp = h->m[l];
       TB_TRY(member_step(gp, eng[l], xc, mc, cp.G[l], grad, &mb.G[l], &mb.McPad[l]));
@@ -3284,7 +3278,7 @@ static int ehvi_run(tb_ehvi* h, EvalRequest& rq) {
       mb.dmv[l] = grad ? gp->sMisc.as<double>() : nullptr;
       mb.variance[l] = gp->variance;
     }
-    TB_TRY(launch_ehvi(h, grad, mb, mc, c0, vals.out(c0), rq.want_argmax));
+    TB_TRY(combine(mb, mc, c0, vals.out(c0)));
     if (grad) {
       TB_TRY(fan_out());
       double* gl = h->sGradL.as<double>();
@@ -3292,7 +3286,7 @@ static int ehvi_run(tb_ehvi* h, EvalRequest& rq) {
         TB_TRY(launch_grad(h->m[l], xc, mc, gl + (size_t)l * mc * D));
         TB_TRY(join(l));
       }
-      ehvi_grad_sum_kernel<<<(unsigned)((mc * D + 255) / 256), 256, 0, st>>>(gl, L, mc * D, grads.out(c0));
+      member_grad_sum_kernel<<<(unsigned)((mc * D + 255) / 256), 256, 0, st>>>(gl, L, mc * D, grads.out(c0));
       TB_LAUNCHED();
       TB_CUDA(cudaGetLastError());
     }
@@ -3307,6 +3301,88 @@ static int ehvi_run(tb_ehvi* h, EvalRequest& rq) {
   return 0;
 }
 
+// a function over several handles as the ABI takes it: eval, and argmax when best_index is set; run(rq) runs the loop
+template <class Run>
+static int members_call(const MemberSet* h, const void* Xc, int64_t M, void* out, void* grad, void* best_value,
+                        int64_t* best_index, Run&& run) {
+  EvalRequest rq;
+  rq.M = M;
+  rq.want_argmax = best_index != nullptr;
+  DtypeBridge br(h->m[0]);
+  TB_TRY(br.in(Xc, M * h->D, &rq.Xc));
+  TB_TRY(br.out(out, M, &rq.out_vals));
+  TB_TRY(br.out(grad, M * h->D, &rq.out_grad));
+  TB_TRY(run(rq));
+  if (best_index) argmax_result(rq, h->dtype, best_value, best_index);
+  return br.finish();
+}
+
+}  // namespace tb
+
+// =================================================================================================
+// expected hypervolume improvement over a stack of L handles (ehvi.cuh)
+// =================================================================================================
+struct tb_ehvi : tb::MemberSet {  // one member per objective
+  int64_t K = 0;          // cells; 0: not set
+  tb::DevBuf dCells;      // lower [K][L] then upper [K][L]
+  int P = 0;              // HIPPO pending points (tb_ehvi_set_penalty); 0: no penalty
+  tb::DevBuf dPen;        // their means [P][L] then standard deviations [P][L]
+  std::vector<double> hPen;  // the means and variances [2][P][L] as last set, to recognise an unchanged push
+};
+
+namespace tb {
+
+template <int L>
+static void launch_ehvi_l(bool grad, const ChunkMembers& mb, const EhviPenalty& pen, const double* cells, int64_t K, int64_t mc,
+                          int64_t c0, double* vals, double* bb, int64_t* bi, cudaStream_t st) {
+  const unsigned blocks = (unsigned)((mc + 255) / 256);
+  if (pen.P > 0) {
+    if (grad)
+      ehvi_kernel<L, true, true><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+    else
+      ehvi_kernel<L, false, true><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+  } else if (grad) {
+    ehvi_kernel<L, true, false><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+  } else {
+    ehvi_kernel<L, false, false><<<blocks, 256, 0, st>>>(mb, pen, cells, K, mc, c0, vals, bb, bi);
+  }
+}
+
+static int launch_ehvi(tb_ehvi* h, bool grad, const ChunkMembers& mb, int64_t mc, int64_t c0, double* vals, bool argmax) {
+  tb_gp* g0 = h->m[0];
+  double* bb = argmax ? g0->sBlkBest.as<double>() : nullptr;
+  int64_t* bi = argmax ? g0->sBlkIdx.as<int64_t>() : nullptr;
+  const double* cells = h->dCells.as<double>();
+  const double* pd = h->P > 0 ? h->dPen.as<double>() : nullptr;
+  const EhviPenalty pen{pd, pd ? pd + (size_t)h->P * h->L : nullptr, h->P};
+  switch (h->L) {
+    case 2: launch_ehvi_l<2>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 3: launch_ehvi_l<3>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 4: launch_ehvi_l<4>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 5: launch_ehvi_l<5>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 6: launch_ehvi_l<6>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    case 7: launch_ehvi_l<7>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+    default: launch_ehvi_l<8>(grad, mb, pen, cells, h->K, mc, c0, vals, bb, bi, g0->stream); break;
+  }
+  TB_LAUNCHED();
+  TB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// what every EHVI evaluation needs of the object and its members, checked before anything is staged
+static int ehvi_check(const tb_ehvi* h, const char* who) {
+  TB_CHECK(h->K >= 1, std::string(who) + ": the partition cells are not set (tb_ehvi_set_cells)");
+  return members_check(h, who);
+}
+
+// the EHVI chunk loop: members_run with the EHVI kernel as the combining step
+static int ehvi_run(tb_ehvi* h, EvalRequest& rq) {
+  const bool grad = rq.out_grad != nullptr;
+  return members_run(h, rq, [&](const ChunkMembers& mb, int64_t mc, int64_t c0, double* vals) {
+    return launch_ehvi(h, grad, mb, mc, c0, vals, rq.want_argmax);
+  });
+}
+
 }  // namespace tb
 
 extern "C" {
@@ -3315,39 +3391,16 @@ int tb_ehvi_create(tb_ehvi** out, tb_gp* const* models, int L) {
   TB_CHECK(out && models, "tb_ehvi_create: null argument");
   TB_CHECK(L >= 2 && L <= tb::EHVI_LMAX, "tb_ehvi_create: the number of objectives must be in [2, " +
                                              std::to_string(tb::EHVI_LMAX) + "], got " + std::to_string(L));
-  for (int l = 0; l < L; ++l) {
-    TB_CHECK(models[l], "tb_ehvi_create: null model handle");
-    TB_CHECK(models[l]->have_data, "tb_ehvi_create: member " + std::to_string(l) + " has no data");
-    for (int j = 0; j < l; ++j) TB_CHECK(models[j] != models[l], "tb_ehvi_create: the same model handle appears twice");
-    TB_CHECK(models[l]->device == models[0]->device, "tb_ehvi_create: the members must be on one device");
-    TB_CHECK(models[l]->dtype == models[0]->dtype, "tb_ehvi_create: the members must have one dtype");
-    TB_CHECK(models[l]->D == models[0]->D, "tb_ehvi_create: the members must have one input dimension");
-  }
-  TB_CUDA(cudaSetDevice(models[0]->device));
-  tb_ehvi* h = new tb_ehvi();
-  h->m.assign(models, models + L);
-  h->L = L;
-  h->D = models[0]->D;
-  h->device = models[0]->device;
-  h->dtype = models[0]->dtype;
-  h->ev.assign(L, nullptr);
-  for (int l = 0; l < L; ++l) {
-    if (cudaEventCreateWithFlags(&h->ev[l], cudaEventDisableTiming) != cudaSuccess) {
-      cudaGetLastError();
-      tb_ehvi_destroy(h);
-      return tb::fail("tb_ehvi_create: cudaEventCreate failed", tb::ERR_RUNTIME);
-    }
-  }
-  *out = h;
+  std::unique_ptr<tb_ehvi> h(new tb_ehvi());
+  TB_TRY(tb::members_init(h.get(), models, L, "tb_ehvi_create"));
+  *out = h.release();
   return 0;
 }
 
 int tb_ehvi_destroy(tb_ehvi* h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
-  for (cudaEvent_t e : h->ev)
-    if (e) cudaEventDestroy(e);
-  delete h;  // frees the device buffers; the member handles are borrowed
+  delete h;  // frees the device buffers and the events; the member handles are borrowed
   return 0;
 }
 
@@ -3410,16 +3463,7 @@ int tb_ehvi_set_penalty(tb_ehvi* h, const double* pending_mean, const double* pe
 static int ehvi_call(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad, void* best_value, int64_t* best_index,
                      const char* who) {
   TB_TRY(tb::ehvi_check(h, who));
-  tb::EvalRequest rq;
-  rq.M = M;
-  rq.want_argmax = best_index != nullptr;
-  tb::DtypeBridge br(h->m[0]);
-  TB_TRY(br.in(Xc, M * h->D, &rq.Xc));
-  TB_TRY(br.out(out, M, &rq.out_vals));
-  TB_TRY(br.out(grad, M * h->D, &rq.out_grad));
-  TB_TRY(tb::ehvi_run(h, rq));
-  if (best_index) argmax_result(rq, h->dtype, best_value, best_index);
-  return br.finish();
+  return tb::members_call(h, Xc, M, out, grad, best_value, best_index, [&](tb::EvalRequest& rq) { return tb::ehvi_run(h, rq); });
 }
 
 int tb_ehvi_eval(tb_ehvi* h, const void* Xc, int64_t M, void* out, void* grad) {
@@ -3452,6 +3496,167 @@ int tb_ehvi_maximize(tb_ehvi* h, const double* lower, const double* upper, const
   };
   return tb::lbfgs_run("tb_ehvi_maximize", h->m[0]->stream, h->D, lower, upper, 1, 1, starts, P, maxcor, maxiter, maxls, gtol, ftol,
                        eval, x_out, f_out, success, nfev);
+}
+
+}  // extern "C"
+
+// =================================================================================================
+// reducers over single-query acquisitions of several handles (reduce.cuh)
+// =================================================================================================
+struct tb_reduce : tb::MemberSet {  // the distinct handles the terms use
+  int op = -1;  // tb_reduce_op; -1: the terms are not set
+  int T = 0;
+  int member[tb::REDUCE_TMAX] = {}, acq[tb::REDUCE_TMAX] = {};
+  double param[tb::REDUCE_TMAX] = {}, alpha[tb::REDUCE_TMAX] = {};  // alpha: the feasibility terms' only, else 0
+};
+
+namespace tb {
+
+static bool reduce_kind(int acq) {
+  return acq == TB_ACQ_EI || acq == TB_ACQ_LOG_EI || acq == TB_ACQ_NEG_LCB || acq == TB_ACQ_LCB || acq == TB_ACQ_PBT ||
+         acq == TB_ACQ_AEI || acq == TB_ACQ_MES || active_learning_kind(acq);
+}
+
+// what every evaluation needs of the object and its members, checked before anything is staged
+static int reduce_check(const tb_reduce* h, const char* who) {
+  TB_CHECK(h->op >= 0, std::string(who) + ": the terms are not set (tb_reduce_set_terms)");
+  TB_TRY(members_check(h, who));
+  for (int k = 0; k < h->T; ++k)
+    if (h->acq[k] == TB_ACQ_MES)
+      TB_CHECK(h->m[h->member[k]]->mesS > 0, std::string(who) + ": term " + std::to_string(k) +
+                                                 " (min-value entropy search) needs its member's min-value samples first "
+                                                 "(tb_acq_set_min_value_samples)");
+  return 0;
+}
+
+template <int OP>
+static void launch_reduce_op(bool grad, const ChunkMembers& mb, const ReduceTerms& tm, int L, int64_t mc, int64_t c0,
+                             double* vals, double* bb, int64_t* bi, cudaStream_t st) {
+  const unsigned blocks = (unsigned)((mc + 255) / 256);
+  if (grad)
+    reduce_kernel<OP, true><<<blocks, 256, 0, st>>>(mb, tm, L, mc, c0, vals, bb, bi);
+  else
+    reduce_kernel<OP, false><<<blocks, 256, 0, st>>>(mb, tm, L, mc, c0, vals, bb, bi);
+}
+
+// the chunk loop: members_run with reduce_kernel as the combining step
+static int reduce_run(tb_reduce* h, EvalRequest& rq) {
+  const bool grad = rq.out_grad != nullptr;
+  ReduceTerms tm{};
+  tm.T = h->T;
+  for (int k = 0; k < h->T; ++k) {
+    const tb_gp* gp = h->m[h->member[k]];
+    tm.member[k] = h->member[k];
+    tm.acq[k] = h->acq[k];
+    tm.param[k] = h->param[k];
+    tm.aux[k] = feasibility_kind(h->acq[k]) ? h->alpha[k] : gp->noise;
+    tm.samp[k] = h->acq[k] == TB_ACQ_MES ? gp->dMes.as<double>() : nullptr;
+    tm.nsamp[k] = h->acq[k] == TB_ACQ_MES ? gp->mesS : 0;
+  }
+  return members_run(h, rq, [&](const ChunkMembers& mb, int64_t mc, int64_t c0, double* vals) -> int {
+    tb_gp* g0 = h->m[0];
+    double* bb = rq.want_argmax ? g0->sBlkBest.as<double>() : nullptr;
+    int64_t* bi = rq.want_argmax ? g0->sBlkIdx.as<int64_t>() : nullptr;
+    if (h->op == TB_REDUCE_SUM)
+      launch_reduce_op<TB_REDUCE_SUM>(grad, mb, tm, h->L, mc, c0, vals, bb, bi, g0->stream);
+    else if (h->op == TB_REDUCE_PRODUCT)
+      launch_reduce_op<TB_REDUCE_PRODUCT>(grad, mb, tm, h->L, mc, c0, vals, bb, bi, g0->stream);
+    else
+      launch_reduce_op<TB_REDUCE_SOFTPLUS>(grad, mb, tm, h->L, mc, c0, vals, bb, bi, g0->stream);
+    TB_LAUNCHED();
+    TB_CUDA(cudaGetLastError());
+    return 0;
+  });
+}
+
+}  // namespace tb
+
+extern "C" {
+
+int tb_reduce_create(tb_reduce** out, tb_gp* const* models, int n) {
+  TB_CHECK(out && models, "tb_reduce_create: null argument");
+  TB_CHECK(n >= 1 && n <= tb::MEMBERS_MAX, "tb_reduce_create: the number of distinct models must be in [1, " +
+                                                std::to_string(tb::MEMBERS_MAX) + "], got " + std::to_string(n));
+  std::unique_ptr<tb_reduce> h(new tb_reduce());
+  TB_TRY(tb::members_init(h.get(), models, n, "tb_reduce_create"));
+  *out = h.release();
+  return 0;
+}
+
+int tb_reduce_destroy(tb_reduce* h) {
+  if (!h) return 0;
+  cudaSetDevice(h->device);
+  delete h;  // frees the device buffers and the events; the member handles are borrowed
+  return 0;
+}
+
+int tb_reduce_set_terms(tb_reduce* h, int op, int T, const int* member, const int* acq, const double* param,
+                        const double* alpha) {
+  TB_CHECK(h && member && acq && param, "tb_reduce_set_terms: null argument");
+  TB_CHECK(op == TB_REDUCE_SUM || op == TB_REDUCE_PRODUCT || op == TB_REDUCE_SOFTPLUS,
+           "tb_reduce_set_terms: unknown reduction " + std::to_string(op));
+  TB_CHECK(T >= 1 && T <= tb::REDUCE_TMAX, "tb_reduce_set_terms: the number of terms must be in [1, " +
+                                               std::to_string(tb::REDUCE_TMAX) + "], got " + std::to_string(T));
+  TB_CHECK(op != TB_REDUCE_SOFTPLUS || T == 1, "tb_reduce_set_terms: the softplus takes one term, got " + std::to_string(T));
+  double al[tb::REDUCE_TMAX] = {};
+  for (int k = 0; k < T; ++k) {
+    const std::string term = "tb_reduce_set_terms: term " + std::to_string(k);
+    TB_CHECK(member[k] >= 0 && member[k] < h->L, term + ": member index " + std::to_string(member[k]) + " is not in [0, " +
+                                                     std::to_string(h->L) + ")");
+    TB_CHECK(tb::reduce_kind(acq[k]), term + ": kind " + std::to_string(acq[k]) +
+                                          " is not one a reduction fuses (GIBBON, penalised and unknown kinds are not)");
+    if (acq[k] == TB_ACQ_LCB || acq[k] == TB_ACQ_NEG_LCB)
+      TB_CHECK(param[k] >= 0.0, term + ": Standard deviation scaling parameter beta must not be negative");
+    if (acq[k] == TB_ACQ_BALD) TB_CHECK(param[k] > 0.0, term + ": Jitter must be positive.");
+    if (tb::feasibility_kind(acq[k])) {
+      TB_CHECK(alpha, "tb_reduce_set_terms: null alpha with a feasibility term");
+      TB_CHECK(alpha[k] > 0.0 && std::isfinite(alpha[k]), term + ": alpha must be positive and finite, got " + std::to_string(alpha[k]));
+      al[k] = alpha[k];
+    }
+  }
+  h->op = op;
+  h->T = T;
+  for (int k = 0; k < T; ++k) {
+    h->member[k] = member[k];
+    h->acq[k] = acq[k];
+    h->param[k] = param[k];
+    h->alpha[k] = al[k];
+  }
+  return 0;
+}
+
+int tb_reduce_eval(tb_reduce* h, const void* Xc, int64_t M, void* out, void* grad) {
+  TB_CHECK(h && (M == 0 || (Xc && out)), "tb_reduce_eval: null argument");
+  TB_CHECK(M >= 0, "tb_reduce_eval: negative candidate count");
+  TB_TRY(tb::reduce_check(h, "tb_reduce_eval"));
+  return tb::members_call(h, Xc, M, out, grad, nullptr, nullptr, [&](tb::EvalRequest& rq) { return tb::reduce_run(h, rq); });
+}
+
+int tb_reduce_argmax(tb_reduce* h, const void* Xc, int64_t M, void* out, void* best_value, int64_t* best_index) {
+  TB_CHECK(h && Xc && best_value && best_index, "tb_reduce_argmax: null argument");
+  TB_CHECK(M > 0, "tb_reduce_argmax: argmax over an empty candidate set");
+  TB_TRY(tb::reduce_check(h, "tb_reduce_argmax"));
+  return tb::members_call(h, Xc, M, out, nullptr, best_value, best_index, [&](tb::EvalRequest& rq) { return tb::reduce_run(h, rq); });
+}
+
+int tb_reduce_maximize(tb_reduce* h, const double* lower, const double* upper, const double* starts, int64_t P, int maxcor,
+                       int maxiter, int maxls, double gtol, double ftol, double* x_out, double* f_out, int32_t* success,
+                       int64_t* nfev) {
+  TB_CHECK(h && lower && upper, "tb_reduce_maximize: null argument");
+  TB_TRY(tb::check_starts("tb_reduce_maximize", P, starts, x_out, f_out, success, nfev, maxcor, maxiter, maxls, gtol, ftol));
+  TB_TRY(tb::reduce_check(h, "tb_reduce_maximize"));
+  if (P == 0) return 0;
+  TB_CUDA(cudaSetDevice(h->device));
+  auto eval = [&](const double* xt, const int*, int n, double* vals, double* grad, const int*) -> int {
+    tb::EvalRequest rq;
+    rq.Xc = xt;
+    rq.M = n;
+    rq.out_vals = vals;
+    rq.out_grad = grad;
+    return tb::reduce_run(h, rq);
+  };
+  return tb::lbfgs_run("tb_reduce_maximize", h->m[0]->stream, h->D, lower, upper, 1, 1, starts, P, maxcor, maxiter, maxls, gtol,
+                       ftol, eval, x_out, f_out, success, nfev);
 }
 
 }  // extern "C"
